@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- frames/sec of the GeneFace++ render hot path on B200 (BASELINE.json metric).
+"""bench.py -- frames/sec of the GeneFace++ render hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]                 # this repo's sm_100a kernels
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this repo's sm_90a kernels
     python bench.py --impl reference [--gpus N] [--steps K] [--warmup W] # the reference's path on the host CPU cores
 
 One "step" = one pass of the hot path over one batch of synthetic input = rendering this rank's shard of a
-512x512 head+torso clip (BASELINE config "May head+torso two-pass 512x512, 250 frames, 1xB200"; at N GPUs every
+512x512 head+torso clip (BASELINE config "May head+torso two-pass 512x512, 250 frames, 1xH100"; at N GPUs every
 rank renders its own 250 frames -- config 4, 2000 frames over 8 GPUs -- and one NCCL all-gather of the RGB
 follows: weak scaling).  Random-init May-shaped weights, synthetic poses/conditioning (no checkpoint or dataset
 ships with the reference): "data": "synthetic".
@@ -51,6 +51,8 @@ def parse():
     ap.add_argument("--no-gpu-reference", action="store_true", help="skip timing the reference's own CUDA kernels (oracle/_ref) beside ours")
     ap.add_argument("--no-sr-variants", action="store_true", help="skip the short measurement of the SR-checkpoint paths (SURVEY 8(f) rank 3)")
     ap.add_argument("--no-train-ops", action="store_true", help="skip timing the training-side native ops beside the reference's kernels (SURVEY 8(f) rank 4)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (fixed seeded sample, < 64 MB)")
     ap.add_argument("--precision", default=os.environ.get("GFPP_BENCH_PRECISION", DEFAULT_PRECISION), choices=["fp32", "fp16", "bf16x3", "bf16", "robust"],
                     help="arithmetic of the head MLP GEMMs (marching/gather/compositing are fp32 in every mode)")
     return ap.parse_args()
@@ -60,12 +62,12 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), "measured", d
-    return 6650.0, "fallback", {}
+        return d.get("hbm_gbs", 3350.0), "measured", d
+    return 3350.0, "H100 SXM data sheet", {}
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason sampling during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle-reason sampling during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -229,6 +231,23 @@ def measure_other_mode(args, sc, model, prec, poses_dev, pose6_dev, cond_dev, bg
     return out
 
 
+def dump_outputs(d, frames, stats):
+    """The last timed step's frames as float32 (first and last frame whole + a seeded sample of 2^20 pixels) and its per-frame
+    stats (B_total, n_survivors, S, P) as float64."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    f = frames.reshape(frames.shape[0], -1, 3)
+    n = f.shape[0] * f.shape[1]
+    k = min(n, 1 << 20)
+    idx = torch.randint(0, n, (k,), generator=torch.Generator().manual_seed(1234)).sort().values   # seeded: the same pixels every run
+    sample = f.reshape(-1, 3)[idx.to(f.device)]
+    np.save(os.path.join(d, "frame_first.npy"), f[0].float().cpu().numpy())
+    np.save(os.path.join(d, "frame_last.npy"), f[-1].float().cpu().numpy())
+    np.save(os.path.join(d, "pixels_sample.npy"), sample.float().cpu().numpy())
+    np.save(os.path.join(d, "stats.npy"), stats.double().numpy())
+
+
 def workload_name(args):
     return (f"May {'head-NeRF' if args.head_only else 'head+torso two-pass'} {args.size}x{args.size}, {args.frames}-frame driving clip per GPU, "
             f"max_steps=16, T_thresh=0.01, density_scale={args.density_scale:g}")
@@ -384,8 +403,9 @@ def _main(args, out):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     sync_all()
     ev0.record()
+    last = None
     for _ in range(args.steps):
-        step_device()
+        last = step_device()
     ev1.record()
     sync_all()
     clocks = sampler.stop() if rank == 0 else {}
@@ -396,6 +416,8 @@ def _main(args, out):
     ms = tms.item()
     timed_launches = launches
     st = torch.cat(stats_acc, 0).cpu()   # [steps*T, 4]: B_total, n_survivors, S, P
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_outputs(args.dump_outputs, last, st[-T:])
     S_per_frame = st[:, 2].float().mean().item()
     P_per_frame = st[:, 3].float().mean().item()
     fps = world * T * args.steps / (ms / 1000.0)
@@ -432,10 +454,10 @@ def _main(args, out):
     # what physically moves: the fp16 / int16 'oct' layouts hold the 8 corners of a cell in ONE 32-byte sector per (sample, level),
     # the fp32 'quad' layout in two; everything is L2-resident, so the binding resources are L1/L2 sector rate and the tensor pipe
     sectors_per_sample = 2 * 16 * (1 if args.precision in ("fp16", "robust") else 2)
-    sm_hz = 1e6 * (clocks.get("sm_mhz") or 1965.0) if rank == 0 else 1.965e9
+    sm_hz = 1e6 * (clocks.get("sm_mhz") or 1980.0) if rank == 0 else 1.98e9
     n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
     sector_rate = Fc * S_per_frame * sectors_per_sample / head_t          # sectors / s
-    bf16_peak = (pk.get("bf16_tflops_sustained") or 1460.6)
+    bf16_peak = (pk.get("bf16_tflops_sustained") or 989.0)
     kname = {"fp32": "k_head (pass 1)", "bf16": "k_head_tc (pass 1)", "bf16x3": "k_head_tc (pass 1)"}.get(args.precision, "k_head_v2 (pass 1)")
     if os.environ.get("GFPP_HEAD_V1"):
         kname = "k_head_tc (pass 1)"
@@ -447,9 +469,9 @@ def _main(args, out):
                 "alg_bytes_per_frame": alg_bytes / Fc, "alg_flops_per_frame": alg_flops / Fc,
                 "gathered_bytes_per_frame": S_per_frame * sectors_per_sample * 32,
                 "l2_sector_frac": sector_rate / (1.0 * n_sm * sm_hz),
-                "l2_sector_note": "scattered 32-byte sectors per second / (1.0 sector per clock per SM: the measured ceiling, profiles/microbench_gather_r01.txt)",
+                "l2_sector_note": "scattered 32-byte sectors per second / (1.0 sector per clock per SM)",
                 "tensor_frac": alg_flops / head_t / 1e12 / bf16_peak,
-                "tensor_note": "algorithmic MLP flops per second / measured sustained dense bf16 peak (MEASURED_PEAKS.json)"}
+                "tensor_note": "algorithmic MLP flops per second / dense bf16 peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet)"}
 
     # ---------------- end to end (host buffers in, uint8 frames out) ----------------
     _stage("roofline leg done, end-to-end")
@@ -516,11 +538,11 @@ def _main(args, out):
     sr = None
     if rank == 0 and world == 1 and not args.no_sr_variants:
         # SURVEY 8(f) rank 3, measured in the same run: the SR checkpoints' clip paths (NeRF at 256x256 + torso-SR field + 256->512 SR
-        # head on tcgen05), every stage in libgfpp, beside the SR head as host-side PyTorch / cuDNN (tools/sr_bench.py)
+        # head on wgmma), every stage in libgfpp, beside the SR head as host-side PyTorch / cuDNN (tools/sr_bench.py)
         try:
             sys.path.insert(0, os.path.join(ROOT, "tools"))
             import sr_bench
-            sr = {"config": "256x256 NeRF (fp16 tcgen05) -> 512x512, 32-frame clips, resident inputs, CUDA events, median of 3", "results": sr_bench.measure(32, 3)}
+            sr = {"config": "256x256 NeRF (fp16 wgmma) -> 512x512, 32-frame clips, resident inputs, CUDA events, median of 3", "results": sr_bench.measure(32, 3)}
         except Exception as ex:   # an extra measurement must never take the bench down
             sr = {"unavailable": f"{type(ex).__name__}: {ex}"[:300]}
     train = None
@@ -537,13 +559,13 @@ def _main(args, out):
         line = {"metric": metric_name(args), "value": fps,
                 "unit": "frames/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps,
                 "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": {"fp32": "f32", "fp16": "f16 operands, f32 accumulate (tcgen05)", "bf16x3": "bf16 hi/lo split x3, f32 accumulate (tcgen05)", "bf16": "bf16 operands, f32 accumulate (tcgen05)",
-                          "robust": "f16 operands, f32 accumulate (tcgen05); hi/lo split x3 on the ambient net, 16-bit fixed-point position table"}[args.precision],
+                "dtype": {"fp32": "f32", "fp16": "f16 operands, f32 accumulate (wgmma)", "bf16x3": "bf16 hi/lo split x3, f32 accumulate (wgmma)", "bf16": "bf16 operands, f32 accumulate (wgmma)",
+                          "robust": "f16 operands, f32 accumulate (wgmma); hi/lo split x3 on the ambient net, 16-bit fixed-point position table"}[args.precision],
                 "data": "synthetic",
                 "config": {"workload": workload_name(args), "mlp_precision": args.precision, "frames_per_gpu_per_step": T, "frames_per_call": args.frames_per_call,
                            "S_valid_samples_per_frame": S_per_frame, "P_torso_pixels_per_frame": P_per_frame, "B_total": int(st[0, 0]),
                            "parallelism": f"frame-sharded x{world}, one NCCL all-gather of the uint8 clip at the end" if world > 1 else "single GPU",
-                           "l2": "per-step working set (786 MB fp32 frames out + 1.8 GB workspace) >> 126 MB L2; grid tables (14.4 MB) are L2-resident by design"},
+                           "l2": "per-step working set (786 MB fp32 frames out + 1.8 GB workspace) >> 50 MB L2; grid tables (14.4 MB) are L2-resident by design"},
                 "clocks": clocks, "e2e": {"value": e2e_fps, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                                           "note": "pinned host poses+conditioning in (H2D, pose conversion and conditioning nets inside the timed "
                                                   "region), uint8 [T,H,W,3] frames written by the epilogue kernel" +

@@ -39,7 +39,7 @@ _OFFSETS_HOST = {}
 def _offsets_host(offsets):
     """Host copy of a grid's level offsets, cached per offsets TENSOR: no D2H sync per encoder call.  The cache entry holds a
     reference to the tensor, so its device address cannot be handed to another tensor while the entry lives (a cache keyed by
-    data_ptr alone returned a previous grid's offsets when a freed buffer's address was reused -- found on the B200)."""
+    data_ptr alone returned a previous grid's offsets when a freed buffer's address was reused -- found on the GPU)."""
     key = (offsets.data_ptr(), offsets.numel(), int(offsets._version))
     hit = _OFFSETS_HOST.get(key)
     if hit is None or hit[0] is not offsets:

@@ -1,8 +1,8 @@
-"""Build libgfpp.so (hand-written sm_100a CUDA behind the C-ABI of include/gfpp.h) IN-TREE with nvcc.
+"""Build libgfpp.so (hand-written sm_90a CUDA behind the C-ABI of include/gfpp.h) IN-TREE with nvcc.
 
     python -m genefaceplusplus_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the resulting genefaceplusplus_b200/libgfpp.so travels to the GPU box.
+nvcc cross-compiles without a GPU; the resulting genefaceplusplus_b200/libgfpp.so is loaded from the package directory.
 """
 import concurrent.futures as cf
 import os
@@ -15,7 +15,7 @@ OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libgfpp.so")
 SOURCES = ["capi.cu", "ops_kernels.cu", "head_kernel.cu", "torso_kernel.cu", "tc_pack.cu", "head_tc_kernel.cu", "head_v2_kernel.cu", "sr_kernel.cu", "torso_sr_kernel.cu", "train_kernels.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 

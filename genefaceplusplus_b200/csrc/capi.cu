@@ -285,8 +285,8 @@ int gfpp_check_device(void) {
     cudaDeviceProp p;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&p, dev) != cudaSuccess)
         return fail(GFPP_ERR_CUDA, "no CUDA device%s");
-    if (p.major != 10) {
-        snprintf(g_err, sizeof(g_err), "libgfpp is built for sm_100a only; device is sm_%d%d", p.major, p.minor);
+    if (p.major != 9 || p.minor != 0) {
+        snprintf(g_err, sizeof(g_err), "libgfpp is built for sm_90a only; device is sm_%d%d", p.major, p.minor);
         return GFPP_ERR_UNSUPPORTED;
     }
     return GFPP_OK;
@@ -363,7 +363,7 @@ int gfpp_tc_selftest(const float *A, const float *W, uint32_t N, uint32_t K, int
                      float *out, void *stream) {
     if (!A || !W || !scratch || !out) return fail(GFPP_ERR_INVALID, "tc_selftest: null pointer%s");
     const int k64 = (int)K - (k16_tail ? 16 : 0);
-    if (N % 16 || N < 16 || N > 144 || k64 <= 0 || k64 % 16 || K > 144 || precision < 1 || precision > 3)
+    if ((N != 16 && N != 128 && N != 144) || k64 <= 0 || k64 % 16 || K > 144 || precision < 1 || precision > 3)
         return fail(GFPP_ERR_INVALID, "tc_selftest: unsupported shape%s");
     const int nt64 = (k64 + 63) / 64;
     cudaStream_t st = (cudaStream_t)stream;
@@ -779,7 +779,7 @@ int gfpp_sr_pack(const gfpp_sr_desc *d, void *packed, size_t packed_bytes, gfpp_
     CKN(cudaMemcpyAsync(base + L.rgb_w[1], d->rgb_w[1], 3 * 64 * 4, cudaMemcpyDeviceToDevice, st));
     CKN(cudaMemcpyAsync(base + L.rgb_b[0], d->rgb_b[0], 12, cudaMemcpyDeviceToDevice, st));
     CKN(cudaMemcpyAsync(base + L.rgb_b[1], d->rgb_b[1], 12, cudaMemcpyDeviceToDevice, st));
-    // GEMM matrices [N_total][9 * C_in] -> fp16 UMMA K-major SW128 tiles in the kernels' streaming order:
+    // GEMM matrices [N_total][9 * C_in] -> fp16 GMMA K-major SW128 tiles in the kernels' streaming order:
     // chunk c covers k in [64c, 64c + 64) (tap c / CB, channel block c % CB); inside a chunk one tile per N-block
     const float *mat[3] = {d->conv0_w, d->up_w, d->conv1_w};
     for (int l = 0; l < 3; ++l) {

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers of libgfpp (sm_100a).
+// common.cuh -- shared device helpers of libgfpp (sm_90a).
 //
 // The ray-march helpers make DISCRETE decisions (cell index, occupancy bit, "t < far"), so their fp32
 // arithmetic is written with explicit round-to-nearest intrinsics (no FMA contraction) in exactly the
@@ -306,7 +306,8 @@ __device__ __forceinline__ float2 grid_lookup3(const GridMeta &gm, const float2 
 // re-laid out at pack time as 32-byte blocks  Q[i] = { T[i], T[i+1], T[i+m1], T[i+m1+1] }  (indices mod the level size):
 // one 32-byte sector per (cell, z-plane) instead of four scattered 8-byte entries.  The gather is bound by the number of
 // outstanding L1 misses x L2 latency; this cuts sectors per (sample, level) from ~4-8 to 2 and LDG instructions from 8 to 4.
-// Costs 4x table memory (2 x 29 MB for the May head), which still sits in the 126 MB L2.  Values and arithmetic are
+// Costs 4x table memory (2 x 28.8 MB for the May head: more than the H100's 50 MB L2, yet still faster there than the
+// reference layout, DESIGN.md section 4).  Values and arithmetic are
 // unchanged, so results are bit-identical to the unpacked path.
 __device__ __forceinline__ uint32_t grid_mod(const GridMeta &gm, int l, uint32_t idx) {
     const uint32_t hm = gm.hmask[l];
@@ -315,20 +316,15 @@ __device__ __forceinline__ uint32_t grid_mod(const GridMeta &gm, int l, uint32_t
     return idx >= hs ? idx % hs : idx;
 }
 
-// one 256-bit read-only global load (sm_100: LDG.E.256); p must be 32-byte aligned.  (The .v4.u64 form: ptxas 12.9 crashes on
-// .v8.u32 in this translation unit.)
+// one 32-byte read-only global load as two 16-byte loads of the same sector (Hopper has no 256-bit load); p must be 32-byte aligned
 __device__ __forceinline__ void ldg256(const uint4 *p, uint4 &lo, uint4 &hi) {
-    unsigned long long a, b, c2, d;
-    asm volatile("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c2), "=l"(d) : "l"(p));
-    lo.x = (uint32_t)a; lo.y = (uint32_t)(a >> 32); lo.z = (uint32_t)b; lo.w = (uint32_t)(b >> 32);
-    hi.x = (uint32_t)c2; hi.y = (uint32_t)(c2 >> 32); hi.z = (uint32_t)d; hi.w = (uint32_t)(d >> 32);
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w) : "l"(p));
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(hi.x), "=r"(hi.y), "=r"(hi.z), "=r"(hi.w) : "l"(p + 1));
 }
 // same, streaming past L1 (no line allocated): the fp16 oct gathers of the 2-CTA kernel, which leaves L1 only ~28 KB
 __device__ __forceinline__ void ldg256_na(const uint4 *p, uint4 &lo, uint4 &hi) {
-    unsigned long long a, b, c2, d;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c2), "=l"(d) : "l"(p));
-    lo.x = (uint32_t)a; lo.y = (uint32_t)(a >> 32); lo.z = (uint32_t)b; lo.w = (uint32_t)(b >> 32);
-    hi.x = (uint32_t)c2; hi.y = (uint32_t)(c2 >> 32); hi.z = (uint32_t)d; hi.w = (uint32_t)(d >> 32);
+    asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w) : "l"(p));
+    asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(hi.x), "=r"(hi.y), "=r"(hi.z), "=r"(hi.w) : "l"(p + 1));
 }
 __device__ __forceinline__ float2 grid_lookup3q(const GridMeta &gm, const float4 *__restrict__ quads, int l, float u, float v, float w) {
     if (u < 0.f || u > 1.f || v < 0.f || v > 1.f || w < 0.f || w > 1.f) return make_float2(0.f, 0.f);

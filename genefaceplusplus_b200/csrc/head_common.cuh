@@ -1,5 +1,5 @@
 // head_common.cuh -- ray-slot state and helpers shared by the two fused head kernels
-// (head_kernel.cu: fp32 FFMA MLP; head_tc_kernel.cu: tcgen05 tensor-core MLP).
+// (head_kernel.cu: fp32 FFMA MLP; head_tc_kernel.cu: wgmma tensor-core MLP).
 #pragma once
 #include <cooperative_groups.h>
 

@@ -88,9 +88,7 @@ struct HeadV2Args {
     const unsigned char *cond_hi;    // [F,64] fp16: the frame's conditioning vector, pre-rounded (k_cond_images)
     const unsigned char *cond_lo;    // [F,64] fp16 residuals (robust mode)
     const float *pos_step;           // [16] per-level step of the 16-bit fixed-point position table (robust mode) or nullptr
-    unsigned flags;                  // set by launch_head_v2: bit 0 = serve the slots of a layer in arrival order
 };
-constexpr unsigned V2_DEFAULT_FLAGS = 0u;
 cudaError_t launch_head_v2(const HeadArgs &a, const HeadV2Args &t, int precision, cudaStream_t st);
 cudaError_t launch_cond_images(const float *cond_feat, int n_frames, void *cond_hi, void *cond_lo, cudaStream_t st);
 size_t head_v2_smem_bytes(bool robust);

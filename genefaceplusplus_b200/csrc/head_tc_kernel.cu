@@ -1,14 +1,14 @@
-// head_tc_kernel.cu -- fused persistent head renderer, tensor-core variant (tcgen05 + TMEM + TMA bulk copies).
+// head_tc_kernel.cu -- fused persistent head renderer, tensor-core variant (wgmma + TMA bulk copies).
 //
 // Same ray-slot machinery, marching, gather and compositing as head_kernel.cu; only the dense tiny-MLP GEMMs differ:
-// every 128-row batch runs its eight layers as tcgen05.mma (kind::f16, M=128, N in {128,144,16}) with
-//   * A (activations) written by the CTA's threads straight into UMMA K-major SW128 tiles in shared memory
+// every 128-row batch runs its eight layers as wgmma.mma_async (16-bit operands, fp32 accumulate, N in {128,144}), the
+// two warpgroups of the CTA taking rows 0-63 and 64-127, with
+//   * A (activations) written by the CTA's threads straight into GMMA K-major SW128 tiles in shared memory
 //     (gathered grid features, conditioning, previous layer's epilogue), 16-bit, optionally hi/lo split;
 //   * W streamed as pre-swizzled 16-bit tiles through a 3-stage ring with cp.async.bulk + mbarrier;
-//   * D (fp32 accumulators) in TMEM, read back with tcgen05.ld by all 256 threads (2 threads per row) for the
-//     ReLU / tanh / exp / sigmoid epilogues;
-//   * position-grid features parked in 32 spare TMEM columns between the ambient and sigma nets.
-// One thread issues all MMAs; completion is signalled with tcgen05.commit on an mbarrier.
+//   * D (fp32 accumulators) in registers, consumed in the accumulator fragment layout by the ReLU / tanh / exp /
+//     sigmoid epilogues;
+//   * position-grid features parked in registers (their 16-bit operand chunks) between the ambient and sigma nets.
 //
 // Precision modes (tc::Precision): FP16_X1 (what the reference itself runs under autocast, fp32 accumulate),
 // BF16_X1, BF16_X3 (hi/lo split, 3 MMAs per k-step: ~16 mantissa bits).  See DESIGN.md "precision".
@@ -35,8 +35,6 @@ constexpr int A_TILE = 16384;        // 128 rows x 64 k x 2 B (SW128)
 constexpr int A_K16 = 4096;          // 128 rows x 16 k x 2 B (no swizzle)
 constexpr int W_HALF = 18432;        // up to 144 rows x 64 k x 2 B
 constexpr int W_NSTAGE = 3;
-constexpr uint32_t TMEM_COLS = 256;
-constexpr uint32_t TMEM_P = 160;     // 32 columns of parked position features
 
 // the lo (split) operand images exist only in the bf16x3 instantiation; the single-pass kernels stay under 113 KB of
 // shared memory and 128 registers so that TWO CTAs are resident per SM (their barrier / latency stalls overlap)
@@ -51,7 +49,7 @@ struct SmemTC {
     alignas(SPLIT ? 256 : 16) unsigned char s_lo[SPLIT ? A_K16 : 16];
     float bias[128];                  // color L0 bias (individual code folded)
     float nw[6 * 128];                // fp32 rows of the two 3-wide output layers: ambient out (0-2), color out (3-5)
-    float part[2 * 3 * TM];           // their partial dot products, one per column half
+    float part[3 * TM];               // their dot products
     float sx[TM], sy[TM], sz[TM];
     float amb[3 * TM];
     float sig[TM];
@@ -59,8 +57,6 @@ struct SmemTC {
     int frame[TM];
     int valid[TM];
     unsigned long long bar_full[W_NSTAGE];
-    unsigned long long bar_acc;
-    uint32_t tmem_base;
     uint32_t coarse[HEAD_COARSE_WORDS];
     uint4 lvl[2][2 * GFPP_MAX_LEVELS];   // per-level grid metadata (position, ambient) for lookup8o
     int next, end, done;
@@ -68,9 +64,6 @@ struct SmemTC {
 
 // The weight stream is static: batch b consumes tiles b*12 + (0..11) in the order of kHeadTcChunks, and 12 is a multiple
 // of the ring depth, so tile id c always lives in stage c % W_NSTAGE and completes the mbarrier phase (c / W_NSTAGE) & 1.
-// Everything the issuing warp needs is therefore a compile-time constant or a CTA-uniform address: the MMA / bulk-copy
-// operands sit in uniform registers and one elected lane of warp 0 issues them back to back.  (A lone `tid == 0` branch
-// makes the compiler wrap every tcgen05.mma in a register->uniform-register waterfall loop: ~250 cycles per MMA.)
 static_assert(HEAD_TC_NCHUNK % W_NSTAGE == 0, "the static stage/parity schedule needs the ring depth to divide the tiles per batch");
 
 template <bool SPLIT, int ID>
@@ -89,108 +82,88 @@ __device__ __forceinline__ void issue_loads(const HeadTcArgs &t, SmemTC<SPLIT> &
     }
 }
 
-template <bool SPLIT, int ID, bool ACC0>
-__device__ __forceinline__ void issue_tile_mmas(SmemTC<SPLIT> &s, int a_tile, uint32_t d_tmem, uint32_t idesc) {
+// the MMAs of tile ID against A tile `a_tile` (the K16 SH tile for the k16 chunk), rows of warpgroup `wg`
+template <bool BF16, bool SPLIT, int ID, bool ACC0, int N>
+__device__ __forceinline__ void mma_tile(SmemTC<SPLIT> &s, int a_tile, int wg, float (&d)[N / 2]) {
     constexpr int stage = ID % W_NSTAGE, ksteps = head_tc_chunk_ksteps(ID);
     constexpr bool k16 = kHeadTcChunks[ID].k16 != 0;
-    const uint32_t ah = k16 ? smem_u32(s.s_hi) : smem_u32(s.a_hi[a_tile]);
-    const uint32_t al = k16 ? smem_u32(s.s_lo) : smem_u32(s.a_lo[SPLIT ? a_tile : 0]);
+    const uint32_t half = (uint32_t)wg * (k16 ? K16_HALF : SW128_HALF);
+    const uint32_t ah = (k16 ? smem_u32(s.s_hi) : smem_u32(s.a_hi[a_tile])) + half;
+    const uint32_t al = (k16 ? smem_u32(s.s_lo) : smem_u32(s.a_lo[SPLIT ? a_tile : 0])) + half;
     const uint32_t wh = smem_u32(s.w_hi[stage]), wl = smem_u32(s.w_lo[SPLIT ? stage : 0]);
 #pragma unroll
     for (int k = 0; k < ksteps; ++k) {
         const uint32_t adv = (uint32_t)k * 32u;   // 16 elements x 2 B inside the 128-byte swizzle row
         const uint64_t dah = k16 ? desc_k16(ah) : desc_sw128(ah + adv), dwh = k16 ? desc_k16(wh) : desc_sw128(wh + adv);
+        const uint32_t acc0 = (ACC0 || k > 0) ? 1u : 0u;
         if (SPLIT) {
             const uint64_t dal = k16 ? desc_k16(al) : desc_sw128(al + adv), dwl = k16 ? desc_k16(wl) : desc_sw128(wl + adv);
-            if (ACC0 || k > 0) mma_f16_s<true>(d_tmem, dal, dwh, idesc);   // small terms first
-            else mma_f16_s<false>(d_tmem, dal, dwh, idesc);
-            mma_f16_s<true>(d_tmem, dah, dwl, idesc);
-            mma_f16_s<true>(d_tmem, dah, dwh, idesc);
+            wgmma<N, BF16>(d, dal, dwh, acc0);   // small terms first
+            wgmma<N, BF16>(d, dah, dwl, 1u);
+            wgmma<N, BF16>(d, dah, dwh, 1u);
         } else {
-            if (ACC0 || k > 0) mma_f16_s<true>(d_tmem, dah, dwh, idesc);
-            else mma_f16_s<false>(d_tmem, dah, dwh, idesc);
+            wgmma<N, BF16>(d, dah, dwh, acc0);
         }
     }
 }
-template <bool SPLIT, int ID, int C, int NCH>
-__device__ __forceinline__ void issue_tiles(SmemTC<SPLIT> &s, uint32_t d_tmem, uint32_t idesc) {
+template <bool BF16, bool SPLIT, int ID, int C, int NCH, int N>
+__device__ __forceinline__ void mma_tiles(SmemTC<SPLIT> &s, int wg, float (&d)[N / 2]) {
     if constexpr (C < NCH) {
-        constexpr int stage = ID % W_NSTAGE;
-        mbar_wait(&s.bar_full[stage], (ID / W_NSTAGE) & 1);
-        fence_after_sync();
-        if (elect_one()) issue_tile_mmas<SPLIT, ID, (C > 0)>(s, C, d_tmem, idesc);
-        __syncwarp();
-        issue_tiles<SPLIT, ID + 1, C + 1, NCH>(s, d_tmem, idesc);
+        mma_tile<BF16, SPLIT, ID, (C > 0), N>(s, C, wg, d);
+        mma_tiles<BF16, SPLIT, ID + 1, C + 1, NCH, N>(s, wg, d);
     }
 }
 
-// Warp 0 (all lanes, converged): issue one layer = tiles ID0 .. ID0+NCH-1 against A tiles 0,1,.. (the K16 SH tile for the
-// k16 chunk), then commit to the accumulator barrier.
-template <bool SPLIT, int ID0, int NCH>
-__device__ __forceinline__ void issue_layer(SmemTC<SPLIT> &s, uint32_t d_tmem, uint32_t idesc) {
-    fence_after_sync();
-    issue_tiles<SPLIT, ID0, 0, NCH>(s, d_tmem, idesc);
-    if (elect_one()) mma_commit(&s.bar_acc);
-    __syncwarp();
-}
-
-// All threads: wait for the accumulator; warp 0 then refills the weight stages the layer has released.
-template <bool SPLIT, int ID0, int NCH>
-__device__ __forceinline__ void wait_acc(const HeadTcArgs &t, SmemTC<SPLIT> &s, uint32_t &acc_uses, int warp) {
-    mbar_wait(&s.bar_acc, acc_uses & 1);
-    acc_uses += 1;
-    fence_after_sync();
+// One layer = tiles ID0 .. ID0+NCH-1 against A tiles 0,1,.. for the 64 rows of the calling warpgroup; returns with the
+// accumulators complete.  Then (CTA barrier: both warpgroups are done with the weight stages) warp 0 refills the stages.
+template <bool BF16, bool SPLIT, int ID0, int NCH, int N>
+__device__ __forceinline__ void mma_layer(const HeadTcArgs &t, SmemTC<SPLIT> &s, int wg, int warp, float (&d)[N / 2]) {
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) mbar_wait(&s.bar_full[(ID0 + c) % W_NSTAGE], ((ID0 + c) / W_NSTAGE) & 1);
+    wg_fence();
+    mma_tiles<BF16, SPLIT, ID0, 0, NCH, N>(s, wg, d);
+    wg_commit();
+    wg_wait<0>();
+    acc_fence(d);
+    __syncthreads();
     if (warp == 0) {
         if (elect_one()) issue_loads<SPLIT, ID0 + W_NSTAGE, NCH>(t, s);
         __syncwarp();
     }
 }
 
-// Epilogue of a 128-wide layer: thread (row, half) reads 64 accumulator columns (two passes of 32), applies bias/ReLU and
-//   * NARROW == false: writes them as the next layer's A operand (k = column) into tile `half`;
-//   * NARROW == true : the layer feeds only a 3-wide output layer (ambient coordinates / rgb), so the activations never go
-//     back to shared memory: the thread accumulates its half of the three dot products in fp32 (weights `nw`, [3][128])
-//     and stores the partials in part[half][o][row] -- no fp16 round trip, no extra MMA, no extra barrier.
-// Not inlined: it is called six times per batch and the kernel must stay instruction-cache friendly.
-template <bool BF16, bool SPLIT, bool RELU, bool BIAS, bool NARROW>
-__device__ __noinline__ void epilogue_wide(unsigned char *a_hi, unsigned char *a_lo, uint32_t tmem, int tid, const float *bias,
-                                           const float *nw, float *part) {
-    const int row = tid & 127, half = tid >> 7;
-    const uint32_t lane_base = (uint32_t)((tid >> 5) & 3) * 32u;
-    const uint32_t taddr = tmem + (lane_base << 16) + (uint32_t)half * 64u;
-    unsigned char *hi = a_hi + half * A_TILE, *lo = a_lo + (SPLIT ? half * A_TILE : 0);
-    float d0 = 0.f, d1 = 0.f, d2 = 0.f;
-#pragma unroll 1
-    for (int p = 0; p < 2; ++p) {
-        float v[2][16];
-        tmem_ld16(taddr + p * 32, v[0]);
-        tmem_ld16(taddr + p * 32 + 16, v[1]);
-        wait_ld();
+// Epilogue of a 128-wide layer from the accumulator fragment (columns 0..127 of d): bias/ReLU, then either the next layer's
+// A operand (tiles 0 and 1) or, NARROW, the fp32 dot products of a 3-wide output layer (weights `nw` [3][128]) reduced over
+// the four lanes of a row into part[o][row].
+template <bool BF16, bool SPLIT, bool RELU, bool BIAS, bool NARROW, int R>
+__device__ __forceinline__ void epilogue_wide(unsigned char *a_hi, unsigned char *a_lo, const float (&d)[R], int tid, const float *bias,
+                                              const float *nw, float *part) {
+    const int lane = tid & 31, wwarp = (tid >> 5) & 3, wg = tid >> 7;
+    float dot[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
+    for (int i = 0; i < 64; i += 2) {
+        const int h = (i >> 1) & 1, row = 64 * wg + frag_row(i, lane, wwarp), col = frag_col(i, lane);
+        float x0 = d[i], x1 = d[i + 1];
+        if (BIAS) { x0 += bias[col]; x1 += bias[col + 1]; }
+        if (RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        if (NARROW) {
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int col = half * 64 + p * 32 + q * 16 + i;
-                float x = v[q][i];
-                if (BIAS) x += bias[col];
-                if (RELU) x = fmaxf(x, 0.f);
-                v[q][i] = x;
-                if (NARROW) {
-                    d0 = fmaf(x, nw[col], d0);
-                    d1 = fmaf(x, nw[128 + col], d1);
-                    d2 = fmaf(x, nw[256 + col], d2);
-                }
-            }
-            if (!NARROW) {
-                store_chunk<BF16, SPLIT>(hi, lo, sw128_off(row, 4 * p + 2 * q), &v[q][0]);
-                store_chunk<BF16, SPLIT>(hi, lo, sw128_off(row, 4 * p + 2 * q + 1), &v[q][8]);
-            }
+            for (int o = 0; o < 3; ++o) dot[h][o] = fmaf(x1, nw[o * 128 + col + 1], fmaf(x0, nw[o * 128 + col], dot[h][o]));
+        } else {
+            store_pair<BF16, SPLIT>(a_hi + (col >> 6) * A_TILE, a_lo + (SPLIT ? (col >> 6) * A_TILE : 0), row, col & 63, x0, x1);
         }
     }
     if (NARROW) {
-        part[(half * 3 + 0) * TM + row] = d0;
-        part[(half * 3 + 1) * TM + row] = d1;
-        part[(half * 3 + 2) * TM + row] = d2;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int o = 0; o < 3; ++o) {
+                float v = dot[h][o];
+                v += __shfl_xor_sync(0xffffffffu, v, 1);
+                v += __shfl_xor_sync(0xffffffffu, v, 2);
+                if ((lane & 3) == 0) part[o * TM + 64 * wg + 16 * wwarp + (lane >> 2) + 8 * h] = v;
+            }
+        }
     }
 }
 
@@ -220,17 +193,15 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
     extern __shared__ __align__(1024) unsigned char smem_raw_[];
     unsigned char *smem_raw = smem_raw_ + ((1024u - (smem_u32(smem_raw_) & 1023u)) & 1023u);
     SmemTC<SPLIT> &s = *reinterpret_cast<SmemTC<SPLIT> *>(smem_raw);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, wg = tid >> 7, lane = tid & 31;
 
     // ---- one-time setup ----
     MarchConst mc = a.mc;
     float occ_lo[3] = {0.f, 0.f, 0.f}, occ_hi[3] = {0.f, 0.f, 0.f};
     const bool have_box = setup_occupancy(a, mc, occ_lo, occ_hi);
     install_coarse(a, s, mc, tid, NT);
-    if (warp == 0) tmem_alloc(&s.tmem_base, TMEM_COLS);
     if (tid == 32) {
         for (int i = 0; i < W_NSTAGE; ++i) mbar_init(&s.bar_full[i], 1);
-        mbar_init(&s.bar_acc, 1);
         mbar_fence_init();
         s.next = 0; s.end = 0; s.done = 0;
     }
@@ -242,17 +213,11 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
     stage_level_meta(a.pos_gm, nullptr, s.lvl[0], tid);
     stage_level_meta(a.amb_gm, nullptr, s.lvl[1], tid);
     fence_async_smem();
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tmem = s.tmem_base;
     if (warp == 0) {
         if (elect_one()) issue_loads<SPLIT, 0, W_NSTAGE>(t, s);
         __syncwarp();
     }
-    uint32_t acc_uses = 0;   // completed accumulator hand-offs (uniform across the CTA)
-    const uint32_t idesc128 = make_idesc(BF16 ? 1 : 0, 128), idesc144 = make_idesc(BF16 ? 1 : 0, 144);
-    const uint32_t lane_base = (uint32_t)(warp & 3) * 32u;
 
     const int total = (a.pass == 1) ? *a.n_hits : *a.n_survivors;
     Slot sl;
@@ -275,7 +240,8 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
 
         const int slot = tid & (TM - 1), lg = tid >> 7;
         const bool v = s.valid[slot] != 0;
-        // ---- position grid -> A tile0 k[0,32) and TMEM park; conditioning -> tile0 k[32,64), tile1 k[0,32) ----
+        uint4 park_h[2], park_l[2];   // this thread's two position-feature operand chunks, parked across the ambient net
+        // ---- position grid -> A tile0 k[0,32) and the park; conditioning -> tile0 k[32,64), tile1 k[0,32) ----
         {
             float u = 0.f, vv = 0.f, w = 0.f;
             if (v) {
@@ -293,7 +259,6 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
                 }
                 store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 2 * lg), &f[0]);
                 store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 2 * lg + 1), &f[8]);
-                tmem_st16(tmem + (lane_base << 16) + TMEM_P + (uint32_t)(lg * 16), f);
             } else {
 #pragma unroll 1
                 for (int c = 0; c < 2; ++c) {
@@ -304,8 +269,12 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
                         for (int i = 0; i < 8; ++i) f[i] = 0.f;
                     }
                     store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 2 * lg + c), f);
-                    tmem_st8(tmem + (lane_base << 16) + TMEM_P + (uint32_t)(lg * 16 + c * 8), f);
                 }
+            }
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                park_h[c] = *reinterpret_cast<const uint4 *>(s.a_hi[0] + sw128_off(slot, 2 * lg + c));
+                if (SPLIT) park_l[c] = *reinterpret_cast<const uint4 *>(s.a_lo[0] + sw128_off(slot, 2 * lg + c));
             }
             // cond values [lg*32, lg*32+32) sit at k = 32 + lg*32 + i: lg 0 -> tile0 chunks 4..7, lg 1 -> tile1 chunks 0..3
             const float4 *cf = reinterpret_cast<const float4 *>(a.cond_feat + (size_t)s.frame[slot] * 64 + lg * 32);
@@ -321,33 +290,33 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
                 }
                 store_chunk<BF16, SPLIT>(s.a_hi[lg], s.a_lo[SPLIT ? lg : 0], sw128_off(slot, (lg == 0 ? 4 : 0) + j), c8);
             }
-            wait_st();
         }
         fence_async_smem();
-        fence_before_sync();
         __syncthreads();
         PH(1)   // position gather + cond + park
 
         // ---- ambient net 96 -> 128 -> 128 -> 3 ----
-        if (warp == 0) issue_layer<SPLIT, 0, 2>(s, tmem, idesc128);
-        wait_acc<SPLIT, 0, 2>(t, s, acc_uses, warp);
-        PH(2)   // MMA issue + wait (ambient L0)
-        epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], tmem, tid, nullptr, nullptr, nullptr);
-        fence_async_smem(); fence_before_sync(); __syncthreads();
+        {
+            float d[64];
+            mma_layer<BF16, SPLIT, 0, 2, 128>(t, s, wg, warp, d);
+            PH(2)   // MMA issue + wait (ambient L0)
+            epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], d, tid, nullptr, nullptr, nullptr);
+        }
+        fence_async_smem(); __syncthreads();
         PH(3)   // epilogue (ambient L0) + barrier
-        if (warp == 0) issue_layer<SPLIT, 2, 2>(s, tmem, idesc128);
-        wait_acc<SPLIT, 2, 2>(t, s, acc_uses, warp);
-        PH(4)   // MMA (ambient L1)
-        // ambient L1 epilogue fused with the 3-wide ambient output layer (fp32 dot products straight from the accumulators)
-        epilogue_wide<BF16, SPLIT, true, false, true>(&s.a_hi[0][0], &s.a_lo[0][0], tmem, tid, nullptr, s.nw, s.part);
-        fence_before_sync();
+        {
+            float d[64];
+            mma_layer<BF16, SPLIT, 2, 2, 128>(t, s, wg, warp, d);
+            PH(4)   // MMA (ambient L1)
+            // ambient L1 epilogue fused with the 3-wide ambient output layer (fp32 dot products straight from the accumulators)
+            epilogue_wide<BF16, SPLIT, true, false, true>(&s.a_hi[0][0], &s.a_lo[0][0], d, tid, nullptr, s.nw, s.part);
+        }
         __syncthreads();
-        fence_after_sync();
-        PH(5)   // epilogue (ambient L1) + partial dots
+        PH(5)   // epilogue (ambient L1) + dots
         if (tid < TM) {
-            s.amb[tid] = tanhf(s.part[0 * TM + tid] + s.part[3 * TM + tid]);
-            s.amb[TM + tid] = tanhf(s.part[1 * TM + tid] + s.part[4 * TM + tid]);
-            s.amb[2 * TM + tid] = tanhf(s.part[2 * TM + tid] + s.part[5 * TM + tid]);
+            s.amb[tid] = tanhf(s.part[0 * TM + tid]);
+            s.amb[TM + tid] = tanhf(s.part[1 * TM + tid]);
+            s.amb[2 * TM + tid] = tanhf(s.part[2 * TM + tid]);
         }
         __syncthreads();
         PH(6)   // narrow ambient out: MMA + tanh
@@ -359,12 +328,10 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
                 vv = __fdiv_rn(__fadd_rn(s.amb[TM + slot], 1.0f), 2.0f);
                 w = __fdiv_rn(__fadd_rn(s.amb[2 * TM + slot], 1.0f), 2.0f);
             }
-            {   // parked position features back into tile 0, k[0,32)
-                float p16[16];
-                tmem_ld16(tmem + (lane_base << 16) + TMEM_P + (uint32_t)(lg * 16), p16);
-                wait_ld();
-                store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 2 * lg), &p16[0]);
-                store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 2 * lg + 1), &p16[8]);
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {   // parked position features back into tile 0, k[0,32)
+                *reinterpret_cast<uint4 *>(s.a_hi[0] + sw128_off(slot, 2 * lg + c)) = park_h[c];
+                if (SPLIT) *reinterpret_cast<uint4 *>(s.a_lo[0] + sw128_off(slot, 2 * lg + c)) = park_l[c];
             }
             if (a.amb_octs) {
                 float f[16];
@@ -388,26 +355,33 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
                 }
             }
         }
-        fence_async_smem(); fence_before_sync(); __syncthreads();
+        fence_async_smem(); __syncthreads();
         PH(7)   // ambient gather + unpark
 
         // ---- sigma net 64 -> 128 -> 128 -> (128 geo + sigma) ----
-        if (warp == 0) issue_layer<SPLIT, 4, 1>(s, tmem, idesc128);
-        wait_acc<SPLIT, 4, 1>(t, s, acc_uses, warp);
-        epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], tmem, tid, nullptr, nullptr, nullptr);
-        fence_async_smem(); fence_before_sync(); __syncthreads();
-        if (warp == 0) issue_layer<SPLIT, 5, 2>(s, tmem, idesc128);
-        wait_acc<SPLIT, 5, 2>(t, s, acc_uses, warp);
-        epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], tmem, tid, nullptr, nullptr, nullptr);
-        fence_async_smem(); fence_before_sync(); __syncthreads();
-        if (warp == 0) issue_layer<SPLIT, 7, 2>(s, tmem, idesc144);
-        wait_acc<SPLIT, 7, 2>(t, s, acc_uses, warp);
-        if (tid < TM) {   // column 128 = sigma logit (weight row 0 was packed last); sigma = density_scale * exp(h)
-            float o[16];
-            tmem_ld16(tmem + (lane_base << 16) + 128u, o);
-            wait_ld();
-            s.sig[tid] = a.density_scale * expf(o[0]);
-            // SH(dir) -> K16 tile
+        {
+            float d[64];
+            mma_layer<BF16, SPLIT, 4, 1, 128>(t, s, wg, warp, d);
+            epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], d, tid, nullptr, nullptr, nullptr);
+        }
+        fence_async_smem(); __syncthreads();
+        {
+            float d[64];
+            mma_layer<BF16, SPLIT, 5, 2, 128>(t, s, wg, warp, d);
+            epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], d, tid, nullptr, nullptr, nullptr);
+        }
+        fence_async_smem(); __syncthreads();
+        {
+            float d[72];
+            mma_layer<BF16, SPLIT, 7, 2, 144>(t, s, wg, warp, d);
+            if ((lane & 3) == 0) {   // column 128 = sigma logit (weight row 0 was packed last); sigma = density_scale * exp(h)
+                const int r = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+                s.sig[r] = a.density_scale * expf(d[64]);
+                s.sig[r + 8] = a.density_scale * expf(d[66]);
+            }
+            epilogue_wide<BF16, SPLIT, false, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], d, tid, nullptr, nullptr, nullptr);   // geo features -> tiles 0,1 (k = 0..127)
+        }
+        if (tid < TM) {   // SH(dir) -> K16 tile
             float sh[16];
             sh4(sl.g.dx, sl.g.dy, sl.g.dz, sh);
             if (!sl.active) {
@@ -417,22 +391,21 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
             store_chunk<BF16, SPLIT>(s.s_hi, s.s_lo, k16_off(tid, 0), &sh[0]);
             store_chunk<BF16, SPLIT>(s.s_hi, s.s_lo, k16_off(tid, 1), &sh[8]);
         }
-        epilogue_wide<BF16, SPLIT, false, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], tmem, tid, nullptr, nullptr, nullptr);   // geo features -> tiles 0,1 (k = 0..127)
-        fence_async_smem(); fence_before_sync(); __syncthreads();
+        fence_async_smem(); __syncthreads();
 
         PH(8)   // sigma net: 3 MMA layers + 3 epilogues
         // ---- color net (128 geo + 16 SH [+ folded individual code]) -> 128 -> 3 ----
-        if (warp == 0) issue_layer<SPLIT, 9, 3>(s, tmem, idesc128);
-        wait_acc<SPLIT, 9, 3>(t, s, acc_uses, warp);
-        // color L0 epilogue fused with the 3-wide rgb output layer
-        epilogue_wide<BF16, SPLIT, true, true, true>(&s.a_hi[0][0], &s.a_lo[0][0], tmem, tid, s.bias, s.nw + 3 * 128, s.part);
-        fence_before_sync();
+        {
+            float d[64];
+            mma_layer<BF16, SPLIT, 9, 3, 128>(t, s, wg, warp, d);
+            // color L0 epilogue fused with the 3-wide rgb output layer
+            epilogue_wide<BF16, SPLIT, true, true, true>(&s.a_hi[0][0], &s.a_lo[0][0], d, tid, s.bias, s.nw + 3 * 128, s.part);
+        }
         __syncthreads();
-        fence_after_sync();
         if (tid < TM) {
-            s.rgb[tid] = 1.0f / (1.0f + expf(-(s.part[0 * TM + tid] + s.part[3 * TM + tid])));
-            s.rgb[TM + tid] = 1.0f / (1.0f + expf(-(s.part[1 * TM + tid] + s.part[4 * TM + tid])));
-            s.rgb[2 * TM + tid] = 1.0f / (1.0f + expf(-(s.part[2 * TM + tid] + s.part[5 * TM + tid])));
+            s.rgb[tid] = 1.0f / (1.0f + expf(-s.part[0 * TM + tid]));
+            s.rgb[TM + tid] = 1.0f / (1.0f + expf(-s.part[1 * TM + tid]));
+            s.rgb[2 * TM + tid] = 1.0f / (1.0f + expf(-s.part[2 * TM + tid]));
         }
         __syncthreads();
 
@@ -444,11 +417,8 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
         // no barrier needed here: the refill starts with one before shared memory is touched again
     }
 
-    // drain the prefetched weight tiles, then release TMEM
+    // drain the prefetched weight tiles: the bulk copies must land before the CTA exits
     for (uint32_t q = 0; q < W_NSTAGE; ++q) mbar_wait(&s.bar_full[q], 0);   // tiles 0..2 of a batch that never comes
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, TMEM_COLS);
 }
 
 static_assert(sizeof(SmemTC<false>) + 1024 <= 113 * 1024, "single-pass kernel must fit twice per SM (228 KB - 2 x 1 KB reserved)");

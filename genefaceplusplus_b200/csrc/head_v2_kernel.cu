@@ -1,24 +1,18 @@
-// head_v2_kernel.cu -- fused persistent head renderer, second generation (tcgen05 + TMEM + bulk-copy weight stream).
+// head_v2_kernel.cu -- fused persistent head renderer, second generation (wgmma + bulk-copy weight stream).
 //
 // Replaces the reference's host-driven round loop (modules/radnerfs/renderer.py:340-384: march_rays -> GridEncoder ->
 // ambient MLP -> GridEncoder -> sigma MLP -> SHEncoder -> color MLP -> composite_rays, ~40 launches per round) like
 // head_tc_kernel.cu does, but organised around ROW OWNERSHIP instead of CTA-wide phases:
 //
-//   * one CTA per SM; NSLOT "slots" of 128 samples, each served by 4 warps whose thread r owns row r END TO END: it owns
-//     the ray (marching, compositing, refill), gathers the row's 2 x 16 grid levels, runs every epilogue of the row
-//     (TMEM lane r -> ReLU -> 16-bit operand row of the next layer) and keeps the row's scalars (sample position, ambient
-//     coordinates, sigma, rgb) in REGISTERS.  No thread ever reads another thread's row, so the steady state has no
-//     __syncthreads and no worker<->worker barrier at all;
-//   * one issue warp walks the eight MMA groups of the MLPs layer by layer and, inside a layer, slot by slot: it waits on
-//     the slot's `a_ready` mbarrier (4 warp arrivals), issues that slot's tcgen05.mma's against the staged weight tile and
-//     commits to the slot's `d_ready` mbarrier.  While slot s's MMAs execute, the owners of the other slots run their
-//     epilogues / gathers / ray work: the slots pipeline against each other by construction;
-//   * the weight stream is SHARED: a tile is copied once (cp.async.bulk by the loader warp, NSTAGE-deep ring) and used by all
-//     NSLOT slots before its stage is released (tcgen05.commit -> `w_free`), which cuts the L2->SM weight traffic per sample
-//     by NSLOT -- at this kernel's rate an unshared stream (200 KB per 128 samples) would alone eat half of the ~42 B/clk an
-//     SM can pull from L2;
-//   * the 3-wide output layers (ambient coordinates, rgb) and the sigma logit are N=16 MMAs against small RESIDENT tiles;
-//     the conditioning columns of ambient L0 are folded into a per-frame fp32 bias (k_amb_frame_bias) added in the epilogue.
+//   * one CTA per SM; NSLOT "slots" of 128 samples, each one warpgroup whose thread r owns row r: the ray, the gather of the
+//     row's grid levels into its 16-bit operand row, and the row's scalars in registers;
+//   * the warpgroup runs its own layers with wgmma, rows 0-63 then 64-127 (fp32 accumulators in registers), each half's
+//     epilogue straight from the accumulator fragment (the halves touch disjoint operand rows); while one slot's MMAs run,
+//     the other slots do their gathers and ray work;
+//   * the weight stream is SHARED: the loader warp copies each tile once (NSTAGE-deep ring) for all slots; a stage is refilled
+//     once every owner warp has arrived on `w_free`;
+//   * the 3-wide outputs and the sigma logit are N=16 MMAs against small RESIDENT tiles, handed to the row owners through a
+//     small buffer at the head of the slot's second operand tile.
 //
 // Precision modes: FP16_X1 (the reference's autocast arithmetic) with 3 slots, and FP16_ROBUST with 2 slots: fp16 hi/lo
 // split (3 MMAs per k-step, ~22 mantissa bits) on the ambient net and a 16-bit fixed-point position table (gather8.cuh) --
@@ -41,15 +35,14 @@ using namespace headc;
 namespace {
 
 constexpr int TM = HEAD_TM;          // rows per slot
-constexpr uint32_t D_COLS = 144;     // TMEM columns per slot: 128 wide outputs + 16 for the N=16 groups
 
 template <bool ROBUST>
 struct Cfg {
     static constexpr int NSLOT = ROBUST ? 2 : 3;
-    static constexpr int NSTAGE = 4;   // robust: 4 stages fit with 240 bytes to spare; with 3 the lo-image tiles of ambient L1 arrived late (7.4 K cycles of wait)
+    static constexpr int NSTAGE = 4;   // >= 4: a robust ambient layer waits for four tiles at once
     static constexpr int NTILE = ROBUST ? V2_NTILE_ROBUST : V2_NTILE_X1;
     static constexpr int NWORK = 4 * NSLOT;                 // row-owner warps
-    static constexpr int NT = 32 * (NWORK + 2);             // + issue warp + loader warp
+    static constexpr int NT = 32 * (NWORK + 1);             // + loader warp
     static constexpr int SLOT_BYTES = (ROBUST ? 4 : 2) * V2_TILE_BYTES + 4096;   // h0 h1 [l0 l1] sh
     static constexpr int OFF_W = NSLOT * SLOT_BYTES;
     static constexpr int OFF_RES = OFF_W + NSTAGE * V2_TILE_BYTES;
@@ -60,8 +53,7 @@ struct Misc {
     float cbias[128];                    // color L0 bias (individual code folded)
     uint32_t coarse[HEAD_COARSE_WORDS];
     uint4 lvl[2][2 * GFPP_MAX_LEVELS];
-    unsigned long long a_ready[3], d_ready[3], w_full[4], w_free[4], res_full, batch_bar;
-    uint32_t tmem_base;
+    unsigned long long w_full[4], w_free[4], res_full, batch_bar;
     volatile int stop;
     volatile int flag[2][16];            // per batch parity, per owner warp: "I have live rows"
 };
@@ -70,65 +62,36 @@ template <bool ROBUST>
 constexpr size_t smem_bytes() { return (size_t)Cfg<ROBUST>::OFF_MISC + sizeof(Misc) + 1024; }
 static_assert(smem_bytes<false>() <= 227 * 1024 && smem_bytes<true>() <= 227 * 1024, "v2 shared memory budget");
 
-// ---------------------------------------------------------------- issue-side helpers (warp-uniform operands)
-__device__ __forceinline__ void mma_sw(uint32_t d, uint32_t a, uint32_t w, int ksteps, uint32_t idesc, uint32_t acc_first) {
+// Epilogue of one M = 64 half (rows 64*half ..) of a 128-wide layer from the accumulator fragment: (+bias) -> (ReLU) ->
+// operand tiles h0|h1 (cols 0-63 | 64-127) and, when LO, the residual images l0|l1.  BIAS: shared-memory vector (color L0).
+template <bool RELU, bool BIAS, bool LO>
+__device__ __forceinline__ void epilogue_half(const float (&d)[64], unsigned char *h, unsigned char *l, int half, int lane, int wwarp,
+                                              const float *bias) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-        if (k < ksteps) mma_f16(d, desc_sw128(a + (uint32_t)k * 32u), desc_sw128(w + (uint32_t)k * 32u), idesc, (k > 0) ? 1u : acc_first);
+    for (int i = 0; i < 64; i += 2) {
+        const int row = 64 * half + frag_row(i, lane, wwarp), col = frag_col(i, lane);
+        float x0 = d[i], x1 = d[i + 1];
+        if (BIAS) { x0 += bias[col]; x1 += bias[col + 1]; }
+        if (RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        store_pair<false, LO>(h + (col >> 6) * V2_TILE_BYTES, l + (LO ? (col >> 6) * V2_TILE_BYTES : 0), row, col & 63, x0, x1);
+    }
 }
 
-// ---------------------------------------------------------------- owner-side helpers
-__device__ __forceinline__ uint32_t relu_h2(uint32_t h) {
-    const __half2 z = __float2half2_rn(0.f);
-    const __half2 r = __hmax2(*reinterpret_cast<const __half2 *>(&h), z);
-    return *reinterpret_cast<const uint32_t *>(&r);
-}
 __device__ __forceinline__ float2 unpack_h2(uint32_t h) { return __half22float2(*reinterpret_cast<const __half2 *>(&h)); }
 
-// eight consecutive K values of row `row` -> chunk `chunk` of an SW128 tile (hi) and, when LO, their residuals into `lo`
-template <bool RELU, bool LO>
-__device__ __forceinline__ void put8(unsigned char *hi, unsigned char *lo, int row, int chunk, const float *v) {
-    const uint32_t off = sw128_off(row, chunk);
-    uint4 h;
-    if (LO) {
-        float x[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) x[i] = RELU ? fmaxf(v[i], 0.f) : v[i];
-        h.x = pack2<false>(x[0], x[1]); h.y = pack2<false>(x[2], x[3]); h.z = pack2<false>(x[4], x[5]); h.w = pack2<false>(x[6], x[7]);
-        const float2 a = unpack_h2(h.x), b = unpack_h2(h.y), c = unpack_h2(h.z), d = unpack_h2(h.w);
-        uint4 l;
-        l.x = pack2<false>(x[0] - a.x, x[1] - a.y); l.y = pack2<false>(x[2] - b.x, x[3] - b.y);
-        l.z = pack2<false>(x[4] - c.x, x[5] - c.y); l.w = pack2<false>(x[6] - d.x, x[7] - d.y);
-        *reinterpret_cast<uint4 *>(lo + off) = l;
-    } else {
-        h.x = pack2<false>(v[0], v[1]); h.y = pack2<false>(v[2], v[3]); h.z = pack2<false>(v[4], v[5]); h.w = pack2<false>(v[6], v[7]);
-        if (RELU) { h.x = relu_h2(h.x); h.y = relu_h2(h.y); h.z = relu_h2(h.z); h.w = relu_h2(h.w); }   // max(rn(x), 0) == rn(max(x, 0))
-    }
-    *reinterpret_cast<uint4 *>(hi + off) = h;
+// N = 16 group over K = 128: operand tiles a | a + one tile against the two 2 KB halves of a resident tile at w
+__device__ __forceinline__ void mma16(float (&d)[8], uint32_t a, uint32_t w, uint32_t acc_first) {
+    wgmma_sw<16, false>(d, a, w, 4, acc_first);
+    wgmma_sw<16, false>(d, a + V2_TILE_BYTES, w + 2048, 4, 1u);
 }
 
-// Epilogue of a 128-wide layer for the calling thread's row: TMEM lane -> (+bias) -> (ReLU) -> operand tiles h0|h1 (cols 0-63 | 64-127).
-// BIAS: 0 none, 1 per-frame global vector (ambient L0: the folded conditioning columns), 2 shared-memory vector (color L0).
-template <bool RELU, int BIAS, bool LO>
-__device__ __forceinline__ void epilogue_row(uint32_t taddr, unsigned char *h, unsigned char *l, int row, const float *bias) {
-#pragma unroll 1
-    for (int p = 0; p < 4; ++p) {
-        float v[32];
-        tmem_ld32(taddr + (uint32_t)p * 32u, v);
-        float4 bq[8];
-        if (BIAS) {
+// Columns c0 .. c0+NC-1 of an N = 16 accumulator fragment -> out[c][row] (rows of this half), read back by the row owners
+template <int NC>
+__device__ __forceinline__ void put_cols(const float (&d)[8], float *out, int c0, int half, int lane, int wwarp) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-                bq[j] = BIAS == 1 ? __ldg(reinterpret_cast<const float4 *>(bias) + p * 8 + j) : reinterpret_cast<const float4 *>(bias)[p * 8 + j];
-        }
-        wait_ld();
-        if (BIAS) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { v[4 * j] += bq[j].x; v[4 * j + 1] += bq[j].y; v[4 * j + 2] += bq[j].z; v[4 * j + 3] += bq[j].w; }
-        }
-        unsigned char *ht = h + (p >> 1) * V2_TILE_BYTES, *lt = l + (LO ? (p >> 1) * V2_TILE_BYTES : 0);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) put8<RELU, LO>(ht, lt, row, (p & 1) * 4 + q, &v[8 * q]);
+    for (int i = 0; i < 8; ++i) {
+        const int col = frag_col(i, lane) - c0;
+        if (col >= 0 && col < NC) out[col * TM + 64 * half + frag_row(i, lane, wwarp)] = d[i];
     }
 }
 
@@ -151,7 +114,7 @@ __global__ void k_cond_images(const float *__restrict__ cond /*[F,64]*/, int n, 
 template <bool ROBUST, bool PROFILE>
 __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_constant__ HeadArgs a, const __grid_constant__ HeadV2Args t) {
     using C = Cfg<ROBUST>;
-    constexpr int NSLOT = C::NSLOT, NSTAGE = C::NSTAGE, NTILE = C::NTILE, NWORK = C::NWORK;
+    constexpr int NSTAGE = C::NSTAGE, NTILE = C::NTILE, NWORK = C::NWORK;
     extern __shared__ __align__(1024) unsigned char smem_raw_[];
     unsigned char *sm = smem_raw_ + ((1024u - (smem_u32(smem_raw_) & 1023u)) & 1023u);
     Misc &ms = *reinterpret_cast<Misc *>(sm + C::OFF_MISC);
@@ -168,10 +131,8 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
     } else {
         mc.coarse = a.coarse_bits;
     }
-    if (warp == NWORK) tmem_alloc(&ms.tmem_base, 512);
     if (tid == 0) {
-        for (int i = 0; i < 3; ++i) { mbar_init(&ms.a_ready[i], 4); mbar_init(&ms.d_ready[i], 1); }
-        for (int i = 0; i < 4; ++i) { mbar_init(&ms.w_full[i], 1); mbar_init(&ms.w_free[i], 1); }
+        for (int i = 0; i < 4; ++i) { mbar_init(&ms.w_full[i], 1); mbar_init(&ms.w_free[i], NWORK); }
         mbar_init(&ms.res_full, 1);
         mbar_init(&ms.batch_bar, NWORK);
         mbar_fence_init();
@@ -182,10 +143,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
     stage_level_meta(a.pos_gm, ROBUST ? t.pos_step : nullptr, ms.lvl[0], tid);
     stage_level_meta(a.amb_gm, nullptr, ms.lvl[1], tid);
     fence_async_smem();
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tmem = ms.tmem_base;
     const int total = (a.pass == 1) ? *a.n_hits : *a.n_survivors;
 
     if (warp < NWORK) {
@@ -198,9 +156,13 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         // does not depend on the sample's own sigma, so the march to the next sample, the adoption of a new ray and the gather
         // of the next sample's position features all run in the shadow of the current batch's MMAs.
         // =====================================================================================================
-        const int s = warp >> 2, row = tid & (TM - 1);
+        const int s = warp >> 2, row = tid & (TM - 1), wwarp = warp & 3;
         unsigned char *h = sm + s * C::SLOT_BYTES, *l = h + 2 * V2_TILE_BYTES, *sht = h + (ROBUST ? 4 : 2) * V2_TILE_BYTES;
-        const uint32_t taddr = tmem + ((uint32_t)(warp & 3) * 32u << 16) + (uint32_t)s * D_COLS;
+        // live columns of the N = 16 layers, [4][TM] floats at the head of tile h1: they only overlap operand rows 0-15 of h1,
+        // which half 0 has consumed before they are written and which are rewritten only after the owners have read them
+        float *outc = reinterpret_cast<float *>(h + V2_TILE_BYTES);
+        const uint32_t h_u = smem_u32(h), l_u = smem_u32(l), sh_u = smem_u32(sht), res_u = smem_u32(res), ring_u = smem_u32(wring);
+        uint32_t wc = 0;            // streamed tiles consumed so far (the same sequence in every slot)
         const bool smooth_p = a.pos_gm.interp == 1, smooth_a = a.amb_gm.interp == 1;
         Slot sl;
         sl.active = false;
@@ -209,7 +171,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         sl.near = sl.far = sl.far_m = 0.f;
         ray_geom_init(sl.g, 0.f, 0.f, 0.f, 1.f, 1.f, 1.f);
         WarpFeed wf{0, 0, false};
-        uint32_t dpar = 0, bpar = 0;
+        uint32_t bpar = 0;
         bool newray = false;      // sl holds a freshly adopted ray whose SH operand row is not written yet
         // the sample being shaded: accumulators BEFORE it, its dt / post-sample t, and what happens to its ray afterwards
         struct { bool valid; int fate, D, gid, frame, nsamp; float dt, t_post, ws, depth, r, g, b, near, far; } cu;
@@ -218,19 +180,40 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         uint32_t feat[16];        // position features of the current sample (packed fp16 pairs), prefetched during the previous batch
         uint32_t featl[ROBUST ? 16 : 1];
 
+        // operand rows written by this warpgroup -> visible to its MMAs
 #define ARRIVE_A()                                   \
     do {                                             \
         fence_async_smem();                          \
-        fence_before_sync();                         \
-        __syncwarp();                                \
-        if (lane == 0) mbar_arrive(&ms.a_ready[s]);  \
+        wg_sync(1 + s);                              \
     } while (0)
-#define WAIT_D()                                     \
-    do {                                             \
-        mbar_wait(&ms.d_ready[s], dpar);             \
-        dpar ^= 1u;                                  \
-        fence_after_sync();                          \
-    } while (0)
+        // wait for streamed tile wc + j, return its shared-memory address
+        auto tile = [&](uint32_t j) -> uint32_t {
+            const uint32_t i = wc + j, stage = i % NSTAGE;
+            mbar_wait(&ms.w_full[stage], (i / NSTAGE) & 1u);
+            return ring_u + stage * V2_TILE_BYTES;
+        };
+        // the n tiles just used are free for this warp (its MMAs have completed); a stage is refilled once every owner warp arrived
+        auto release = [&](uint32_t n) {
+            if (lane == 0)
+                for (uint32_t j = 0; j < n; ++j) mbar_arrive(&ms.w_free[(wc + j) % NSTAGE]);
+            __syncwarp();
+            wc += n;
+        };
+        // one 128-wide layer against `ntile` streamed tiles: per M-half, `mma(d, half offset, w0, w1)` then `epi(d, half)`
+        auto layer128 = [&](int ntile, auto &&mma, auto &&epi) {
+            const uint32_t w0 = tile(0), w1 = ntile > 1 ? tile(1) : w0;
+#pragma unroll 1
+            for (int hf = 0; hf < 2; ++hf) {
+                float d[64];
+                wg_fence();
+                mma(d, (uint32_t)hf * SW128_HALF, w0, w1);
+                wg_commit();
+                wg_wait<0>();
+                acc_fence(d);
+                epi(d, hf);
+            }
+            release((uint32_t)ntile);
+        };
         // optional phase stamps (thread 0 = row 0 of slot 0 of every CTA): cycles between consecutive PH() points
         long long ph_last = clock64();
 #define PH(i)                                                                              \
@@ -333,6 +316,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         prefetch_pos(0);
         prefetch_pos(1);
         rotate();
+        mbar_wait(&ms.res_full, 0);   // the resident N = 16 / SH weight tiles
 
         for (;;) {
             const bool valid = cu.valid;
@@ -367,9 +351,8 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                 }
             }
             PH(0)   // operand rows of ambient L0
-            ARRIVE_A();   // -> ambient L0
 
-            // ---------------- in the shadow of the ambient net: fate of the ray, march to the next sample, refill ----------------
+            // ---------------- fate of the ray, march to the next sample, refill (the other slots' MMAs run meanwhile) ----------------
             if (valid) {
                 const int ns = cu.nsamp + 1;                 // samples composited once this one is
                 const float T = 1.0f - cu.ws;
@@ -382,27 +365,65 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
             __syncwarp();
             refill();
             PH(1)   // fate + march + refill
+            ARRIVE_A();   // -> ambient L0
 
             // ---------------- ambient net 96 -> 128 -> 128 -> 3 (radnerf.py:121) ----------------
-            WAIT_D();
-            PH(2)   // wait: ambient L0
-            epilogue_row<true, 0, ROBUST>(taddr, h, l, row, nullptr);
+            // one 128-wide ambient layer: two K tiles (ks0, ks1 k-steps), in the robust mode each as (hi, lo) weight images and
+            // D = Al*Wh + Ah*Wl + Ah*Wh, small terms first
+            auto amb_layer = [&](int ks0, int ks1) {
+                uint32_t wt[ROBUST ? 4 : 2];
+#pragma unroll
+                for (int j = 0; j < (ROBUST ? 4 : 2); ++j) wt[j] = tile((uint32_t)j);
+#pragma unroll 1
+                for (int hf = 0; hf < 2; ++hf) {
+                    const uint32_t o = (uint32_t)hf * SW128_HALF;
+                    float d[64];
+                    wg_fence();
+                    if (ROBUST) {
+#pragma unroll
+                        for (int kt = 0; kt < 2; ++kt) {
+                            const uint32_t wh = wt[ROBUST ? 2 * kt : 0], wl = wt[ROBUST ? 2 * kt + 1 : 0], tk = (uint32_t)kt * V2_TILE_BYTES + o;
+                            const int ks = kt ? ks1 : ks0;
+                            wgmma_sw<128, false>(d, l_u + tk, wh, ks, kt ? 1u : 0u);
+                            wgmma_sw<128, false>(d, h_u + tk, wl, ks, 1u);
+                            wgmma_sw<128, false>(d, h_u + tk, wh, ks, 1u);
+                        }
+                    } else {
+                        wgmma_sw<128, false>(d, h_u + o, wt[0], ks0, 0u);
+                        wgmma_sw<128, false>(d, h_u + V2_TILE_BYTES + o, wt[1], ks1, 1u);
+                    }
+                    wg_commit();
+                    wg_wait<0>();
+                    acc_fence(d);
+                    epilogue_half<true, false, ROBUST>(d, h, l, hf, lane, wwarp, nullptr);
+                }
+                release(ROBUST ? 4 : 2);
+            };
+            amb_layer(4, 2);   // ambient L0: K = 96 = 32 position features + 64 conditioning values (h0 k[0,64), h1 k[0,32))
             ARRIVE_A();   // -> ambient L1
-            PH(3)   // epilogue: ambient L0
-            WAIT_D();
-            PH(4)   // wait: ambient L1
-            epilogue_row<true, 0, ROBUST>(taddr, h, l, row, nullptr);
+            PH(2)   // MMA + epilogue: ambient L0
+            amb_layer(4, 4);   // ambient L1: K = 128
             ARRIVE_A();   // -> ambient out (N = 16)
-            PH(5)   // epilogue: ambient L1
-            WAIT_D();
-            PH(6)   // wait: ambient out
-            float amb0, amb1, amb2;
-            {
-                float o[16];
-                tmem_ld16(taddr + 128u, o);
-                wait_ld();
-                amb0 = tanhf(o[0]); amb1 = tanhf(o[1]); amb2 = tanhf(o[2]);
+            PH(3)   // MMA + epilogue: ambient L1
+#pragma unroll 1
+            for (int hf = 0; hf < 2; ++hf) {   // ambient out: N = 16 group from the resident tiles
+                const uint32_t o = (uint32_t)hf * SW128_HALF;
+                float d[8];
+                wg_fence();
+                if (ROBUST) {
+                    mma16(d, l_u + o, res_u + V2_RES_AMBN_HI, 0u);
+                    mma16(d, h_u + o, res_u + V2_RES_AMBN_LO, 1u);
+                }
+                mma16(d, h_u + o, res_u + V2_RES_AMBN_HI, ROBUST ? 1u : 0u);
+                wg_commit();
+                wg_wait<0>();
+                acc_fence(d);
+                put_cols<3>(d, outc, 0, hf, lane, wwarp);
             }
+            wg_sync(1 + s);
+            PH(4)   // MMA: ambient out
+            const float amb0 = tanhf(outc[row]), amb1 = tanhf(outc[TM + row]), amb2 = tanhf(outc[2 * TM + row]);
+            PH(5)   // tanh
             // ---------------- sigma-net input: h0 k[0,32) <- position features (registers), k[32,64) <- ambient grid ----------------
             {
                 float u = 0.f, vv = 0.f, w = 0.f;
@@ -423,60 +444,86 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
 #pragma unroll
                         for (int i = 0; i < 16; ++i) f[i] = 0.f;
                     }
-                    put8<false, false>(h, h, row, 4 + 2 * half, &f[0]);
-                    put8<false, false>(h, h, row, 4 + 2 * half + 1, &f[8]);
+                    store_chunk<false, false>(h, h, sw128_off(row, 4 + 2 * half), &f[0]);
+                    store_chunk<false, false>(h, h, sw128_off(row, 4 + 2 * half + 1), &f[8]);
                 }
             }
-            PH(7)   // tanh + ambient gather
-            ARRIVE_A();   // -> sigma L0
-
-            // ---------------- sigma net 64 -> 128 -> 128 -> (128 geo + sigma) (radnerf.py:127-130); in its shadow: the NEXT sample's
-            //                  position features (the current ones are in the operand tile now) ----------------
+            PH(7)   // ambient gather
+            // the NEXT sample's position features (the current ones are in the operand tile now)
             prefetch_pos(0);
             PH(8)   // prefetch: position levels 0-7 of the next sample
-            WAIT_D();
-            PH(9)   // wait: sigma L0
-            epilogue_row<true, 0, false>(taddr, h, h, row, nullptr);
+            ARRIVE_A();   // -> sigma L0
+
+            // ---------------- sigma net 64 -> 128 -> 128 -> (128 geo + sigma) (radnerf.py:127-130) ----------------
+            layer128(1, [&](float (&d)[64], uint32_t o, uint32_t w0, uint32_t) { wgmma_sw<128, false>(d, h_u + o, w0, 4, 0u); },   // sigma L0: K = 64
+                     [&](const float (&d)[64], int hf) { epilogue_half<true, false, false>(d, h, h, hf, lane, wwarp, nullptr); });
             ARRIVE_A();   // -> sigma L1
-            PH(10)  // epilogue: sigma L0
+            PH(9)   // MMA + epilogue: sigma L0
             prefetch_pos(1);
-            PH(11)  // prefetch: position levels 8-15 of the next sample
-            WAIT_D();
-            PH(12)  // wait: sigma L1
-            epilogue_row<true, 0, false>(taddr, h, h, row, nullptr);
-            ARRIVE_A();   // -> sigma L2 (geo rows + the sigma row as an N = 16 group)
-            PH(13)  // epilogue: sigma L1
-            WAIT_D();
-            PH(14)  // wait: sigma L2
-            float sigma;
-            {
-                float o[16];
-                tmem_ld16(taddr + 128u, o);
-                wait_ld();
-                sigma = a.density_scale * expf(o[0]);   // trunc_exp forward (utils.py:36-49) * density_scale (renderer.py:365)
+            PH(10)  // prefetch: position levels 8-15 of the next sample
+            layer128(2, [&](float (&d)[64], uint32_t o, uint32_t w0, uint32_t w1) {   // sigma L1: K = 128
+                wgmma_sw<128, false>(d, h_u + o, w0, 4, 0u);
+                wgmma_sw<128, false>(d, h_u + V2_TILE_BYTES + o, w1, 4, 1u);
+            }, [&](const float (&d)[64], int hf) { epilogue_half<true, false, false>(d, h, h, hf, lane, wwarp, nullptr); });
+            ARRIVE_A();   // -> sigma L2
+            PH(11)  // MMA + epilogue: sigma L1
+            float slogit[2][2];   // sigma logit of fragment rows r, r+8 of each half (lanes with lane % 4 == 0)
+            {   // sigma L2: 128 geo rows (streamed) + the sigma row (resident N = 16 tile)
+                const uint32_t w0 = tile(0), w1 = tile(1);
+#pragma unroll
+                for (int hf = 0; hf < 2; ++hf) {
+                    const uint32_t o = (uint32_t)hf * SW128_HALF;
+                    float d[64], d16[8];
+                    wg_fence();
+                    wgmma_sw<128, false>(d, h_u + o, w0, 4, 0u);
+                    wgmma_sw<128, false>(d, h_u + V2_TILE_BYTES + o, w1, 4, 1u);
+                    mma16(d16, h_u + o, res_u + V2_RES_SIGROW, 0u);
+                    wg_commit();
+                    wg_wait<0>();
+                    acc_fence(d);
+                    acc_fence(d16);
+                    slogit[hf][0] = d16[0];
+                    slogit[hf][1] = d16[2];
+                    epilogue_half<false, false, false>(d, h, h, hf, lane, wwarp, nullptr);   // geo features (no activation) -> color-net input
+                }
+                release(2);
             }
-            epilogue_row<false, 0, false>(taddr, h, h, row, nullptr);   // geo features (no activation) -> color-net input
             ARRIVE_A();   // -> color L0 (geo K = 128 + SH K = 16)
-            PH(15)  // epilogue: sigma L2 (sigma + geo)
+            PH(12)  // MMA + epilogue: sigma L2 (sigma + geo)
 
             // ---------------- color net (16 SH + 128 geo [+ folded individual code]) -> 128 -> 3 (radnerf.py:137-141) ----------------
-            WAIT_D();
-            PH(16)  // wait: color L0
-            epilogue_row<true, 2, false>(taddr, h, h, row, ms.cbias);
+            // color L0: geo K = 128 (streamed) + SH K = 16 (resident no-swizzle tile against the slot's SH operand tile)
+            layer128(2, [&](float (&d)[64], uint32_t o, uint32_t w0, uint32_t w1) {
+                wgmma_sw<128, false>(d, h_u + o, w0, 4, 0u);
+                wgmma_sw<128, false>(d, h_u + V2_TILE_BYTES + o, w1, 4, 1u);
+                wgmma<128, false>(d, desc_k16(sh_u + (o ? K16_HALF : 0u)), desc_k16(res_u + V2_RES_COLSH), 1u);
+            }, [&](const float (&d)[64], int hf) { epilogue_half<true, true, false>(d, h, h, hf, lane, wwarp, ms.cbias); });
             ARRIVE_A();   // -> color out (N = 16)
-            PH(17)  // epilogue: color L0
-            WAIT_D();
-            PH(18)  // wait: color out
-            float cr, cg, cb;
-            {
-                float o[16];
-                tmem_ld16(taddr + 128u, o);
-                wait_ld();
-                cr = 1.0f / (1.0f + expf(-o[0]));
-                cg = 1.0f / (1.0f + expf(-o[1]));
-                cb = 1.0f / (1.0f + expf(-o[2]));
+            PH(13)  // MMA + epilogue: color L0
+#pragma unroll
+            for (int hf = 0; hf < 2; ++hf) {   // color out: N = 16 group; the sigma logits join the rgb logits in the hand-over buffer
+                const uint32_t o = (uint32_t)hf * SW128_HALF;
+                float d[8];
+                wg_fence();
+                mma16(d, h_u + o, res_u + V2_RES_COLN, 0u);
+                wg_commit();
+                wg_wait<0>();
+                acc_fence(d);
+                put_cols<3>(d, outc, 0, hf, lane, wwarp);
+                if ((lane & 3) == 0) {
+                    outc[3 * TM + 64 * hf + frag_row(0, lane, wwarp)] = slogit[hf][0];
+                    outc[3 * TM + 64 * hf + frag_row(2, lane, wwarp)] = slogit[hf][1];
+                }
             }
-            fence_before_sync();   // the next batch's MMAs overwrite these TMEM columns: order the loads above before the next arrive
+            wg_sync(1 + s);
+            PH(14)  // MMA: color out
+            // trunc_exp forward (utils.py:36-49) * density_scale (renderer.py:365)
+            const float sigma = a.density_scale * expf(outc[3 * TM + row]);
+            const float cr = 1.0f / (1.0f + expf(-outc[row]));
+            const float cg = 1.0f / (1.0f + expf(-outc[TM + row]));
+            const float cb = 1.0f / (1.0f + expf(-outc[2 * TM + row]));
+            wg_sync(1 + s);   // the next batch's operand rows overwrite the hand-over buffer
+            PH(15)  // sigmoid
 
             // ---------------- composite the sample (raymarching.cu:978-1006) and retire / suspend / continue its ray ----------------
             if (valid) {
@@ -520,212 +567,23 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
             for (int i = 0; i < NWORK; ++i) any |= ms.flag[bpar][i];
             bpar ^= 1u;
             __syncwarp();
-            PH(19)  // sigmoid + composite + end-of-batch check
+            PH(19)  // composite + end-of-batch check
             if (PROFILE && a.phase_cycles && tid == 0) atomicAdd(a.phase_cycles + 31, 1ull);   // batches
             if (!any) break;
         }
 #undef PH
 #undef ARRIVE_A
-#undef WAIT_D
-    } else if (warp == NWORK) {
-        // =====================================================================================================
-        // ISSUE WARP: layer-major, slot-minor; all lanes converged, one elected lane issues
-        // =====================================================================================================
-        const uint32_t idesc128 = make_idesc(0, 128), idesc16 = make_idesc(0, 16);
-        const uint32_t res_u = smem_u32(res), ring_u = smem_u32(wring), slot_u = smem_u32(sm);
-        uint32_t apar = 0;          // all slots arrive the same number of times: one parity bit serves them all
-        uint32_t wc = 0;            // streamed tiles consumed so far
-        uint32_t bpar = 0;
-        mbar_wait(&ms.res_full, 0);
-        fence_after_sync();
-
-        auto h_of = [&](int s, int i) -> uint32_t { return slot_u + (uint32_t)(s * C::SLOT_BYTES + i * V2_TILE_BYTES); };
-        auto l_of = [&](int s, int i) -> uint32_t { return slot_u + (uint32_t)(s * C::SLOT_BYTES + (2 + i) * V2_TILE_BYTES); };
-        auto sh_of = [&](int s) -> uint32_t { return slot_u + (uint32_t)(s * C::SLOT_BYTES + (ROBUST ? 4 : 2) * V2_TILE_BYTES); };
-        auto d_of = [&](int s) -> uint32_t { return tmem + (uint32_t)s * D_COLS; };
-        // wait for streamed tile wc + j, return its shared-memory address
-        auto tile = [&](uint32_t j) -> uint32_t {
-            const uint32_t i = wc + j, stage = i % NSTAGE;
-            mbar_wait(&ms.w_full[stage], (i / NSTAGE) & 1u);
-            return ring_u + stage * V2_TILE_BYTES;
-        };
-        auto release = [&](uint32_t n) {   // the n tiles just used are free once every MMA issued so far has completed
-            if (elect_one()) {
-                for (uint32_t j = 0; j < n; ++j) mma_commit(&ms.w_free[(wc + j) % NSTAGE]);
-            }
-            __syncwarp();
-            wc += n;
-        };
-        // one 128-wide ambient layer in the split arithmetic: two K tiles, each as (hi, lo) weight images shared by all slots;
-        // D = Al*Wh + Ah*Wl + Ah*Wh, small terms first
-        auto robust_layer = [&](int ks0, int ks1) {
-#pragma unroll
-            for (int kt = 0; kt < 2; ++kt) {
-                const uint32_t wh = tile(0), wl = tile(1);
-                const int ks = kt ? ks1 : ks0;
-                fence_after_sync();
-#pragma unroll
-                for (int s = 0; s < NSLOT; ++s) {
-                    if (kt == 0) { mbar_wait(&ms.a_ready[s], apar); fence_after_sync(); }
-                    if (elect_one()) {
-                        mma_sw(d_of(s), l_of(s, kt), wh, ks, idesc128, kt ? 1u : 0u);
-                        mma_sw(d_of(s), h_of(s, kt), wl, ks, idesc128, 1u);
-                        mma_sw(d_of(s), h_of(s, kt), wh, ks, idesc128, 1u);
-                        if (kt == 1) mma_commit(&ms.d_ready[s]);
-                    }
-                    __syncwarp();
-                }
-                release(2);
-            }
-        };
-        // Slots of a layer are served in index order (blocking waits) or -- `relaxed` -- in the order their owners arrive: a sweep of
-        // non-blocking tests serves whoever is ready; only when nobody is does the warp block on the first slot still pending.
-        const bool relaxed = (t.flags & 1u) != 0u;
-#define FOR_SLOTS                                                                                                     \
-    for (uint32_t pend = (1u << NSLOT) - 1u, force = relaxed ? 0u : 1u, got = 0u; pend; force = (relaxed && got) ? 0u : 1u, got = 0u) \
-        _Pragma("unroll") for (int s = 0; s < NSLOT; ++s)
-#define SLOT_BEGIN(sv)                                                         \
-    if (!((pend >> (sv)) & 1u)) continue;                                      \
-    if (force) { mbar_wait(&ms.a_ready[sv], apar); if (relaxed) force = 0u; }  \
-    else if (!mbar_test(&ms.a_ready[sv], apar)) continue;                      \
-    pend &= ~(1u << (sv)); got = 1u;                                           \
-    fence_after_sync();                                                        \
-    if (elect_one()) {
-#define SLOT_END(sv)                              \
-        mma_commit(&ms.d_ready[sv]);              \
-    }                                             \
-    __syncwarp();
-
-        for (;;) {
-            // ---- ambient L0: K = 96 = 32 position features + 64 conditioning values (h0 k[0,64), h1 k[0,32)) ----
-            if (ROBUST) {
-                robust_layer(4, 2);
-            } else {
-                const uint32_t w0 = tile(0), w1 = tile(1);
-                fence_after_sync();
-                FOR_SLOTS {
-                    SLOT_BEGIN(s)
-                    mma_sw(d_of(s), h_of(s, 0), w0, 4, idesc128, 0u);
-                    mma_sw(d_of(s), h_of(s, 1), w1, 2, idesc128, 1u);
-                    SLOT_END(s)
-                }
-                release(2);
-            }
-            apar ^= 1u;
-            // everyone has arrived for this batch: is anything alive in it?  (read now, acted upon at the end of the batch)
-            mbar_wait(&ms.batch_bar, bpar);
-            int any = 0;
-#pragma unroll
-            for (int i = 0; i < NWORK; ++i) any |= ms.flag[bpar][i];
-            bpar ^= 1u;
-            // ---- ambient L1: K = 128 ----
-            if (ROBUST) {
-                robust_layer(4, 4);
-            } else {
-                const uint32_t w0 = tile(0), w1 = tile(1);
-                fence_after_sync();
-                FOR_SLOTS {
-                    SLOT_BEGIN(s)
-                    mma_sw(d_of(s), h_of(s, 0), w0, 4, idesc128, 0u);
-                    mma_sw(d_of(s), h_of(s, 1), w1, 4, idesc128, 1u);
-                    SLOT_END(s)
-                }
-                release(2);
-            }
-            apar ^= 1u;
-            // ---- ambient out: N = 16 group from the resident tiles, into columns 128..143 ----
-            FOR_SLOTS {
-                SLOT_BEGIN(s)
-                if (ROBUST) {
-                    mma_sw(d_of(s) + 128u, l_of(s, 0), res_u + V2_RES_AMBN_HI, 4, idesc16, 0u);
-                    mma_sw(d_of(s) + 128u, l_of(s, 1), res_u + V2_RES_AMBN_HI + 2048, 4, idesc16, 1u);
-                    mma_sw(d_of(s) + 128u, h_of(s, 0), res_u + V2_RES_AMBN_LO, 4, idesc16, 1u);
-                    mma_sw(d_of(s) + 128u, h_of(s, 1), res_u + V2_RES_AMBN_LO + 2048, 4, idesc16, 1u);
-                    mma_sw(d_of(s) + 128u, h_of(s, 0), res_u + V2_RES_AMBN_HI, 4, idesc16, 1u);
-                    mma_sw(d_of(s) + 128u, h_of(s, 1), res_u + V2_RES_AMBN_HI + 2048, 4, idesc16, 1u);
-                } else {
-                    mma_sw(d_of(s) + 128u, h_of(s, 0), res_u + V2_RES_AMBN_HI, 4, idesc16, 0u);
-                    mma_sw(d_of(s) + 128u, h_of(s, 1), res_u + V2_RES_AMBN_HI + 2048, 4, idesc16, 1u);
-                }
-                SLOT_END(s)
-            }
-            apar ^= 1u;
-            // ---- sigma L0: K = 64 ----
-            {
-                const uint32_t w0 = tile(0);
-                fence_after_sync();
-                FOR_SLOTS {
-                    SLOT_BEGIN(s)
-                    mma_sw(d_of(s), h_of(s, 0), w0, 4, idesc128, 0u);
-                    SLOT_END(s)
-                }
-                release(1);
-                apar ^= 1u;
-            }
-            // ---- sigma L1: K = 128 ----
-            {
-                const uint32_t w0 = tile(0), w1 = tile(1);
-                fence_after_sync();
-                FOR_SLOTS {
-                    SLOT_BEGIN(s)
-                    mma_sw(d_of(s), h_of(s, 0), w0, 4, idesc128, 0u);
-                    mma_sw(d_of(s), h_of(s, 1), w1, 4, idesc128, 1u);
-                    SLOT_END(s)
-                }
-                release(2);
-                apar ^= 1u;
-            }
-            // ---- sigma L2: 128 geo rows + the sigma row (resident N = 16 tile -> column 128) ----
-            {
-                const uint32_t w0 = tile(0), w1 = tile(1);
-                fence_after_sync();
-                FOR_SLOTS {
-                    SLOT_BEGIN(s)
-                    mma_sw(d_of(s), h_of(s, 0), w0, 4, idesc128, 0u);
-                    mma_sw(d_of(s), h_of(s, 1), w1, 4, idesc128, 1u);
-                    mma_sw(d_of(s) + 128u, h_of(s, 0), res_u + V2_RES_SIGROW, 4, idesc16, 0u);
-                    mma_sw(d_of(s) + 128u, h_of(s, 1), res_u + V2_RES_SIGROW + 2048, 4, idesc16, 1u);
-                    SLOT_END(s)
-                }
-                release(2);
-                apar ^= 1u;
-            }
-            // ---- color L0: geo K = 128 (streamed) + SH K = 16 (resident no-swizzle tile against the slot's SH operand tile) ----
-            {
-                const uint32_t w0 = tile(0), w1 = tile(1);
-                fence_after_sync();
-                FOR_SLOTS {
-                    SLOT_BEGIN(s)
-                    mma_sw(d_of(s), h_of(s, 0), w0, 4, idesc128, 0u);
-                    mma_sw(d_of(s), h_of(s, 1), w1, 4, idesc128, 1u);
-                    mma_f16(d_of(s), desc_k16(sh_of(s)), desc_k16(res_u + V2_RES_COLSH), idesc128, 1u);
-                    SLOT_END(s)
-                }
-                release(2);
-                apar ^= 1u;
-            }
-            // ---- color out: N = 16 group ----
-            FOR_SLOTS {
-                SLOT_BEGIN(s)
-                mma_sw(d_of(s) + 128u, h_of(s, 0), res_u + V2_RES_COLN, 4, idesc16, 0u);
-                mma_sw(d_of(s) + 128u, h_of(s, 1), res_u + V2_RES_COLN + 2048, 4, idesc16, 1u);
-                SLOT_END(s)
-            }
-            apar ^= 1u;
-            if (!any) break;
+        // stop the loader: the NSTAGE tiles it has prefetched for a batch that never comes must land before the CTA may exit.
+        // `stop` is raised only once all of them have landed: the other slots may still be releasing their last tiles, and a
+        // loader that saw `stop` before issuing these would leave the waits below hanging.
+#pragma unroll 1
+        for (uint32_t j = 0; j < (uint32_t)NSTAGE; ++j) mbar_wait(&ms.w_full[(wc + j) % NSTAGE], ((wc + j) / NSTAGE) & 1u);
+        if (lane == 0) {
+            ms.stop = 1;
+            __threadfence_block();
+            for (uint32_t j = 0; j < (uint32_t)NSTAGE; ++j) mbar_arrive(&ms.w_free[(wc + j) % NSTAGE]);
         }
-#undef FOR_SLOTS
-#undef SLOT_BEGIN
-#undef SLOT_END
-        // stop the loader: the NSTAGE tiles it has prefetched for a batch that never comes must land before the CTA may exit
-        ms.stop = 1;
-        __threadfence_block();
-        for (uint32_t j = 0; j < (uint32_t)NSTAGE; ++j) {
-            const uint32_t i = wc + j, stage = i % NSTAGE;
-            mbar_wait(&ms.w_full[stage], (i / NSTAGE) & 1u);
-            if (lane == 0) mbar_arrive(&ms.w_free[stage]);
-            __syncwarp();
-        }
+        __syncwarp();
     } else {
         // =====================================================================================================
         // LOADER WARP: resident tiles once, then the weight stream, NSTAGE tiles ahead of the issue warp
@@ -747,9 +605,6 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         }
     }
 
-    fence_before_sync();
-    __syncthreads();
-    if (warp == NWORK) tmem_dealloc(tmem, 512);
 }
 
 size_t head_v2_smem_bytes(bool robust) { return robust ? smem_bytes<true>() : smem_bytes<false>(); }
@@ -761,12 +616,10 @@ cudaError_t launch_cond_images(const float *cond_feat, int n_frames, void *cond_
 }
 
 cudaError_t launch_head_v2(const HeadArgs &a, const HeadV2Args &t_in, int precision, cudaStream_t st) {
-    HeadV2Args t = t_in;
-    // scheduling knob of the issue warp (bit 0: serve the slots of a layer in arrival order); GFPP_V2_RELAXED overrides the default for A/B runs
-    t.flags = getenv("GFPP_V2_RELAXED") ? (atoi(getenv("GFPP_V2_RELAXED")) ? 1u : 0u) : V2_DEFAULT_FLAGS;
+    const HeadV2Args &t = t_in;
     const bool robust = precision == FP16_ROBUST;
     if (!robust && precision != FP16_X1) return cudaErrorInvalidValue;
-    const int blocks = sm_count();   // persistent: one CTA per SM (512 TMEM columns and ~200 KB of shared memory each)
+    const int blocks = sm_count();   // persistent: one CTA per SM (~200 KB of shared memory each)
     const size_t smem = head_v2_smem_bytes(robust);
     cudaError_t e;
     // function attributes are per device: set on every launch.  The phase-stamped instantiation only runs under tools/phase_breakdown.py.

@@ -1,4 +1,4 @@
-// launch.cuh -- launch helpers: grids are sized in multiples of the SM count (148 on B200) and
+// launch.cuh -- launch helpers: grids are sized in multiples of the SM count (132 on H100) and
 // kernels are grid-stride, so a launch is never a ragged fraction of a wave.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// sr_kernel.cu -- super-resolution head of the SR checkpoints (256x256 NeRF image -> 512x512) on sm_100a.
+// sr_kernel.cu -- super-resolution head of the SR checkpoints (256x256 NeRF image -> 512x512) on sm_90a.
 //
 // Replaces `Superresolution.forward` of modules/radnerfs/radnerf_sr.py:15-48, which the reference assembles from StyleGAN2
 // synthesis blocks (modules/eg3ds/models/superresolution.py:159-257, networks_stylegan2.py:286-475) and runs as per-sample
@@ -7,7 +7,7 @@
 // plain convolution weights once (genefaceplusplus_b200/superres.py) and the six layers become four launches per clip chunk:
 //
 //   k_sr_conv_in   block0.conv0    3 -> 128, 3x3          fp32 FFMA (K = 27 is no tensor-core shape), fp16 NHWC out
-//   k_sr_conv<0>   block0.conv1  128 -> 128, 3x3          implicit GEMM on tcgen05; epilogue: noise, bias, leaky-ReLU*sqrt2,
+//   k_sr_conv<0>   block0.conv1  128 -> 128, 3x3          implicit GEMM on wgmma;   epilogue: noise, bias, leaky-ReLU*sqrt2,
 //                                                         clamp, fp16 NHWC out + fused toRGB (128 -> 3, fp32) + rgb skip -> img0
 //   k_sr_conv<1>   block1.conv0  128 -> 64, up x2         transposed stride-2 conv + [1,3,3,1] FIR merged into four 3x3 phase
 //                                                         kernels on the INPUT grid: one GEMM with N = 4 x 64, no 513x513
@@ -17,10 +17,10 @@
 //
 // Implicit GEMM: a tile is 128 consecutive pixels of one image row (the 128 rows of the MMA); K runs over the 9 taps x
 // C_in in chunks of 64 channels.  For every chunk the CTA's threads copy the shifted 128 x 64 fp16 window of the NHWC
-// activation straight into a UMMA K-major SW128 operand tile (one 16-byte load + one 16-byte store per thread and task,
-// zeros outside the image), double-buffered against the MMAs through tcgen05.commit -> mbarrier; the weight chunks stream
-// through a 4-deep cp.async.bulk + mbarrier ring; accumulators live in TMEM (64 / 128 / 256 columns) and are read back with
-// tcgen05.ld for the epilogue.  Operands are fp16, accumulation fp32 -- the reference runs these blocks in fp16 on CUDA
+// activation straight into a GMMA K-major SW128 operand tile (one 16-byte load + one 16-byte store per thread and task,
+// zeros outside the image), double-buffered against the MMAs (one wgmma group of each warpgroup stays in flight while the
+// next window is copied); the weight chunks stream through a 4-deep cp.async.bulk + mbarrier ring; the two warpgroups of
+// the CTA own pixel rows 0-63 and 64-127 and keep their accumulators (64 / 128 / 32 fp32 registers) for the epilogue.  Operands are fp16, accumulation fp32 -- the reference runs these blocks in fp16 on CUDA
 // (use_fp16 of the synthesis blocks), toRGB and the skip path stay fp32.
 #include <math.h>
 
@@ -46,31 +46,14 @@ struct SmemSR {
     alignas(1024) unsigned char w[RING][sr_layer_chunk_bytes(LAYER)];
     float bias[128];
     float rgbw[3 * 128];
-    float part[2 * 3 * TM];
+    float part[3 * TM];
     unsigned long long bar_wfull[RING];
-    unsigned long long bar_afree[2];
-    unsigned long long bar_acc;
-    uint32_t tmem_base;
 };
 
 // bias_act of the synthesis layers: leaky-ReLU(0.2) * sqrt(2), then clamp to +-256 (networks_stylegan2.py:330-333)
 __device__ __forceinline__ float lrelu_clamp(float t) {
     t = (t < 0.f ? 0.2f * t : t) * kSqrt2;
     return fminf(fmaxf(t, -256.f), 256.f);
-}
-
-// 32 activations -> 64 bytes of fp16
-__device__ __forceinline__ void store_half32(__half *dst, const float (&v)[32]) {
-    uint4 *d = reinterpret_cast<uint4 *>(dst);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        uint4 u;
-        u.x = pack2<false>(v[8 * q + 0], v[8 * q + 1]);
-        u.y = pack2<false>(v[8 * q + 2], v[8 * q + 3]);
-        u.z = pack2<false>(v[8 * q + 4], v[8 * q + 5]);
-        u.w = pack2<false>(v[8 * q + 6], v[8 * q + 7]);
-        d[q] = u;
-    }
 }
 
 // upfirdn2d.upsample2d with the [1,3,3,1] binomial filter at output pixel (y, x) of the 2h x 2w image: zero insertion,
@@ -107,13 +90,13 @@ __global__ void __launch_bounds__(NT, LAYER == 1 ? 1 : 2) k_sr_conv(const __grid
     constexpr int CIN = sr_layer_cin(LAYER), CB = CIN / 64, NC = sr_layer_nchunk(LAYER);
     constexpr int NB = sr_layer_nb(LAYER), NROWS = sr_layer_nrows(LAYER);
     constexpr uint32_t WCHUNK = (uint32_t)sr_layer_chunk_bytes(LAYER);
-    constexpr uint32_t TMEM_COLS = (uint32_t)(NB * NROWS);   // 128 / 256 / 64: powers of two >= 32
     constexpr int COUT = LAYER == 0 ? 128 : 64;
+    constexpr int R = NROWS / 2;   // accumulator registers per N-block
 
     extern __shared__ __align__(1024) unsigned char smem_raw_[];
     unsigned char *smem_raw = smem_raw_ + ((1024u - (smem_u32(smem_raw_) & 1023u)) & 1023u);
     SmemSR<LAYER> &s = *reinterpret_cast<SmemSR<LAYER> *>(smem_raw);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7, wwarp = warp & 3;
 
     const int tiles_per_row = a.W / TM;
     const int n_tiles = a.F * a.H * tiles_per_row;
@@ -121,22 +104,14 @@ __global__ void __launch_bounds__(NT, LAYER == 1 ? 1 : 2) k_sr_conv(const __grid
     const uint32_t g_total = (uint32_t)n_my * (uint32_t)NC;
 
     // ---- one-time setup ----
-    if (warp == 0) tmem_alloc(&s.tmem_base, TMEM_COLS);
     if (tid == 32) {
         for (int i = 0; i < RING; ++i) mbar_init(&s.bar_wfull[i], 1);
-        mbar_init(&s.bar_afree[0], 1);
-        mbar_init(&s.bar_afree[1], 1);
-        mbar_init(&s.bar_acc, 1);
         mbar_fence_init();
     }
     for (int i = tid; i < COUT; i += NT) s.bias[i] = a.bias[i];
     if (LAYER != 1)
         for (int i = tid; i < 3 * COUT; i += NT) s.rgbw[i] = a.rgb_w[i];
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tmem = s.tmem_base;
-    const uint32_t idesc = make_idesc(0, NROWS);
     if (warp == 0) {   // first RING weight chunks of the (cyclic) stream
         if (elect_one()) {
             for (uint32_t q = 0; q < (uint32_t)RING && q < g_total; ++q) {
@@ -147,8 +122,6 @@ __global__ void __launch_bounds__(NT, LAYER == 1 ? 1 : 2) k_sr_conv(const __grid
         __syncwarp();
     }
 
-    const int row_e = tid & (TM - 1), half = tid >> 7;             // epilogue role: (pixel row, column half)
-    const uint32_t lane_base = (uint32_t)(warp & 3) * 32u;          // TMEM lanes this warp may read
     uint32_t g = 0;                                                 // running K-chunk counter (CTA-uniform)
 #pragma unroll 1
     for (int it = 0; it < n_my; ++it) {
@@ -158,12 +131,15 @@ __global__ void __launch_bounds__(NT, LAYER == 1 ? 1 : 2) k_sr_conv(const __grid
         const int y = fy % a.H, f = fy / a.H;
         const int x0 = xseg * TM;
 
+        float d[NB][R];
 #pragma unroll 1
         for (int c = 0; c < NC; ++c, ++g) {
             const int b = (int)(g & 1u);
             if (g >= 2) {
-                // the MMAs of chunk g-2 have finished reading A[b] and their weight slot
-                mbar_wait(&s.bar_afree[b], ((g >> 1) - 1u) & 1u);
+                // this warpgroup's MMAs of chunk g-2 have finished reading A[b] and their weight slot; the CTA barrier makes
+                // that true of both warpgroups (chunk g-1 may still run)
+                if (c > 0) wg_wait<1>();
+                __syncthreads();
                 if (warp == 0) {
                     if (g + 2 < g_total && elect_one()) {   // refill that slot with chunk g+2
                         const uint32_t q = g + 2, slot = q % RING;
@@ -195,131 +171,97 @@ __global__ void __launch_bounds__(NT, LAYER == 1 ? 1 : 2) k_sr_conv(const __grid
             }
             fence_async_smem();
             __syncthreads();
-            if (warp == 0) {
+            {
                 const uint32_t slot = g % RING;
                 mbar_wait(&s.bar_wfull[slot], (g / RING) & 1u);
-                fence_after_sync();
-                if (elect_one()) {
-                    const uint32_t a_addr = smem_u32(s.a[b]), w_addr = smem_u32(s.w[slot]);
+                const uint32_t a_addr = smem_u32(s.a[b]) + (uint32_t)wg * SW128_HALF, w_addr = smem_u32(s.w[slot]);
+                wg_fence();
 #pragma unroll
-                    for (int nb = 0; nb < NB; ++nb) {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            mma_f16(tmem + (uint32_t)(nb * NROWS), desc_sw128(a_addr + (uint32_t)k * 32u),
-                                    desc_sw128(w_addr + (uint32_t)(nb * NROWS * 128) + (uint32_t)k * 32u), idesc, (c > 0 || k > 0) ? 1u : 0u);
-                    }
-                    mma_commit(&s.bar_afree[b]);
-                    if (c == NC - 1) mma_commit(&s.bar_acc);
-                }
-                __syncwarp();
+                for (int nb = 0; nb < NB; ++nb)
+                    wgmma_sw<NROWS, false>(d[nb], a_addr, w_addr + (uint32_t)(nb * NROWS * 128), 4, c > 0 ? 1u : 0u);
+                wg_commit();
             }
         }
-
-        // ================= epilogue of the tile =================
-        mbar_wait(&s.bar_acc, (uint32_t)it & 1u);
-        fence_after_sync();
-        const int x = x0 + row_e;
-        const uint32_t taddr = tmem + (lane_base << 16);
-        if (LAYER == 0) {
-            const size_t pix = ((size_t)f * a.H + y) * a.W + x;
-            const float nz = a.noise ? __ldg(a.noise + (size_t)f * a.noise_fstride + (size_t)y * a.W + x) : 0.f;
-            float d0 = 0.f, d1 = 0.f, d2 = 0.f;
-#pragma unroll 1
-            for (int p = 0; p < 2; ++p) {
-                float v[32];
-                const int col0 = half * 64 + p * 32;
-                tmem_ld32(taddr + (uint32_t)col0, v);
-                wait_ld();
+        wg_wait<0>();
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    const float t = lrelu_clamp(v[i] + nz + s.bias[col0 + i]);
-                    v[i] = t;
-                    d0 = fmaf(t, s.rgbw[col0 + i], d0);
-                    d1 = fmaf(t, s.rgbw[COUT + col0 + i], d1);
-                    d2 = fmaf(t, s.rgbw[2 * COUT + col0 + i], d2);
-                }
-                store_half32(a.out + pix * COUT + col0, v);
+        for (int nb = 0; nb < NB; ++nb) acc_fence(d[nb]);
+
+        // ================= epilogue of the tile (accumulator fragment: rows 64*wg + frag_row, columns frag_col) =================
+        if (LAYER == 0 || LAYER == 2) {
+            float dot[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+            float nz[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int x = x0 + 64 * wg + frag_row(2 * h, lane, wwarp);
+                nz[h] = a.noise ? __ldg(a.noise + (size_t)f * a.noise_fstride + (size_t)y * a.W + x) : 0.f;
             }
-            s.part[(half * 3 + 0) * TM + row_e] = d0;
-            s.part[(half * 3 + 1) * TM + row_e] = d1;
-            s.part[(half * 3 + 2) * TM + row_e] = d2;
-            fence_before_sync();
-            __syncthreads();
-            if (tid < TM) {   // toRGB (+ bias, clamp) added to the rgb skip (networks_stylegan2.py:395-403, 462-466)
+#pragma unroll
+            for (int i = 0; i < R; i += 2) {
+                const int h = (i >> 1) & 1, col = frag_col(i, lane);
+                const float t0 = lrelu_clamp(d[0][i] + nz[h] + s.bias[col]), t1 = lrelu_clamp(d[0][i + 1] + nz[h] + s.bias[col + 1]);
+#pragma unroll
+                for (int o = 0; o < 3; ++o) dot[h][o] = fmaf(t1, s.rgbw[o * COUT + col + 1], fmaf(t0, s.rgbw[o * COUT + col], dot[h][o]));
+                if (LAYER == 0) {
+                    const size_t pix = ((size_t)f * a.H + y) * a.W + x0 + 64 * wg + frag_row(i, lane, wwarp);
+                    *reinterpret_cast<uint32_t *>(a.out + pix * COUT + col) = pack2<false>(t0, t1);
+                }
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
 #pragma unroll
                 for (int o = 0; o < 3; ++o) {
-                    float r = s.part[o * TM + tid] + s.part[(3 + o) * TM + tid] + __ldg(a.rgb_b + o);
-                    r = fminf(fmaxf(r, -256.f), 256.f);
-                    a.img_out[pix * 3 + o] = __ldg(a.img_in + pix * 3 + o) + r;
+                    float v = dot[h][o];
+                    v += __shfl_xor_sync(0xffffffffu, v, 1);
+                    v += __shfl_xor_sync(0xffffffffu, v, 2);
+                    if ((lane & 3) == 0) s.part[o * TM + 64 * wg + frag_row(2 * h, lane, wwarp)] = v;
                 }
             }
-        } else if (LAYER == 1) {
-            // N-block `half` holds the phases (py = half, px = 0 / 1): output pixels (2y + py, 2x + px), 64 channels each
-            const int Ho = 2 * a.H, Wo = 2 * a.W, Y = 2 * y + half;
-#pragma unroll 1
-            for (int px = 0; px < 2; ++px) {
-                const int X = 2 * x + px;
-                const size_t opix = ((size_t)f * Ho + Y) * Wo + X;
-                const float nz = a.noise ? __ldg(a.noise + (size_t)f * a.noise_fstride + (size_t)Y * Wo + X) : 0.f;
-#pragma unroll 1
-                for (int p = 0; p < 2; ++p) {
-                    float v[32];
-                    tmem_ld32(taddr + (uint32_t)(half * 128 + px * 64 + p * 32), v);
-                    wait_ld();
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) v[i] = lrelu_clamp(v[i] + nz + s.bias[p * 32 + i]);
-                    store_half32(a.out + opix * COUT + p * 32, v);
-                }
-            }
-            fence_before_sync();
-        } else {
-            const float nz = a.noise ? __ldg(a.noise + (size_t)f * a.noise_fstride + (size_t)y * a.W + x) : 0.f;
-            float d0 = 0.f, d1 = 0.f, d2 = 0.f;
-            {
-                float v[32];
-                const int col0 = half * 32;
-                tmem_ld32(taddr + (uint32_t)col0, v);
-                wait_ld();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    const float t = lrelu_clamp(v[i] + nz + s.bias[col0 + i]);
-                    d0 = fmaf(t, s.rgbw[col0 + i], d0);
-                    d1 = fmaf(t, s.rgbw[COUT + col0 + i], d1);
-                    d2 = fmaf(t, s.rgbw[2 * COUT + col0 + i], d2);
-                }
-            }
-            s.part[(half * 3 + 0) * TM + row_e] = d0;
-            s.part[(half * 3 + 1) * TM + row_e] = d1;
-            s.part[(half * 3 + 2) * TM + row_e] = d2;
-            fence_before_sync();
             __syncthreads();
             if (tid < TM) {
-                float sk[3];
-                upsampled_skip(a.img_in + (size_t)f * (a.H / 2) * (a.W / 2) * 3, a.H / 2, a.W / 2, y, x, sk);
+                const int x = x0 + tid;
+                if (LAYER == 0) {   // toRGB (+ bias, clamp) added to the rgb skip (networks_stylegan2.py:395-403, 462-466)
+                    const size_t pix = ((size_t)f * a.H + y) * a.W + x;
 #pragma unroll
-                for (int o = 0; o < 3; ++o) {
-                    float r = s.part[o * TM + tid] + s.part[(3 + o) * TM + tid] + __ldg(a.rgb_b + o);
-                    r = sk[o] + fminf(fmaxf(r, -256.f), 256.f);
-                    if (a.clamp01) r = fminf(fmaxf(r, 0.f), 1.f);
-                    a.img_out[(((size_t)f * 3 + o) * a.H + y) * a.W + x] = r;
+                    for (int o = 0; o < 3; ++o) {
+                        float r = s.part[o * TM + tid] + __ldg(a.rgb_b + o);
+                        r = fminf(fmaxf(r, -256.f), 256.f);
+                        a.img_out[pix * 3 + o] = __ldg(a.img_in + pix * 3 + o) + r;
+                    }
+                } else {
+                    float sk[3];
+                    upsampled_skip(a.img_in + (size_t)f * (a.H / 2) * (a.W / 2) * 3, a.H / 2, a.W / 2, y, x, sk);
+#pragma unroll
+                    for (int o = 0; o < 3; ++o) {
+                        float r = s.part[o * TM + tid] + __ldg(a.rgb_b + o);
+                        r = sk[o] + fminf(fmaxf(r, -256.f), 256.f);
+                        if (a.clamp01) r = fminf(fmaxf(r, 0.f), 1.f);
+                        a.img_out[(((size_t)f * 3 + o) * a.H + y) * a.W + x] = r;
+                    }
+                }
+            }
+        } else {
+            // N-block `nb` holds the phases (py = nb, px = column / 64): output pixels (2y + py, 2x + px), 64 channels each
+            const int Ho = 2 * a.H, Wo = 2 * a.W;
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb) {
+#pragma unroll
+                for (int i = 0; i < R; i += 2) {
+                    const int col = frag_col(i, lane), px = col >> 6, ch = col & 63;
+                    const int x = x0 + 64 * wg + frag_row(i, lane, wwarp), Y = 2 * y + nb, X = 2 * x + px;
+                    const size_t opix = ((size_t)f * Ho + Y) * Wo + X;
+                    const float nz = a.noise ? __ldg(a.noise + (size_t)f * a.noise_fstride + (size_t)Y * Wo + X) : 0.f;
+                    const float t0 = lrelu_clamp(d[nb][i] + nz + s.bias[ch]), t1 = lrelu_clamp(d[nb][i + 1] + nz + s.bias[ch + 1]);
+                    *reinterpret_cast<uint32_t *>(a.out + opix * COUT + ch) = pack2<false>(t0, t1);
                 }
             }
         }
-        // the next tile's first MMA overwrites the accumulator: it is issued after the __syncthreads of its first chunk,
-        // which every thread reaches only after its tcgen05.ld's above have completed (wait_ld) and been fenced
-        fence_before_sync();
     }
-
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // block0.conv0: 3 -> 128 channels.  One task = two horizontally adjacent pixels x 16 output channels.  A warp takes ONE group of 16
 // channels for 32 neighbouring pixel pairs, so every shared-memory weight read is a broadcast (one 16-byte wavefront instead of eight:
-// the first version, which spread the eight channel groups over the lanes, was bound by exactly those reads -- ncu: L1TEX 96 %,
-// short-scoreboard 8.4 per issue); the eight warps of a CTA cover the eight channel groups of the same 64 pixels.
+// spreading the eight channel groups over the lanes instead makes those reads the bound); the eight warps of a CTA cover the eight channel groups of the same 64 pixels.
 __global__ void __launch_bounds__(256) k_sr_conv_in(const __grid_constant__ SrConvInArgs a) {
     __shared__ __align__(16) float sw[27 * 128];
     __shared__ float sb[128];
@@ -405,9 +347,7 @@ static cudaError_t launch_sr_conv_t(const SrConvArgs &a, cudaStream_t st) {
     if (e != cudaSuccess) return e;
     const int n_tiles = a.F * a.H * (a.W / TM);
     int per_sm = (int)((227 * 1024) / smem);                        // by shared memory
-    const int by_tmem = 512 / (sr_layer_nb(LAYER) * sr_layer_nrows(LAYER));
-    if (per_sm > by_tmem) per_sm = by_tmem;                          // a CTA that could not allocate TMEM would spin
-    if (per_sm > 2) per_sm = 2;                                      // the launch bound (registers)
+    if (per_sm > (LAYER == 1 ? 1 : 2)) per_sm = LAYER == 1 ? 1 : 2;  // the launch bound (registers)
     if (per_sm < 1) per_sm = 1;
     int blocks = sm_count() * per_sm;
     if (blocks > n_tiles) blocks = n_tiles;

@@ -6,7 +6,7 @@
 
 namespace gfpp {
 
-// One implicit-GEMM convolution layer on tcgen05 (k_sr_conv<LAYER>):
+// One implicit-GEMM convolution layer on wgmma (k_sr_conv<LAYER>):
 //   LAYER 0: block0.conv1  128 -> 128, 3x3, at HxW            (+ toRGB, + rgb skip -> img0)
 //   LAYER 1: block1.conv0  128 -> 64,  3x3 transposed stride 2 + FIR, merged into four 3x3 phase kernels: HxW -> 2Hx2W
 //   LAYER 2: block1.conv1   64 -> 64,  3x3, at HxW (= 512)    (+ toRGB, + 2x FIR up-sampled skip -> final image)

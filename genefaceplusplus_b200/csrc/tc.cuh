@@ -1,17 +1,19 @@
-// tc.cuh -- 5th-generation tensor-core (tcgen05) building blocks for the tiny-MLP GEMMs, sm_100a only.
+// tc.cuh -- Hopper tensor-core (wgmma) building blocks for the tiny-MLP GEMMs and the SR convolutions, sm_90a.
 //
-// D[128 x N] (fp32, in TMEM) += A[128 x K] (smem, K-major) * W[N x K]^T (smem, K-major), 16-bit operands
-// (fp16 or bf16, kind::f16), issued by ONE thread per CTA (tcgen05.mma), accumulators read back with
-// tcgen05.ld for the epilogue.  nn.Linear weights are [out, in] = [N, K] row-major, i.e. already K-major.
+// D[64 x N] (fp32, registers of one warpgroup) (+)= A[64 x K] (smem, K-major) * W[N x K]^T (smem, K-major), 16-bit
+// operands (fp16 or bf16), issued by the 128 threads of a warpgroup (wgmma.mma_async), completion awaited with
+// wgmma.commit_group / wait_group.  nn.Linear weights are [out, in] = [N, K] row-major, i.e. already K-major.
+// A 128-row operand tile is two M = 64 halves: half h starts 64 rows (8 KB of an SW128 tile, 2 KB of a K16 tile) further.
 //
-// Operand tiles in shared memory use the canonical UMMA K-major layouts (encodings cross-checked against the
-// CuTe headers shipped in the image: cute/arch/mma_sm100_desc.hpp, cute/atom/mma_traits_sm100.hpp:190-300):
+// Operand tiles in shared memory use the canonical GMMA K-major layouts:
 //   * SW128 tile: [rows x 64 elements], 128-byte rows, 8-row groups of 1024 B (SBO), 16-byte chunks XOR-swizzled
 //     with the row index (Swizzle<3,4,3>); tile base 1024-byte aligned.
 //   * K16 tile (no swizzle / "interleave"): [rows x 16 elements] as 8x16B core matrices: the two K-chunks of a
 //     group are 128 B apart (LBO), groups are 256 B apart (SBO).
+// Accumulator fragment of m64nNk16: register i of lane l in warp w (0..3) of the warpgroup holds row
+// 16w + l/4 + 8*((i>>1)&1), column 8*(i>>2) + 2*(l%4) + (i&1)  (frag_row / frag_col below).
 // "split" precision: x = hi + lo with hi = rn16(x), lo = rn16(x - hi); A*W ~= Ah*Wh + Ah*Wl + Al*Wh accumulated
-// in the same fp32 TMEM accumulator (3 MMAs per k-step) -- bf16x3 gives ~16 mantissa bits.
+// in the same fp32 accumulator (3 MMAs per k-step) -- bf16x3 gives ~16 mantissa bits.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -47,18 +49,6 @@ __device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t pari
             : "memory");
     } while (!ok);
 }
-// non-blocking: has the phase with this parity completed?
-__device__ __forceinline__ bool mbar_test(unsigned long long *bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
 // plain arrive (count 1) by the executing thread; release semantics at CTA scope
 __device__ __forceinline__ void mbar_arrive(unsigned long long *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -71,115 +61,81 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
 }
 // generic-proxy smem writes -> visible to the async proxy (tensor core / TMA reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// ---- TMEM ----
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_dst, uint32_t ncols) {  // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {    // the same warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 16 consecutive fp32 columns -> 16 registers per thread (thread t of the warp reads lane base+t)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]),
-          "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]),
-          "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-        "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-        "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-        "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-                 "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-                 "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-                 : "memory");
-}
-
-// ---- descriptors ----
-// shared-memory matrix descriptor, SW128 K-major: SBO = 1024 B, LBO unused (=1), version 1, layout type 2
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-           ((uint64_t)2 << 61);
-}
-// no-swizzle K-major, K = 16 elements: LBO = 128 B (between the two 16-byte K chunks), SBO = 256 B (8-row groups)
-__device__ __forceinline__ uint64_t desc_k16(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46);
-}
-// instruction descriptor, kind::f16: D fp32, A/B both `fmt` (0 = fp16, 1 = bf16), both K-major, M = 128, N
-__host__ __device__ __forceinline__ uint32_t make_idesc(int fmt, int N) {
-    return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// same, accumulate flag known at compile time (no predicate set-up on the issue path)
-template <bool ACC>
-__device__ __forceinline__ void mma_f16_s(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc) {
-    if (ACC)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 0, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-                     "l"(a_desc), "l"(b_desc), "r"(idesc)
-                     : "memory");
-    else
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, 0, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-                     "l"(a_desc), "l"(b_desc), "r"(idesc)
-                     : "memory");
-}
 // one lane of a converged warp
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(unsigned long long *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// barrier of the 128 threads of one warpgroup (named barrier `id` > 0; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// ---- descriptors ----
+// shared-memory matrix descriptor (GMMA), SW128 K-major: SBO = 1024 B, LBO unused (=1), layout type 1 (128-byte swizzle)
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+// no-swizzle K-major, K = 16 elements: LBO = 128 B (between the two 16-byte K chunks), SBO = 256 B (8-row groups)
+__device__ __forceinline__ uint64_t desc_k16(uint32_t saddr) {
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32);
+}
+// byte offset of M-half `h` (rows 64h..64h+63) inside a 128-row operand tile
+constexpr uint32_t SW128_HALF = 8192, K16_HALF = 2048;
+
+// ---- wgmma (warpgroup-collective: all 128 threads, converged) ----
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the compiler from moving accumulator reads / writes across the asynchronous MMA window
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int R>
+__device__ __forceinline__ void acc_zero(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) d[i] = 0.f;
+}
+__device__ __forceinline__ int frag_row(int i, int lane, int wwarp) { return 16 * wwarp + (lane >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int i, int lane) { return 8 * (i >> 2) + 2 * (lane & 3) + (i & 1); }
+
+// D[64 x N] (+)= A * W^T, one k-step of 16; `acc` = 0: D = A * W^T
+template <int N, bool BF16>
+__device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc);
+#define GFPP_ACC8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+#define GFPP_WGMMA_N16(TY) \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\twgmma.mma_async.sync.aligned.m64n16k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}" \
+                 : GFPP_ACC8(0) : "l"(da), "l"(db), "r"(acc))
+template <> __device__ __forceinline__ void wgmma<16, false>(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N16("f16"); }
+template <> __device__ __forceinline__ void wgmma<16, true>(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N16("bf16"); }
+#undef GFPP_WGMMA_N16
+#define GFPP_WGMMA_N64(TY) \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}" \
+                 : GFPP_ACC8(0), GFPP_ACC8(8), GFPP_ACC8(16), GFPP_ACC8(24) : "l"(da), "l"(db), "r"(acc))
+template <> __device__ __forceinline__ void wgmma<64, false>(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N64("f16"); }
+template <> __device__ __forceinline__ void wgmma<64, true>(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N64("bf16"); }
+#undef GFPP_WGMMA_N64
+#define GFPP_WGMMA_N128(TY) \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}" \
+                 : GFPP_ACC8(0), GFPP_ACC8(8), GFPP_ACC8(16), GFPP_ACC8(24), GFPP_ACC8(32), GFPP_ACC8(40), GFPP_ACC8(48), GFPP_ACC8(56) : "l"(da), "l"(db), "r"(acc))
+template <> __device__ __forceinline__ void wgmma<128, false>(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N128("f16"); }
+template <> __device__ __forceinline__ void wgmma<128, true>(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N128("bf16"); }
+#undef GFPP_WGMMA_N128
+#define GFPP_WGMMA_N144(TY) \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\twgmma.mma_async.sync.aligned.m64n144k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, %72, %73, p, 1, 1, 0, 0;\n\t}" \
+                 : GFPP_ACC8(0), GFPP_ACC8(8), GFPP_ACC8(16), GFPP_ACC8(24), GFPP_ACC8(32), GFPP_ACC8(40), GFPP_ACC8(48), GFPP_ACC8(56), GFPP_ACC8(64) : "l"(da), "l"(db), "r"(acc))
+template <> __device__ __forceinline__ void wgmma<144, false>(float (&d)[72], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N144("f16"); }
+template <> __device__ __forceinline__ void wgmma<144, true>(float (&d)[72], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N144("bf16"); }
+#undef GFPP_WGMMA_N144
+#undef GFPP_ACC8
+// all k-steps of one SW128 K-tile (ksteps x 16 elements); `acc_first` = 0 starts a new accumulation
+template <int N, bool BF16>
+__device__ __forceinline__ void wgmma_sw(float (&d)[N / 2], uint32_t a, uint32_t w, int ksteps, uint32_t acc_first) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        if (k < ksteps) wgmma<N, BF16>(d, desc_sw128(a + (uint32_t)k * 32u), desc_sw128(w + (uint32_t)k * 32u), (k > 0) ? 1u : acc_first);
 }
 
 // ---- operand tile addressing (byte offsets inside a tile) ----
@@ -221,26 +177,13 @@ __device__ __forceinline__ void store_chunk(unsigned char *hi_tile, unsigned cha
         *reinterpret_cast<uint4 *>(lo_tile + off) = l;
     }
 }
-
-// Issue the MMAs of one K-tile (ksteps x 16 elements): D (+)= A_tile * W_tile^T, optionally with the split terms.
-// a_* / w_* are shared-memory byte addresses of SW128 tiles (or K16 tiles when `k16` is set: then ksteps == 1).
-__device__ __forceinline__ void issue_ktile(uint32_t d_tmem, uint32_t a_hi, uint32_t a_lo, uint32_t w_hi, uint32_t w_lo,
-                                            int ksteps, bool k16, bool split, uint32_t idesc, bool first_accumulates) {
-    for (int k = 0; k < ksteps; ++k) {
-        const uint32_t adv = (uint32_t)k * 32u;  // 16 elements x 2 B inside the 128-byte swizzle row
-        const uint64_t ah = k16 ? desc_k16(a_hi) : desc_sw128(a_hi + adv);
-        const uint64_t wh = k16 ? desc_k16(w_hi) : desc_sw128(w_hi + adv);
-        const uint32_t acc0 = (first_accumulates || k > 0) ? 1u : 0u;
-        if (split) {
-            const uint64_t al = k16 ? desc_k16(a_lo) : desc_sw128(a_lo + adv);
-            const uint64_t wl = k16 ? desc_k16(w_lo) : desc_sw128(w_lo + adv);
-            mma_f16(d_tmem, al, wh, idesc, acc0);   // small terms first
-            mma_f16(d_tmem, ah, wl, idesc, 1u);
-            mma_f16(d_tmem, ah, wh, idesc, 1u);
-        } else {
-            mma_f16(d_tmem, ah, wh, idesc, acc0);
-        }
-    }
+// two consecutive K values (an accumulator pair) -> 4 bytes of the hi tile (and of the lo tile when SPLIT) at column `col`
+// of row `row` of an SW128 tile
+template <bool BF16, bool SPLIT>
+__device__ __forceinline__ void store_pair(unsigned char *hi_tile, unsigned char *lo_tile, int row, int col, float a, float b) {
+    const uint32_t off = sw128_off(row, col >> 3) + (uint32_t)(col & 7) * 2u;
+    *reinterpret_cast<uint32_t *>(hi_tile + off) = pack2<BF16>(a, b);
+    if (SPLIT) *reinterpret_cast<uint32_t *>(lo_tile + off) = pack2<BF16>(a - round16<BF16>(a), b - round16<BF16>(b));
 }
 
 }  // namespace tc

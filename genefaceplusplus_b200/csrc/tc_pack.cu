@@ -1,4 +1,4 @@
-// tc_pack.cu -- weight repacking for the tcgen05 path + a one-tile GEMM self-test of the tcgen05 plumbing.
+// tc_pack.cu -- weight repacking for the wgmma path + a one-tile GEMM self-test of the wgmma plumbing.
 #include "launch.cuh"
 #include "tc.cuh"
 
@@ -6,7 +6,7 @@ namespace gfpp {
 
 using namespace tc;
 
-// One K-tile of nn.Linear weights W[.][ld] (fp32) -> 16-bit hi (and lo) tiles in the UMMA K-major layout, ready to be
+// One K-tile of nn.Linear weights W[.][ld] (fp32) -> 16-bit hi (and lo) tiles in the GMMA K-major layout, ready to be
 // bulk-copied into shared memory: tile row dst_row0+n, column k  <-  W[row0+n][col0+k] for n < N, k < kc.
 // The destination must be zero-initialised (padding rows / columns stay zero).
 __global__ void k_pack_tc_tile(const float *__restrict__ W, int ld, int row0, int col0, int N, int kc, int dst_row0,
@@ -35,16 +35,52 @@ cudaError_t launch_pack_tc_tile(const float *W, int ld, int row0, int col0, int 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Self-test: out[128][N] = A[128][K] * W[N][K]^T through exactly the tile layouts, descriptors, MMA issue, commit and
-// TMEM read-back the fused kernel uses.  K = 64*nt64 (+16 when k16_tail); the weight tiles come pre-packed.
+// Self-test: out[128][N] = A[128][K] * W[N][K]^T through exactly the tile layouts, descriptors, wgmma issue and accumulator
+// fragment layout the fused kernels use (warpgroup g computes rows 64g..64g+63).  K = 64*nt64 (+16 when k16_tail); the weight
+// tiles come pre-packed.
 struct TcTestSmem {
     unsigned char a_hi[3][16384];
     unsigned char a_lo[3][16384];
     unsigned char w_hi[3][18432];
     unsigned char w_lo[3][18432];
-    unsigned long long bar_w, bar_acc;
-    uint32_t tmem_base;
+    unsigned long long bar_w;
 };
+
+template <int N, bool BF16, bool SPLIT>
+__device__ __forceinline__ void selftest_mma(TcTestSmem &s, int K, int nt64, int k16_tail, float *__restrict__ out) {
+    const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31, wwarp = (tid >> 5) & 3;
+    const int ntiles = nt64 + (k16_tail ? 1 : 0);
+    float d[N / 2];
+    acc_zero(d);
+    wg_fence();
+    for (int t = 0; t < ntiles; ++t) {
+        const bool is16 = k16_tail && t == nt64;
+        // a partial last 64-wide tile only holds (K - 64*t)/16 k-steps of defined operand data
+        const int k64 = K - (k16_tail ? 16 : 0);
+        const int ks = is16 ? 1 : ((k64 - 64 * t) >= 64 ? 4 : (k64 - 64 * t) / 16);
+        const uint32_t half = (uint32_t)wg * (is16 ? K16_HALF : SW128_HALF);
+        const uint32_t a_hi = smem_u32(s.a_hi[t]) + half, a_lo = smem_u32(s.a_lo[t]) + half;
+        const uint32_t w_hi = smem_u32(s.w_hi[t]), w_lo = smem_u32(s.w_lo[t]);
+        for (int k = 0; k < ks; ++k) {
+            const uint32_t adv = (uint32_t)k * 32u;   // 16 elements x 2 B inside the 128-byte swizzle row
+            const uint64_t ah = is16 ? desc_k16(a_hi) : desc_sw128(a_hi + adv), wh = is16 ? desc_k16(w_hi) : desc_sw128(w_hi + adv);
+            const uint32_t acc0 = (t > 0 || k > 0) ? 1u : 0u;
+            if (SPLIT) {
+                const uint64_t al = is16 ? desc_k16(a_lo) : desc_sw128(a_lo + adv), wl = is16 ? desc_k16(w_lo) : desc_sw128(w_lo + adv);
+                wgmma<N, BF16>(d, al, wh, acc0);   // small terms first
+                wgmma<N, BF16>(d, ah, wl, 1u);
+                wgmma<N, BF16>(d, ah, wh, 1u);
+            } else {
+                wgmma<N, BF16>(d, ah, wh, acc0);
+            }
+        }
+    }
+    wg_commit();
+    wg_wait<0>();
+    acc_fence(d);
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) out[(size_t)(64 * wg + frag_row(i, lane, wwarp)) * N + frag_col(i, lane)] = d[i];
+}
 
 template <bool BF16, bool SPLIT>
 __global__ void __launch_bounds__(256, 1) k_tc_selftest(const float *__restrict__ A, int K, const unsigned char *__restrict__ wt_hi,
@@ -53,18 +89,13 @@ __global__ void __launch_bounds__(256, 1) k_tc_selftest(const float *__restrict_
     extern __shared__ __align__(1024) unsigned char raw_[];
     unsigned char *raw = raw_ + ((1024u - (smem_u32(raw_) & 1023u)) & 1023u);  // SW128 tiles need 1024-byte alignment
     TcTestSmem &s = *reinterpret_cast<TcTestSmem *>(raw);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int ntiles = nt64 + (k16_tail ? 1 : 0);
-    if (warp == 0) tmem_alloc(&s.tmem_base, 256);
     if (tid == 32) {
         mbar_init(&s.bar_w, 1);
-        mbar_init(&s.bar_acc, 1);
         mbar_fence_init();
     }
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tmem = s.tmem_base;
     const uint32_t tile_bytes = 18432;
     if (tid == 0) {
         uint32_t bytes = 0;
@@ -90,39 +121,15 @@ __global__ void __launch_bounds__(256, 1) k_tc_selftest(const float *__restrict_
     }
     fence_async_smem();
     __syncthreads();
-    if (tid == 0) {
-        mbar_wait(&s.bar_w, 0);
-        fence_after_sync();
-        const uint32_t idesc = make_idesc(BF16 ? 1 : 0, N);
-        for (int t = 0; t < ntiles; ++t) {
-            const bool is16 = k16_tail && t == nt64;
-            // a partial last 64-wide tile only holds (K - 64*t)/16 k-steps of defined operand data
-            const int k64 = K - (k16_tail ? 16 : 0);
-            const int ks = is16 ? 1 : ((k64 - 64 * t) >= 64 ? 4 : (k64 - 64 * t) / 16);
-            issue_ktile(tmem, smem_u32(s.a_hi[t]), smem_u32(s.a_lo[t]), smem_u32(s.w_hi[t]), smem_u32(s.w_lo[t]), ks, is16,
-                        SPLIT, idesc, t > 0);
-        }
-        mma_commit(&s.bar_acc);
-    }
-    mbar_wait(&s.bar_acc, 0);
-    fence_after_sync();
-    if (tid < 128) {
-        const uint32_t lane_base = (uint32_t)(warp & 3) * 32u;
-        for (int c = 0; c < N / 16; ++c) {
-            float v[16];
-            tmem_ld16(tmem + (lane_base << 16) + (uint32_t)c * 16u, v);
-            wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) out[(size_t)tid * N + c * 16 + i] = v[i];
-        }
-    }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 256);
+    mbar_wait(&s.bar_w, 0);
+    if (N == 16) selftest_mma<16, BF16, SPLIT>(s, K, nt64, k16_tail, out);
+    else if (N == 128) selftest_mma<128, BF16, SPLIT>(s, K, nt64, k16_tail, out);
+    else selftest_mma<144, BF16, SPLIT>(s, K, nt64, k16_tail, out);
 }
 
 cudaError_t launch_tc_selftest(const float *A, int K, const unsigned char *wt_hi, const unsigned char *wt_lo, int N, int nt64,
                                int k16_tail, int precision, float *out, cudaStream_t st) {
+    if (N != 16 && N != 128 && N != 144) return cudaErrorInvalidValue;   // the MMA widths the kernels use
     const size_t smem = sizeof(TcTestSmem) + 1024;
     cudaError_t e;
 #define GO(BF, SP)                                                                                                     \

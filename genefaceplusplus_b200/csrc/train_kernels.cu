@@ -1,4 +1,4 @@
-// train_kernels.cu -- training-side native ops of modules/radnerfs (SURVEY.md 8(f) rank 4), sm_100a.
+// train_kernels.cu -- training-side native ops of modules/radnerfs (SURVEY.md 8(f) rank 4), sm_90a.
 //
 // Replaces, entry point for entry point (include/gfpp.h section D):
 //   march_rays_train / _backward              raymarching.cu:352-598

@@ -1,4 +1,4 @@
-"""B200 drop-ins for the reference's model API (SURVEY.md 8(b), "B-model").
+"""H100 drop-ins for the reference's model API (SURVEY.md 8(b), "B-model").
 
 `RADNeRF` / `RADNeRFTorso` here mirror modules/radnerfs/radnerf.py:13 and modules/radnerfs/radnerf_torso.py:17:
   * same constructor argument (the hparams dict), same parameter / buffer names and shapes, so
@@ -7,11 +7,11 @@
     max_steps, T_thresh, ..., **kwargs)` signature and result dict (renderer.py:286 / radnerf_torso.py:86),
     tolerant of every extra kwarg the driver passes (`staged`, `lm68`, all hparams keys);
   * same errors-as-exceptions behaviour.
-Everything under `render` runs in the fused sm_100a kernels of libgfpp.so through the C-ABI (include/gfpp.h).
+Everything under `render` runs in the fused sm_90a kernels of libgfpp.so through the C-ABI (include/gfpp.h).
 Only the tiny conditioning nets (AudioNet / AudioAttNet, cond_encoder.py:98-180: 5x204 -> 64) stay in PyTorch,
 as SURVEY.md 8(a) a4 prescribes.  Inference only: `self.training` raises (training is out of scope, SURVEY 2.1).
 
-`render_clip` is the B200-first entry point (SURVEY.md 8(f) rank 1): a whole clip of poses + conditioning is
+`render_clip` is the clip-level entry point (SURVEY.md 8(f) rank 1): a whole clip of poses + conditioning is
 rendered by a handful of persistent-kernel launches with rays generated in-kernel and frames kept on device.
 """
 import copy
@@ -178,8 +178,8 @@ class RADNeRF(nn.Module):
                     hp["num_layers_color"] == 2 and self.cond_out_dim == 64 and self.ambient_coord_dim in (2, 3))
         if not shape_ok:
             raise NotImplementedError("libgfpp kernels are built for the May architecture (hidden 128, 3/3/2 layers, cond 64)")
-        # arithmetic of the head MLP GEMMs (gfpp_model_desc.mlp_precision): "fp32" (CUDA-core FFMA), "fp16" (tcgen05, what the
-        # reference runs under autocast), "bf16x3" (tcgen05 hi/lo split, ~fp32 accuracy), "bf16" (tcgen05), "robust" (tcgen05 fp16
+        # arithmetic of the head MLP GEMMs (gfpp_model_desc.mlp_precision): "fp32" (CUDA-core FFMA), "fp16" (wgmma, what the
+        # reference runs under autocast), "bf16x3" (wgmma hi/lo split, ~fp32 accuracy), "bf16" (wgmma), "robust" (wgmma fp16
         # with the hi/lo split on the ambient net only + a 16-bit fixed-point position table: holds 1e-3 on well-conditioned scenes)
         self.mlp_precision = hparams.get("gfpp_mlp_precision", "fp32")
         self._packed = None  # (key, packed_dev, Model, keepalive)
@@ -600,10 +600,10 @@ class RADNeRFTorsowithSR(RADNeRF):
     upscale_torso=)` result dict.  The head NeRF runs in libgfpp's fused kernels at 256x256; this variant's torso field --
     2-D position (42) + code (8) + freq-encoded jaw landmarks (126) [+ a per-pixel 4->16->32->16 encoding of the head colour and
     alpha] -> deform 64-64-2 -> tiled 2-D grid -> canonical 32-32-4 -- and the three-way composite run in libgfpp's `k_torso_sr`
-    (csrc/torso_sr_kernel.cu, `torso_backend = "native"`), the SR head in libgfpp's tcgen05 convolution kernels (superres.py).
+    (csrc/torso_sr_kernel.cu, `torso_backend = "native"`), the SR head in libgfpp's wgmma convolution kernels (superres.py).
     `torso_backend = "torch"` keeps the first correct path -- the field as host-side PyTorch over libgfpp's per-op encoder kernels --
     as the A/B reference of the kernel; it is also what the CPU test drives with the encoders injected from the checker
-    (tests/golden/torso_sr256.npz).  On the B200 both are pinned against the reference's own render() golden."""
+    (tests/golden/torso_sr256.npz).  On the GPU both are pinned against the reference's own render() golden."""
     has_torso = False            # what gets packed for libgfpp is the head field only
     forwards_eye_area = True     # radnerf_torso_sr.py:136
     sr_input_resolution = 256

@@ -19,8 +19,8 @@ the reference's code:
 
 Two implementations live behind `Superresolution.forward`:
 
-  * CUDA tensors, `backend == "native"` (the default): libgfpp's hand-written sm_100a kernels (csrc/sr_kernel.cu through
-    gfpp_sr_pack / gfpp_sr_forward): one fp32 FFMA kernel for the 3-channel input layer and three implicit-GEMM tcgen05
+  * CUDA tensors, `backend == "native"` (the default): libgfpp's hand-written sm_90a kernels (csrc/sr_kernel.cu through
+    gfpp_sr_pack / gfpp_sr_forward): one fp32 FFMA kernel for the 3-channel input layer and three implicit-GEMM wgmma
     kernels with fused noise / bias / leaky-ReLU / clamp / toRGB / skip epilogues; fp16 operands with fp32 accumulation
     (the reference switches these blocks to fp16 on CUDA), toRGB and the skip path fp32.  `folded_weights()` is the host
     half of that path: it folds modulation, demodulation and -- for the up-sampling layer -- the transposed stride-2
@@ -147,7 +147,7 @@ class _Block(nn.Module):
 class Superresolution(nn.Module):
     """radnerf_sr.py:15-48.  forward(rgb [B,3,h,w] in [0,1]) -> [B,3,512,512] (not clamped; the caller clamps)."""
 
-    backend = "native"   # CUDA tensors: libgfpp's sm_100a kernels; "torch": the fp32 convolutions below (always on CPU tensors)
+    backend = "native"   # CUDA tensors: libgfpp's sm_90a kernels; "torch": the fp32 convolutions below (always on CPU tensors)
 
     def __init__(self, channels=3, img_resolution=512, sr_antialias=True):
         super().__init__()
@@ -263,7 +263,7 @@ class Superresolution(nn.Module):
     @torch.no_grad()
     def forward_native(self, rgb_flat, noise_mode="random", clamp=False, out=None, frames_per_call=8, noise_planes=None):
         """rgb_flat [F, R*R, 3] fp32 CUDA in [0,1] (the layout the renderer writes `rgb_map` in), R = 256 -> [F,3,2R,2R]
-        through libgfpp's sm_100a kernels (4 launches per chunk of frames).  `noise_planes`: optional list of four tensors
+        through libgfpp's sm_90a kernels (4 launches per chunk of frames).  `noise_planes`: optional list of four tensors
         ([res,res] shared by all frames or [F,res,res]; None entries = no noise), already multiplied by the layers'
         noise_strength, instead of drawing them here (tests; callers that want reproducible 'random' noise)."""
         from . import _capi

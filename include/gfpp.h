@@ -1,5 +1,5 @@
 /*
- * gfpp.h -- C-ABI of libgfpp.so: the B200 (sm_100a) render hot path of GeneFace++.
+ * gfpp.h -- C-ABI of libgfpp.so: the H100 (sm_90a) render hot path of GeneFace++.
  *
  * Drop-in boundary (SURVEY.md section 8(b)).  Plain pointers and sizes only; no torch types.
  * All pointers are DEVICE pointers unless the name ends in _host.  Every call is
@@ -133,9 +133,9 @@ typedef struct {
     float density_thresh_torso;         /* min(density_thresh_torso, mean_density_torso) as the reference evaluates it */
     float torso_shrink;
     uint32_t torso_code_dim;            /* 8 */
-    /* arithmetic of the head MLP GEMMs: 0 = fp32 FFMA (CUDA cores), 1 = fp16 operands on tcgen05 tensor cores with
-     * fp32 accumulation (what the reference runs under autocast), 2 = bf16 hi/lo split x3 on tcgen05 (~fp32 accuracy),
-     * 3 = bf16 x1, 4 = "robust": fp16 on tcgen05 with the hi/lo split (3 MMAs per k-step, ~22 mantissa bits) on the ambient
+    /* arithmetic of the head MLP GEMMs: 0 = fp32 FFMA (CUDA cores), 1 = fp16 operands on wgmma tensor cores with
+     * fp32 accumulation (what the reference runs under autocast), 2 = bf16 hi/lo split x3 on wgmma (~fp32 accuracy),
+     * 3 = bf16 x1, 4 = "robust": fp16 on wgmma with the hi/lo split (3 MMAs per k-step, ~22 mantissa bits) on the ambient
      * net only and a 16-bit fixed-point position table -- the two roundings the field amplifies; holds 1e-3 max-abs on
      * well-conditioned (trained-like) scenes where plain fp16 does not.  Modes 1 and 4 run the row-owner kernel
      * (head_v2_kernel.cu).  Everything else (marching, compositing, torso) is fp32 in every mode. */
@@ -203,9 +203,9 @@ GFPP_API int gfpp_profile_read(float ms[4]);   /* ms[3] = everything before the 
 /* optional: device buffer of 32 uint64 that the tensor-core head kernel fills with per-phase cycle totals (thread 0 of each
  * CTA; slot 31 = batches processed); NULL switches it off.  Diagnostics only. */
 GFPP_API int gfpp_profile_phases(void *dev_u64x32);
-/* Self-test of the tcgen05 plumbing (tile layouts, descriptors, MMA issue, TMEM read-back) used by the tensor-core MLP:
- * out[128,N] = A[128,K] @ W[N,K]^T with 16-bit operands, fp32 accumulation.  K = 64*j (+16 if k16_tail), N % 16 == 0,
- * N <= 144, K <= 144.  precision: 1 = fp16, 2 = bf16 hi/lo split (3 MMAs), 3 = bf16.  scratch: >= 6*18432 bytes. */
+/* Self-test of the wgmma plumbing (tile layouts, descriptors, MMA issue, accumulator fragment read-back) used by the tensor-core MLP:
+ * out[128,N] = A[128,K] @ W[N,K]^T with 16-bit operands, fp32 accumulation.  K = 64*j (+16 if k16_tail), N in {16, 128, 144}
+ * (the MMA widths the kernels use), K <= 144.  precision: 1 = fp16, 2 = bf16 hi/lo split (3 MMAs), 3 = bf16.  scratch: >= 6*18432 bytes. */
 GFPP_API int gfpp_tc_selftest(const float *A, const float *W, uint32_t N, uint32_t K, int k16_tail, int precision,
                               void *scratch, float *out, void *stream);
 /* Debug / test hook: write out the rays the fused path generates IN-KERNEL from poses + intrinsics (pixel centres, normalised,

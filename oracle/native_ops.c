@@ -5,11 +5,11 @@
  * yerfor/GeneFacePlusPlus: the six inference ops and (second half of the file) the training-side ones.  The reference ships these ops as
  * CUDA only (its Python wrappers force .cuda()); there is no CPU implementation and
  * the reference has no tests or golden vectors for them, so this file is the CPU
- * checker ("oracle") that the B200 kernels are compared against.  It is pinned by
+ * checker ("oracle") that the GPU kernels are compared against.  It is pinned by
  *   (i)  the reference's own PyTorch modules driven on CPU through these functions
  *        (oracle/validate_against_reference.py, run where /root/reference exists), and
  *   (ii) the reference's own CUDA kernels compiled unmodified into oracle/_ref and
- *        run on the B200 box (tests/test_gpu_ref_pin.py).
+ *        run on the GPU (tests/test_gpu_ref_pin.py).
  *
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
  * legs may load this library.  The product path never does.
@@ -359,7 +359,7 @@ ORC_API void orc_linear(const float *x, const float *W, float *y, uint32_t M, ui
 
 /* ==================================================================================================
  * Training-side ops (SURVEY.md 8(f) rank 4): CPU restatement of the reference's training kernels.
- * Parity of these is pinned on the B200 against the reference's own kernels (tests/test_gpu_ref_pin.py).
+ * Parity of these is pinned on the GPU against the reference's own kernels (tests/test_gpu_ref_pin.py).
  * ================================================================================================== */
 
 /* one marching pass of kernel_march_rays_train (raymarching.cu:397-443 count, :464-517 write): walks ray n from t0 and

@@ -9,7 +9,7 @@ Runs only where /root/reference exists (this container; never on the GPU box).  
   4. compares with oracle.render.OracleModel.render on the same inputs.
 Both sides share the native-op restatement, so (3) vs (4) pins the *host* logic the oracle restates
 (round loop, MLP wiring, cond nets, torso composite); the native ops themselves are pinned on the
-B200 against the reference's own CUDA kernels (tests/test_gpu_ref_pin.py).
+GPU against the reference's own CUDA kernels (tests/test_gpu_ref_pin.py).
 
 Usage:  python -m oracle.validate_against_reference [--size 64] [--write-golden]
 """

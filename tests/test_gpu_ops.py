@@ -1,4 +1,4 @@
-"""Per-op parity on the B200: every (A)-level entry point of the C-ABI vs the C oracle on the same inputs.
+"""Per-op parity on the GPU: every (A)-level entry point of the C-ABI vs the C oracle on the same inputs.
 
 Integer / discrete results (near/far, marched positions, which rows are written, alive flags) must be
 bit-exact; smooth fp32 results within 2e-6 relative (different FMA contraction only)."""
@@ -35,7 +35,7 @@ def rays():
     return sc, fi["rays_o"].view(-1, 3).contiguous(), fi["rays_d"].view(-1, 3).contiguous()
 
 
-def test_device_is_blackwell():
+def test_device_is_hopper():
     _capi.check(_capi.lib().gfpp_check_device(), "check_device")
 
 

@@ -1,5 +1,5 @@
 """Second oracle pin: the REFERENCE'S OWN CUDA kernels (compiled unmodified from /root/reference into oracle/_ref by
-oracle/build_ref.py; the .so files travel to the GPU box) vs the C restatement oracle/native_ops.c, op by op, on the B200.
+oracle/build_ref.py; the .so files stay beside the tree) vs the C restatement oracle/native_ops.c, op by op, on the GPU.
 
 What may differ and why (SURVEY.md H2/H6): nvcc contracts a*b+c into FMA in the reference build while the oracle is
 unfused, and the reference uses __expf/__sinf.  So positions are compared exactly where the arithmetic is discrete-safe

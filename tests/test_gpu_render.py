@@ -1,4 +1,4 @@
-"""Fused renderer parity on the B200 (through the reference-shaped render() API and the C-ABI).
+"""Fused renderer parity on the GPU (through the reference-shaped render() API and the C-ABI).
 
 Bar (BASELINE.json north_star): rgb / alpha within 1e-3 max-abs fp32 and PSNR >= 50 dB against the CPU oracle on
 identical rays and conditioning.  The tolerance is written here: TOL = 1e-3, PSNR_MIN = 50.

@@ -1,4 +1,4 @@
-"""Tensor-core (tcgen05) MLP variants of the fused renderer vs the fp32 CPU oracle.
+"""Tensor-core (wgmma) MLP variants of the fused renderer vs the fp32 CPU oracle.
 
 Which precision passes the 1e-3 bar depends on how well-conditioned the scene is (DESIGN.md "precision"):
   * SURVEY.md 8(d) default-init scene (the BASELINE bench scene): every mode passes, fp16 with a 40x margin;

@@ -1,7 +1,6 @@
 """GPU runs of the SR-variant drop-ins (SURVEY 8(f) rank 3) against the reference goldens: `RADNeRFwithSR` / `RADNeRFTorsowithSR`
 with the head field in libgfpp's fused kernels at 256x256 and the SR head (and, for the torso-SR variant, its torso field and
-composite) as host-side PyTorch over libgfpp's per-op encoder kernels.  First run on a B200 in round 2: max |gpu - reference| =
-4.7e-4 on `sr_rgb_map` (82.6 dB), 3e-7 / 8e-6 on the 256x256 maps (gpurun_out/pending/sr_pending.log, profiles/sr_gpu_r02.txt).
+composite) as host-side PyTorch over libgfpp's per-op encoder kernels.
 The CPU halves of these checks run in tests/test_host_logic.py and tests/test_oracle_golden.py."""
 import json
 import os

@@ -1,4 +1,4 @@
-"""tcgen05 plumbing self-test: one 128 x N x K GEMM through the exact tile layouts / descriptors / TMEM read-back of
+"""wgmma plumbing self-test: one 128 x N x K GEMM through the exact tile layouts / descriptors / accumulator fragment read-back of
 the tensor-core MLP, against a float64 reference with operands rounded the way the kernel rounds them."""
 import ctypes
 

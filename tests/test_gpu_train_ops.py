@@ -1,4 +1,4 @@
-"""Training-side native ops of libgfpp (csrc/train_kernels.cu; SURVEY 8(f) rank 4) on the B200:
+"""Training-side native ops of libgfpp (csrc/train_kernels.cu; SURVEY 8(f) rank 4) on the GPU:
   * against the C checker (oracle/native_ops.c, second half) through the wrapper-level API genefaceplusplus_b200/train_ops.py;
   * checker AND libgfpp against the REFERENCE'S OWN training kernels (oracle/_ref, compiled unmodified), ray by ray: the
     reference hands out point offsets in atomicAdd arrival order, so layouts are compared through each implementation's `rays`

@@ -3,7 +3,7 @@
 The reference ships these ops as CUDA only and has no tests for them, so the restatement is pinned here through properties that
 do not need the reference: the train marcher against the (reference-pinned) inference marcher, compositing backward against
 autograd of the rendering formula, the grid backward as the exact adjoint of the (reference-pinned) forward, dy_dx against finite
-differences, Morton / bit-packing identities.  On the B200 the same functions are pinned against the reference's own kernels
+differences, Morton / bit-packing identities.  On the GPU the same functions are pinned against the reference's own kernels
 (tests/test_gpu_train_ops.py)."""
 import numpy as np
 import pytest

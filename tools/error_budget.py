@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Error budget of the head MLP precision modes on the CPU oracle (no GPU needed).
 
-Emulates, one site at a time, the roundings the tcgen05 modes introduce -- 16-bit grid tables, 16-bit A operands
+Emulates, one site at a time, the roundings the wgmma modes introduce -- 16-bit grid tables, 16-bit A operands
 (activations), 16-bit W operands (weights), per layer -- inside oracle/render.py's field query and reports the max-abs RGB
 error of the rendered frame against the untouched fp32 oracle.  This is how the "robust" mode was chosen (DESIGN.md
 "precision"): the site that dominates gets the hi/lo split, the others stay single 16-bit images.

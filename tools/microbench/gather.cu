@@ -5,7 +5,7 @@
 // same access pattern with nothing else in the way, so the phase time measured in the kernel (tools/phase_breakdown.py)
 // can be compared with what the memory system gives when asked nicely.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench/gather.bin tools/microbench/gather.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench/gather.bin tools/microbench/gather.cu
 //   tools/microbench/gather.bin            # prints one line per configuration
 //
 // Reported per configuration: cycles per "phase" (= one round of K loads per thread, all threads of the SM), sectors per

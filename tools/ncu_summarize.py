@@ -1,4 +1,4 @@
-"""Turn ncu output into the text summaries kept under profiles/.
+"""Turn ncu output into text summaries.
 
   python tools/ncu_summarize.py launches <launches.csv>          # per-kernel totals/shares of a `--metrics gpu__time_duration.sum` list
   python tools/ncu_summarize.py full <report.ncu-rep>            # the metrics DESIGN.md quotes from one `--set full` capture

@@ -15,12 +15,14 @@ m.render_clip(poses, sc.intrinsics,512,512,**kw); torch.cuda.synchronize()
 _capi.lib().gfpp_profile_phases(None)
 v = buf.cpu().tolist(); nb = v[31]
 if not os.environ.get('GFPP_HEAD_V1') and prec in ('fp16', 'robust'):   # row-owner kernel: stamps of row 0 of slot 0 of every CTA
-    names2 = ['operand rows (pos feats, cond, SH)', 'fate + march + refill', 'wait amb L0', 'epi amb L0', 'wait amb L1', 'epi amb L1', 'wait amb out',
-              'tanh + ambient gather', 'prefetch pos levels 0-7', 'wait sig L0', 'epi sig L0', 'prefetch pos levels 8-15', 'wait sig L1', 'epi sig L1',
-              'wait sig L2', 'epi sig L2 (sigma + geo)', 'wait col L0', 'epi col L0', 'wait col out', 'sigmoid + composite + batch check']
-    tot = sum(v[:20])
+    # PH(i) index -> phase of csrc/head_v2_kernel.cu (6 and 16-18 are not stamped)
+    names2 = {0: 'operand rows (pos feats, cond, SH)', 1: 'fate + march + refill', 2: 'MMA + epi amb L0', 3: 'MMA + epi amb L1',
+              4: 'MMA amb out', 5: 'tanh', 7: 'ambient gather', 8: 'prefetch pos levels 0-7', 9: 'MMA + epi sig L0',
+              10: 'prefetch pos levels 8-15', 11: 'MMA + epi sig L1', 12: 'MMA + epi sig L2 (sigma + geo)', 13: 'MMA + epi col L0',
+              14: 'MMA col out', 15: 'sigmoid', 19: 'composite + batch check'}
+    tot = sum(v[i] for i in names2)
     print(f'precision {prec} (v2): batches of slot 0 {nb}, cycles per batch of one slot = {tot/nb:.0f}')
-    for n, c in zip(names2, v[:20]): print(f'  {n:28s} {c/nb:9.0f} cyc/batch  {100*c/tot:5.1f}%')
+    for i, n in names2.items(): print(f'  {n:32s} {v[i]/nb:9.0f} cyc/batch  {100*v[i]/tot:5.1f}%')
     sys.exit(0)
 tot=sum(v[:11])
 names=['refill+publish','pos gather+cond','MMA amb0','epi amb0','MMA amb1','epi amb1','narrow amb + tanh','amb gather','sigma net (3 MMA+3 epi)','color net (2 MMA + epi)','composite+march']

@@ -30,7 +30,7 @@ if world > 1:
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     dist.init_process_group("nccl", device_id=dev)
 pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-peak, bf16 = pk.get("hbm_gbs", 6650.0), pk.get("bf16_tflops_sustained", 1460.6)
+peak, bf16 = pk.get("hbm_gbs", 3350.0), pk.get("bf16_tflops_sustained", 989.0)
 n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
 sectors_per_sample = 2 * 16 * (1 if prec in ("fp16", "robust") else 2)
 L = _capi.lib()

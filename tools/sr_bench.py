@@ -1,5 +1,5 @@
-"""tools/sr_bench.py -- measurement of the SR-variant paths (SURVEY 8(f) rank 3) on one B200: frames/s of the clip APIs with every
-stage in libgfpp (head field at 256x256 with in-kernel rays, torso-SR field, SR head on tcgen05) beside the same clip with the SR
+"""tools/sr_bench.py -- measurement of the SR-variant paths (SURVEY 8(f) rank 3) on one H100: frames/s of the clip APIs with every
+stage in libgfpp (head field at 256x256 with in-kernel rays, torso-SR field, SR head on wgmma) beside the same clip with the SR
 head / torso field as host-side PyTorch (cuDNN), and the stages timed alone with CUDA events.  Prints JSON lines.
 
     python tools/sr_bench.py [--frames 64] [--reps 5] [--out gpurun_out/sr_bench.jsonl]
@@ -48,7 +48,7 @@ def measure(frames=64, reps=5):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = float(peaks.get("bf16_tflops_sustained", 1460.6))
+    peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))
     T = a.frames
     lines = []
     ov = {"with_sr": True, "add_eye_blink_cond": True, "eye_blink_dim": 4, "smo_win_size": 3}

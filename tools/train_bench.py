@@ -6,7 +6,7 @@ worth of marching, compositing forward + backward and grid-encoder backward on t
     python tools/train_bench.py [--size 256] [--reps 5]
 
 `measure()` is also what bench.py calls for the `train_ops` object of its JSON line.  Every call below uses exactly the argument
-lists tests/test_gpu_train_ops.py validated on the B200 (ours through the backend shims, the reference's through its pybind
+lists tests/test_gpu_train_ops.py validated on the GPU (ours through the backend shims, the reference's through its pybind
 modules)."""
 import argparse
 import json
