@@ -94,6 +94,7 @@ EXPORTS = [
     "gfpp_march_rays_train_scratch_bytes", "gfpp_march_rays_train", "gfpp_march_rays_train_backward", "gfpp_composite_rays_train_forward",
     "gfpp_composite_rays_train_backward", "gfpp_grid_encode_forward_dydx", "gfpp_grid_encode_backward", "gfpp_grad_total_variation",
     "gfpp_packbits", "gfpp_morton3D", "gfpp_morton3D_invert", "gfpp_morton3D_dilation", "gfpp_sph_from_ray",
+    "gfpp_density_query", "gfpp_density_grid_workspace_bytes", "gfpp_density_grid_update", "gfpp_mark_untrained_grid",
 ]
 
 
@@ -154,6 +155,12 @@ def lib():
         L.gfpp_morton3D_invert.argtypes = [P, c_u32, P, P]
         L.gfpp_morton3D_dilation.argtypes = [P, c_u32, c_u32, P, P]
         L.gfpp_sph_from_ray.argtypes = [P, P, c_f, c_u32, P, P]
+        c_d = ctypes.c_double
+        L.gfpp_density_query.argtypes = [ctypes.POINTER(Model), P, c_u32, P, P, P, P]
+        L.gfpp_density_grid_workspace_bytes.restype = c_size_t
+        L.gfpp_density_grid_workspace_bytes.argtypes = [c_u32, c_u32]
+        L.gfpp_density_grid_update.argtypes = [ctypes.POINTER(Model), P, P, c_f, c_f, P, P, P, P, c_size_t, P]
+        L.gfpp_mark_untrained_grid.argtypes = [P, c_u32, c_d, c_d, c_d, c_d, c_d, c_u32, c_u32, P, P]
         _lib = L
     return _lib
 

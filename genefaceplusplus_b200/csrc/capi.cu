@@ -51,6 +51,11 @@ cudaError_t launch_morton3D(const int *, uint32_t, int *, cudaStream_t);
 cudaError_t launch_morton3D_invert(const int *, uint32_t, int *, cudaStream_t);
 cudaError_t launch_morton3D_dilation(const float *, uint32_t, uint32_t, float *, cudaStream_t);
 cudaError_t launch_sph_from_ray(const float *, const float *, float, uint32_t, float *, cudaStream_t);
+// grid_kernels.cu
+uint32_t dilate_ema_blocks(uint32_t C, uint32_t H);
+cudaError_t launch_grid_refresh_tail(const float *, uint32_t, uint32_t, float, float, float *, double *, float *, float *, uint8_t *, int *,
+                                     cudaStream_t);
+cudaError_t launch_mark_untrained(const float *, uint32_t, float, float, const float *, const float *, uint32_t, uint32_t, float *, cudaStream_t);
 }  // namespace gfpp
 
 using namespace gfpp;
@@ -1122,6 +1127,147 @@ int gfpp_sph_from_ray(const float *rays_o, const float *rays_d, float radius, ui
     if (!rays_o || !rays_d || !coords) return fail(GFPP_ERR_INVALID, "sph_from_ray: null pointer%s");
     g_launches = 0;
     CK(launch_sph_from_ray(rays_o, rays_d, radius, N, coords, (cudaStream_t)stream));
+    return GFPP_OK;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------ (E) occupancy-grid maintenance (head_kernel.cu: k_density; grid_kernels.cu)
+namespace {
+
+bool grid_shape_ok(uint32_t C, uint32_t H) {
+    // Morton codes below H^3 decode to cells inside the grid only for a power-of-two H (the reference assumes one too)
+    return C >= 1 && C <= 8 && H >= 8 && H <= 512 && (H & (H - 1)) == 0 && (uint64_t)C * H * H * H <= (1ull << 30);
+}
+
+struct GridWork {
+    size_t tmp, partial, thresh, total;
+};
+
+GridWork grid_work_layout(uint32_t C, uint32_t H) {
+    GridWork W;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
+    W.tmp = take((size_t)C * H * H * H * 4);
+    W.partial = take((size_t)dilate_ema_blocks(C, H) * 8);
+    W.thresh = take(4);
+    W.total = o;
+    return W;
+}
+
+// the head field of a packed model, for k_density: fp32 weight chunks and fp32 tables (quads where the mode packed them)
+HeadArgs density_head_args(const ModelHost &m) {
+    HeadArgs a;
+    memset(&a, 0, sizeof(a));
+    a.pos_gm = m.pos_gm; a.amb_gm = m.amb_gm;
+    a.pos_tab = m.pos_tab; a.amb_tab = m.amb_tab;
+    a.pos_quads = m.pos_quads; a.amb_quads = m.amb_quads;
+    a.pos_octs = m.pos_octs; a.amb_octs = m.amb_octs;
+    a.wide = m.wide; a.narrow = m.narrow;
+    for (int c = 0; c < HEAD_NCHUNK; ++c) { a.chunk_off[c] = m.chunk_off[c]; a.chunk_k[c] = kChunkK[c]; }
+    return a;
+}
+
+// the field the model's mode renders where a query kernel for it exists: fp16 -> wgmma over the fp16 operand images and oct tables;
+// fp32 / bf16x3 / bf16 / robust -> the fp32 FFMA field (robust renders a split-precision approximation of it, DESIGN.md section 6)
+cudaError_t launch_density_for(const ModelHost &m, const DensityArgs &d, cudaStream_t st) {
+    const HeadArgs a = density_head_args(m);
+    if (m.mlp_precision == 1 && m.tc.w_hi && m.pos_octs && m.amb_octs) return launch_density_tc(a, m.tc, d, st);
+    return launch_density(a, d, st);
+}
+
+// per cascade c: bound_c = min(2^c, bound), hgs_c = bound_c / H in double as the reference's Python does (renderer.py:253-254, 171-172)
+void cascade_constants(double bound, uint32_t C, uint32_t H, float *scale, float *hgs, float *pad) {
+    for (uint32_t c = 0; c < 8; ++c) {
+        const double bc = c < C ? fmin(ldexp(1.0, (int)c), bound) : 0.0, h = bc / (double)H;
+        scale[c] = (float)(bc - h);
+        if (hgs) hgs[c] = (float)h;
+        if (pad) pad[c] = (float)(h * 2.0);
+    }
+}
+
+bool aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
+
+}  // namespace
+
+extern "C" {
+
+int gfpp_density_query(const gfpp_model *model, const float *xyzs, uint32_t n, const float *cond_feat, float *sigma, float *geo_feat,
+                       void *stream) {
+    if (!model || !xyzs || !cond_feat || !sigma) return fail(GFPP_ERR_INVALID, "density_query: null pointer%s");
+    ModelHost m;
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "density_query: model handle not initialised by gfpp_model_pack%s");
+    if (!aligned16(cond_feat) || (geo_feat && !aligned16(geo_feat)))
+        return fail(GFPP_ERR_INVALID, "density_query: cond_feat and geo_feat must be 16-byte aligned%s");
+    if (n >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "density_query: n must be < 2^31%s");
+    DensityArgs d;
+    memset(&d, 0, sizeof(d));
+    d.n = n; d.xyzs = xyzs; d.cond = cond_feat; d.bound = m.bound;
+    d.sigma = sigma; d.geo = geo_feat; d.out_scale = 1.0f;
+    g_launches = 0;
+    CK(launch_density_for(m, d, (cudaStream_t)stream));
+    return GFPP_OK;
+}
+
+size_t gfpp_density_grid_workspace_bytes(uint32_t cascade, uint32_t grid_size) {
+    return grid_shape_ok(cascade, grid_size) ? grid_work_layout(cascade, grid_size).total : 0;
+}
+
+int gfpp_density_grid_update(const gfpp_model *model, const float *cond_feat, const float *noise, float decay, float density_thresh,
+                             float *density_grid, float *mean_out, float *tmp_grid, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!model || !cond_feat || !noise || !density_grid || !mean_out || !workspace)
+        return fail(GFPP_ERR_INVALID, "density_grid_update: null pointer%s");
+    ModelHost m;
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "density_grid_update: model handle not initialised by gfpp_model_pack%s");
+    const uint32_t C = m.cascade, H = m.grid_size;
+    if (!grid_shape_ok(C, H))
+        return fail(GFPP_ERR_UNSUPPORTED, "density_grid_update: needs cascade 1..8, grid_size a power of two in 8..512, C*H^3 <= 2^30%s");
+    if (!aligned16(cond_feat) || !aligned16(density_grid) || (tmp_grid && !aligned16(tmp_grid)))
+        return fail(GFPP_ERR_INVALID, "density_grid_update: cond_feat, density_grid and tmp_grid must be 16-byte aligned%s");
+    const GridWork W = grid_work_layout(C, H);
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "density_grid_update: workspace too small%s");
+    cudaStream_t st = (cudaStream_t)stream;
+    char *ws = (char *)workspace;
+    float *tmp = tmp_grid ? tmp_grid : (float *)(ws + W.tmp);
+    const uint32_t H3 = H * H * H;
+    DensityArgs d;
+    memset(&d, 0, sizeof(d));
+    d.n = C * H3; d.cond = cond_feat; d.bound = m.bound;
+    d.grid_size = H; d.noise = noise;
+    cascade_constants((double)m.bound, C, H, d.cell_scale, d.hgs, nullptr);
+    d.sigma = tmp; d.out_scale = m.density_scale;
+    g_launches = 0;
+    CK(launch_density_for(m, d, st));
+    uint8_t *bits = const_cast<uint8_t *>(m.bitfield);
+    int nl = 0;
+    const cudaError_t et = launch_grid_refresh_tail(tmp, C, H, decay, density_thresh, density_grid, (double *)(ws + W.partial), mean_out,
+                                                    (float *)(ws + W.thresh), bits, &nl, st);
+    g_launches += nl;
+    if (et != cudaSuccess) return fail(GFPP_ERR_CUDA, "launch_grid_refresh_tail: %s", cudaGetErrorString(et));
+    // the packed model's derived occupancy, as gfpp_model_pack builds it: the next gfpp_render_frames marches the new grid
+    int *occ = const_cast<int *>(m.occ_bounds);
+    k_init_bounds<<<1, 32, 0, st>>>(occ);
+    CK(cudaGetLastError());
+    CK(launch_occupancy_bounds(bits, C * H3 / 8, H3, occ, st));
+    uint32_t *coarse = const_cast<uint32_t *>(m.coarse_bits);
+    CKN(cudaMemsetAsync(coarse, 0, (size_t)m.coarse_words * 4, st));
+    CK(launch_coarse_occupancy(bits, C, H, coarse, st));
+    return GFPP_OK;
+}
+
+int gfpp_mark_untrained_grid(const float *poses_c2w, uint32_t n_poses, double fx, double fy, double cx, double cy, double bound,
+                             uint32_t cascade, uint32_t grid_size, float *density_grid, void *stream) {
+    if (!poses_c2w || !density_grid) return fail(GFPP_ERR_INVALID, "mark_untrained_grid: null pointer%s");
+    if (!grid_shape_ok(cascade, grid_size))
+        return fail(GFPP_ERR_UNSUPPORTED, "mark_untrained_grid: needs cascade 1..8, grid_size a power of two in 8..512, C*H^3 <= 2^30%s");
+    if (n_poses == 0 || !(fx != 0.0) || !(fy != 0.0)) return fail(GFPP_ERR_INVALID, "mark_untrained_grid: no poses or zero focal length%s");
+    float scale[8], pad[8];
+    cascade_constants(bound, cascade, grid_size, scale, nullptr, pad);
+    g_launches = 0;
+    CK(launch_mark_untrained(poses_c2w, n_poses, (float)(cx / fx), (float)(cy / fy), scale, pad, cascade, grid_size, density_grid,
+                             (cudaStream_t)stream));
     return GFPP_OK;
 }
 

@@ -27,6 +27,14 @@ __device__ __forceinline__ uint32_t spread3(uint32_t v) {
 __device__ __forceinline__ uint32_t morton3(uint32_t x, uint32_t y, uint32_t z) {
     return spread3(x) | (spread3(y) << 1) | (spread3(z) << 2);
 }
+__device__ __forceinline__ uint32_t compact3(uint32_t x) {   // __morton3D_invert (raymarching.cu:74-81): one axis of a Morton code
+    x &= 0x49249249u;
+    x = (x | (x >> 2)) & 0xC30C30C3u;
+    x = (x | (x >> 4)) & 0x0F00F00Fu;
+    x = (x | (x >> 8)) & 0xFF0000FFu;
+    x = (x | (x >> 16)) & 0x0000FFFFu;
+    return x;
+}
 
 // ---------------------------------------------------------------------------------------------
 // Marching constants shared by the per-op kernel and the fused renderer.

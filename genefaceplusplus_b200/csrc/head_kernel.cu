@@ -89,8 +89,10 @@ struct WStream {
     uint32_t consumed;
 };
 
+// NC: chunks per batch -- the stream cycles through chunks 0..NC-1 (k_density stops before the colour net's chunks)
+template <int NC = HEAD_NCHUNK>
 __device__ __forceinline__ void issue_chunk(const HeadArgs &a, Smem &s, uint32_t seq) {
-    const uint32_t stage = seq % NSTAGE, id = seq % HEAD_NCHUNK;
+    const uint32_t stage = seq % NSTAGE, id = seq % NC;
     const uint32_t bytes = (uint32_t)a.chunk_k[id] * 128u * 4u;
     mbar_expect_tx(&s.bar[stage], bytes);
     bulk_g2s(s.W + stage * WCHUNK, a.wide + a.chunk_off[id], bytes, &s.bar[stage]);
@@ -132,7 +134,7 @@ __device__ __forceinline__ void ffma_chunk(float (&acc)[8][8], const float *__re
 }
 
 // One 128x128xK layer: consume `nchunks` chunks from the stream, then write act(acc + bias) to A[:, coff:coff+128].
-template <bool RELU>
+template <bool RELU, int NC = HEAD_NCHUNK>
 __device__ __forceinline__ void wide_layer(const HeadArgs &a, Smem &s, WStream &ws, int nchunks, int coff,
                                            const float *bias, int tid) {
     const int ty = tid >> 4, tx = tid & 15;
@@ -143,14 +145,14 @@ __device__ __forceinline__ void wide_layer(const HeadArgs &a, Smem &s, WStream &
         for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
     int kbase = 0;
     for (int c = 0; c < nchunks; ++c) {
-        const uint32_t seq = ws.consumed, stage = seq % NSTAGE, id = seq % HEAD_NCHUNK;
+        const uint32_t seq = ws.consumed, stage = seq % NSTAGE, id = seq % NC;
         const int kc = a.chunk_k[id];
         mbar_wait(&s.bar[stage], (seq / NSTAGE) & 1);
         ffma_chunk(acc, s.A, s.W + stage * WCHUNK, kbase, kc, ty, tx);
         kbase += kc;
         ws.consumed = seq + 1;
         __syncthreads();  // everyone is done with this stage (and, after the last chunk, with reading A)
-        if (tid == 0) issue_chunk(a, s, seq + NSTAGE);
+        if (tid == 0) issue_chunk<NC>(a, s, seq + NSTAGE);
     }
     float bv[8];
 #pragma unroll
@@ -372,6 +374,161 @@ __global__ void __launch_bounds__(HEAD_NT, 1) k_head(const __grid_constant__ Hea
         const uint32_t seq = wst.consumed + q;
         mbar_wait(&s.bar[seq % NSTAGE], (seq / NSTAGE) & 1);
     }
+}
+
+// Density query (radnerf.py:143-166): position grid -> ambient net -> tanh -> ambient grid -> sigma net, 128 points per batch,
+// the same shared-memory FFMA tile GEMMs and weight stream as k_head, but the stream stops after the sigma net (7 chunks, or 9
+// when the 128 geo columns of its last layer are wanted).  Persistent CTAs take batches round-robin; nothing is marched.
+// In cell mode a batch is 128 consecutive Morton codes, i.e. a 4x4x8 brick, so a warp's corner gathers share sectors.
+template <bool GEO>
+__global__ void __launch_bounds__(HEAD_NT, 1) k_density(const __grid_constant__ HeadArgs a, const __grid_constant__ DensityArgs d) {
+    constexpr int NC = GEO ? 9 : 7;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    Smem &s = *reinterpret_cast<Smem *>(smem_raw);
+    const int tid = threadIdx.x;
+    for (int i = tid; i < 4 * 128; i += NT) s.narrow[i] = a.narrow[i];   // ambient out rows 0-2, sigma row
+    if (tid == 0) {
+        for (int i = 0; i < NSTAGE; ++i) mbar_init(&s.bar[i], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (tid == 0)
+        for (uint32_t q = 0; q < NSTAGE; ++q) issue_chunk<NC>(a, s, q);
+    WStream wst;
+    wst.consumed = 0;
+
+    const uint32_t n_batches = (d.n + TM - 1) / TM;
+    const uint32_t H = d.grid_size, H3 = H * H * H;
+    const int slot = tid & (TM - 1), lg = tid >> 7;
+    for (uint32_t b = blockIdx.x; b < n_batches; b += gridDim.x) {
+        if (tid < TM) {
+            float q[3];
+            const bool v = density_point(d, b * TM + tid, H, H3, q);
+            const float x = q[0], y = q[1], z = q[2];
+            s.valid[tid] = v ? 1 : 0;
+            s.sx[tid] = x; s.sy[tid] = y; s.sz[tid] = z;
+        }
+        __syncthreads();
+        const bool v = s.valid[slot] != 0;
+        // ---- position grid -> A[:, 0:32] (+ copy in P); conditioning -> A[:, 32:96] (as k_head) ----
+        {
+            float *ar = s.A + slot * LDA, *pr = s.P + slot * LDP;
+            if (v) {
+                const float inv2b = 2.0f * d.bound;
+                const float u = __fdiv_rn(__fadd_rn(s.sx[slot], d.bound), inv2b);
+                const float vv = __fdiv_rn(__fadd_rn(s.sy[slot], d.bound), inv2b);
+                const float w = __fdiv_rn(__fadd_rn(s.sz[slot], d.bound), inv2b);
+#pragma unroll 2
+                for (int l = lg * 8; l < lg * 8 + 8; ++l) {
+                    const float2 f = a.pos_quads ? grid_lookup3q(a.pos_gm, a.pos_quads, l, u, vv, w) : grid_lookup3(a.pos_gm, a.pos_tab, l, u, vv, w);
+                    *reinterpret_cast<float2 *>(ar + 2 * l) = f;
+                    *reinterpret_cast<float2 *>(pr + 2 * l) = f;
+                }
+            } else {
+                for (int l = lg * 8; l < lg * 8 + 8; ++l) {
+                    *reinterpret_cast<float2 *>(ar + 2 * l) = make_float2(0.f, 0.f);
+                    *reinterpret_cast<float2 *>(pr + 2 * l) = make_float2(0.f, 0.f);
+                }
+            }
+            const float4 *cf = reinterpret_cast<const float4 *>(d.cond + lg * 32);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) *reinterpret_cast<float4 *>(ar + 32 + lg * 32 + 4 * j) = __ldg(cf + j);
+        }
+        __syncthreads();
+
+        // ---- ambient net 96 -> 128 -> 128 -> 3, tanh ----
+        wide_layer<true, NC>(a, s, wst, 2, 0, nullptr, tid);
+        wide_layer<true, NC>(a, s, wst, 2, 0, nullptr, tid);
+        {
+            float o[3];
+            narrow_dot<3>(s, s.narrow, tid, o);
+            if ((tid & 1) == 0) {
+                const int row = tid >> 1;
+                s.amb[row] = tanhf(o[0]);
+                s.amb[TM + row] = tanhf(o[1]);
+                s.amb[2 * TM + row] = tanhf(o[2]);
+            }
+        }
+        __syncthreads();
+        // ---- ambient grid -> A[:, 32:64]; A[:, 0:32] <- position features ----
+        {
+            float *ar = s.A + slot * LDA;
+            const float *pr = s.P + slot * LDP;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                *reinterpret_cast<float4 *>(ar + lg * 16 + 4 * j) = *reinterpret_cast<const float4 *>(pr + lg * 16 + 4 * j);
+            if (v) {
+                const float u = __fdiv_rn(__fadd_rn(s.amb[slot], 1.0f), 2.0f);
+                const float vv = __fdiv_rn(__fadd_rn(s.amb[TM + slot], 1.0f), 2.0f);
+                const float w = __fdiv_rn(__fadd_rn(s.amb[2 * TM + slot], 1.0f), 2.0f);
+#pragma unroll 2
+                for (int l = lg * 8; l < lg * 8 + 8; ++l) {
+                    const float2 f = (a.amb_gm.dim == 3) ? (a.amb_quads ? grid_lookup3q(a.amb_gm, a.amb_quads, l, u, vv, w) : grid_lookup3(a.amb_gm, a.amb_tab, l, u, vv, w))
+                                                         : grid_lookup2(a.amb_gm, a.amb_tab, l, u, vv);
+                    *reinterpret_cast<float2 *>(ar + 32 + 2 * l) = f;
+                }
+            } else {
+                for (int l = lg * 8; l < lg * 8 + 8; ++l) *reinterpret_cast<float2 *>(ar + 32 + 2 * l) = make_float2(0.f, 0.f);
+            }
+        }
+        __syncthreads();
+
+        // ---- sigma net 64 -> 128 -> 128 -> (1 + 128) ----
+        wide_layer<true, NC>(a, s, wst, 1, 0, nullptr, tid);
+        wide_layer<true, NC>(a, s, wst, 2, 0, nullptr, tid);
+        {
+            float o[1];
+            narrow_dot<1>(s, s.narrow + 3 * 128, tid, o);
+            const uint32_t p = b * TM + (tid >> 1);
+            // trunc_exp forward is plain exp (utils.py:36-41)
+            if ((tid & 1) == 0 && p < d.n) d.sigma[p] = __fmul_rn(expf(o[0]), d.out_scale);
+        }
+        if (GEO) {   // geo features h[1:129], no activation, straight from the accumulators
+            const int ty = tid >> 4, tx = tid & 15;
+            float acc[8][8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+                for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+            int kbase = 0;
+            for (int c = 0; c < 2; ++c) {
+                const uint32_t seq = wst.consumed, stage = seq % NSTAGE, id = seq % NC;
+                const int kc = a.chunk_k[id];
+                mbar_wait(&s.bar[stage], (seq / NSTAGE) & 1);
+                ffma_chunk(acc, s.A, s.W + stage * WCHUNK, kbase, kc, ty, tx);
+                kbase += kc;
+                wst.consumed = seq + 1;
+                __syncthreads();
+                if (tid == 0) issue_chunk<NC>(a, s, seq + NSTAGE);
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int row = i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4);
+                const uint32_t p = b * TM + row;
+                if (p < d.n) {
+                    float *dst = d.geo + (size_t)p * 128 + tx * 4;
+                    *reinterpret_cast<float4 *>(dst) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+                    *reinterpret_cast<float4 *>(dst + 64) = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
+                }
+            }
+        }
+        __syncthreads();   // A, P and the batch's positions are rewritten by the next batch
+    }
+    for (uint32_t q = 0; q < NSTAGE; ++q) {
+        const uint32_t seq = wst.consumed + q;
+        mbar_wait(&s.bar[seq % NSTAGE], (seq / NSTAGE) & 1);
+    }
+}
+
+cudaError_t launch_density(const HeadArgs &a, const DensityArgs &d, cudaStream_t st) {
+    if (d.n == 0) return cudaSuccess;
+    auto kern = d.geo ? k_density<true> : k_density<false>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem));
+    if (e != cudaSuccess) return e;
+    const uint32_t need = (d.n + TM - 1) / TM;
+    const int blocks = (int)(need < (uint32_t)sm_count() ? need : (uint32_t)sm_count());
+    kern<<<blocks, NT, sizeof(Smem), st>>>(a, d);
+    return cudaGetLastError();
 }
 
 // Ray setup: one thread per (frame, ray).  Generates / loads the ray, slab-tests it, and marches it to its FIRST occupied

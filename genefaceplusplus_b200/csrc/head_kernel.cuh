@@ -93,6 +93,47 @@ cudaError_t launch_head_v2(const HeadArgs &a, const HeadV2Args &t, int precision
 cudaError_t launch_cond_images(const float *cond_feat, int n_frames, void *cond_hi, void *cond_lo, cudaStream_t st);
 size_t head_v2_smem_bytes(bool robust);
 
+// ---- density query (k_density in head_kernel.cu): the head field up to the sigma net, no marching, no colour ----
+// Points come from `xyzs` [n,3] or, when xyzs is null, from the occupancy cells in Morton order (n = C * H^3): point p is cell
+// m = p % H^3 of cascade p / H^3, placed exactly as renderer.py:243-258 does on the CPU in fp32.
+struct DensityArgs {
+    uint32_t n;
+    const float *xyzs;              // [n,3] or nullptr (cell mode)
+    const float *cond;              // [64] one conditioning vector for every point
+    float bound;                    // position grid bound (GridEncoder(..., bound=self.bound))
+    // cell mode
+    uint32_t grid_size;             // H
+    const float *noise;             // [C,H,H,H,3] in [0,1): meshgrid(x,y,z) order of renderer.py:243 with S >= H
+    float cell_scale[8], hgs[8];    // per cascade: float(bound_c - hgs_c) and float(hgs_c), hgs_c = bound_c / H
+    // outputs
+    float *sigma;                   // [n]: trunc_exp(h0) * out_scale
+    float *geo;                     // [n,128] h[1:129], or nullptr (then the 128 geo columns are never computed)
+    float out_scale;
+};
+// point p of a density query: xyzs[p], or the cell of Morton code p % H^3 in cascade p / H^3 placed exactly as renderer.py:246-258
+// does in fp32 (xyzs = 2*c/(H-1) - 1; cas_xyzs = xyzs*(bound_c - hgs_c) + (noise*2 - 1)*hgs_c).  False (and zeros) past the end.
+__device__ __forceinline__ bool density_point(const DensityArgs &d, uint32_t p, uint32_t H, uint32_t H3, float (&q)[3]) {
+    q[0] = q[1] = q[2] = 0.f;
+    if (p >= d.n) return false;
+    if (d.xyzs) {
+        q[0] = d.xyzs[3 * (size_t)p]; q[1] = d.xyzs[3 * (size_t)p + 1]; q[2] = d.xyzs[3 * (size_t)p + 2];
+        return true;
+    }
+    const uint32_t cas = p / H3, m = p - cas * H3;
+    const uint32_t c[3] = {compact3(m), compact3(m >> 1), compact3(m >> 2)};
+    const float *nz = d.noise + ((((size_t)cas * H + c[0]) * H + c[1]) * H + c[2]) * 3;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float xs = __fsub_rn(__fdiv_rn(__fmul_rn(2.0f, (float)c[k]), (float)(H - 1)), 1.0f);
+        const float r = __fmul_rn(__fsub_rn(__fmul_rn(nz[k], 2.0f), 1.0f), d.hgs[cas]);
+        q[k] = __fadd_rn(__fmul_rn(xs, d.cell_scale[cas]), r);
+    }
+    return true;
+}
+// fp32 FFMA field (head_kernel.cu) / fp16 wgmma field over the fp16 operand images and oct tables (head_tc_kernel.cu)
+cudaError_t launch_density(const HeadArgs &a, const DensityArgs &d, cudaStream_t st);
+cudaError_t launch_density_tc(const HeadArgs &a, const HeadTcArgs &t, const DensityArgs &d, cudaStream_t st);
+
 size_t head_smem_bytes();
 cudaError_t launch_head(const HeadArgs &a, int total_hint, cudaStream_t st);
 cudaError_t launch_ray_setup(const HeadArgs &a, cudaStream_t st);

@@ -454,4 +454,170 @@ cudaError_t launch_head_tc(const HeadArgs &a, const HeadTcArgs &t, int precision
     return cudaGetLastError();
 }
 
+// Density query in the fp16 mode (DensityArgs: head_kernel.cuh): the field k_head_tc shades -- fp16 "oct" tables, fp16 operands,
+// fp32 accumulation, the same tile stream -- up to the sigma net, for 128 points per batch and no marching.  The colour tiles of the
+// static 12-tile schedule are waited for and recycled without MMAs, so stage and parity stay compile-time constants.
+template <bool GEO>
+__global__ void __launch_bounds__(HEAD_NT, 2) k_density_tc(const __grid_constant__ HeadArgs a, const __grid_constant__ HeadTcArgs t,
+                                                          const __grid_constant__ DensityArgs d) {
+    constexpr bool BF16 = false, SPLIT = false;
+    extern __shared__ __align__(1024) unsigned char smem_raw_[];
+    unsigned char *smem_raw = smem_raw_ + ((1024u - (smem_u32(smem_raw_) & 1023u)) & 1023u);
+    SmemTC<SPLIT> &s = *reinterpret_cast<SmemTC<SPLIT> *>(smem_raw);
+    const int tid = threadIdx.x, warp = tid >> 5, wg = tid >> 7, lane = tid & 31;
+    if (tid == 32) {
+        for (int i = 0; i < W_NSTAGE; ++i) mbar_init(&s.bar_full[i], 1);
+        mbar_fence_init();
+    }
+    for (int i = tid; i < 3 * 128; i += NT) s.nw[i] = a.narrow[i];   // ambient out rows 0-2
+    stage_level_meta(a.pos_gm, nullptr, s.lvl[0], tid);
+    stage_level_meta(a.amb_gm, nullptr, s.lvl[1], tid);
+    fence_async_smem();
+    __syncthreads();
+    if (warp == 0) {
+        if (elect_one()) issue_loads<SPLIT, 0, W_NSTAGE>(t, s);
+        __syncwarp();
+    }
+    const uint32_t n_batches = (d.n + TM - 1) / TM;
+    const uint32_t H = d.grid_size, H3 = H * H * H;
+    const int slot = tid & (TM - 1), lg = tid >> 7;
+    for (uint32_t b = blockIdx.x; b < n_batches; b += gridDim.x) {
+        if (tid < TM) {
+            float q[3];
+            const bool v = density_point(d, b * TM + tid, H, H3, q);
+            s.valid[tid] = v ? 1 : 0;
+            s.sx[tid] = q[0]; s.sy[tid] = q[1]; s.sz[tid] = q[2];
+        }
+        __syncthreads();
+        const bool v = s.valid[slot] != 0;
+        uint4 park_h[2];
+        // ---- position grid -> A tile0 k[0,32) and the park; conditioning -> tile0 k[32,64), tile1 k[0,32) (as k_head_tc) ----
+        {
+            float u = 0.f, vv = 0.f, w = 0.f;
+            if (v) {
+                const float inv2b = 2.0f * d.bound;
+                u = __fdiv_rn(__fadd_rn(s.sx[slot], d.bound), inv2b);
+                vv = __fdiv_rn(__fadd_rn(s.sy[slot], d.bound), inv2b);
+                w = __fdiv_rn(__fadd_rn(s.sz[slot], d.bound), inv2b);
+            }
+            float f[16];
+            if (v) lookup8o(&s.lvl[0][lg * 16], a.pos_gm.align_off, a.pos_gm.interp == 1, a.pos_octs, u, vv, w, f);
+            else {
+#pragma unroll
+                for (int i = 0; i < 16; ++i) f[i] = 0.f;
+            }
+            store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 2 * lg), &f[0]);
+            store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 2 * lg + 1), &f[8]);
+#pragma unroll
+            for (int c = 0; c < 2; ++c) park_h[c] = *reinterpret_cast<const uint4 *>(s.a_hi[0] + sw128_off(slot, 2 * lg + c));
+            const float4 *cf = reinterpret_cast<const float4 *>(d.cond + lg * 32);
+#pragma unroll 1
+            for (int j = 0; j < 4; ++j) {
+                float c8[8];
+                if (v) {
+                    const float4 q0 = __ldg(cf + 2 * j), q1 = __ldg(cf + 2 * j + 1);
+                    c8[0] = q0.x; c8[1] = q0.y; c8[2] = q0.z; c8[3] = q0.w; c8[4] = q1.x; c8[5] = q1.y; c8[6] = q1.z; c8[7] = q1.w;
+                } else {
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) c8[i] = 0.f;
+                }
+                store_chunk<BF16, SPLIT>(s.a_hi[lg], s.a_lo[0], sw128_off(slot, (lg == 0 ? 4 : 0) + j), c8);
+            }
+        }
+        fence_async_smem();
+        __syncthreads();
+        // ---- ambient net 96 -> 128 -> 128 -> 3, tanh ----
+        {
+            float dd[64];
+            mma_layer<BF16, SPLIT, 0, 2, 128>(t, s, wg, warp, dd);
+            epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], dd, tid, nullptr, nullptr, nullptr);
+        }
+        fence_async_smem(); __syncthreads();
+        {
+            float dd[64];
+            mma_layer<BF16, SPLIT, 2, 2, 128>(t, s, wg, warp, dd);
+            epilogue_wide<BF16, SPLIT, true, false, true>(&s.a_hi[0][0], &s.a_lo[0][0], dd, tid, nullptr, s.nw, s.part);
+        }
+        __syncthreads();
+        if (tid < TM) {
+            s.amb[tid] = tanhf(s.part[0 * TM + tid]);
+            s.amb[TM + tid] = tanhf(s.part[1 * TM + tid]);
+            s.amb[2 * TM + tid] = tanhf(s.part[2 * TM + tid]);
+        }
+        __syncthreads();
+        // ---- sigma-net input: parked position features, ambient grid ----
+        {
+            float u = 0.f, vv = 0.f, w = 0.f;
+            if (v) {
+                u = __fdiv_rn(__fadd_rn(s.amb[slot], 1.0f), 2.0f);
+                vv = __fdiv_rn(__fadd_rn(s.amb[TM + slot], 1.0f), 2.0f);
+                w = __fdiv_rn(__fadd_rn(s.amb[2 * TM + slot], 1.0f), 2.0f);
+            }
+#pragma unroll
+            for (int c = 0; c < 2; ++c) *reinterpret_cast<uint4 *>(s.a_hi[0] + sw128_off(slot, 2 * lg + c)) = park_h[c];
+            float f[16];
+            if (v) lookup8o(&s.lvl[1][lg * 16], a.amb_gm.align_off, a.amb_gm.interp == 1, a.amb_octs, u, vv, w, f);
+            else {
+#pragma unroll
+                for (int i = 0; i < 16; ++i) f[i] = 0.f;
+            }
+            store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 4 + 2 * lg), &f[0]);
+            store_chunk<BF16, SPLIT>(s.a_hi[0], s.a_lo[0], sw128_off(slot, 4 + 2 * lg + 1), &f[8]);
+        }
+        fence_async_smem(); __syncthreads();
+        // ---- sigma net 64 -> 128 -> 128 -> (128 geo + sigma) ----
+        {
+            float dd[64];
+            mma_layer<BF16, SPLIT, 4, 1, 128>(t, s, wg, warp, dd);
+            epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], dd, tid, nullptr, nullptr, nullptr);
+        }
+        fence_async_smem(); __syncthreads();
+        {
+            float dd[64];
+            mma_layer<BF16, SPLIT, 5, 2, 128>(t, s, wg, warp, dd);
+            epilogue_wide<BF16, SPLIT, true, false, false>(&s.a_hi[0][0], &s.a_lo[0][0], dd, tid, nullptr, nullptr, nullptr);
+        }
+        fence_async_smem(); __syncthreads();
+        {
+            float dd[72];
+            mma_layer<BF16, SPLIT, 7, 2, 144>(t, s, wg, warp, dd);
+            const int wwarp = warp & 3;
+            if ((lane & 3) == 0) {   // column 128 = sigma logit
+                const uint32_t p = b * TM + 64 * wg + 16 * wwarp + (lane >> 2);
+                if (p < d.n) d.sigma[p] = __fmul_rn(expf(dd[64]), d.out_scale);
+                if (p + 8 < d.n) d.sigma[p + 8] = __fmul_rn(expf(dd[66]), d.out_scale);
+            }
+            if (GEO) {
+#pragma unroll
+                for (int i = 0; i < 64; i += 2) {
+                    const uint32_t p = b * TM + 64 * wg + frag_row(i, lane, wwarp);
+                    if (p < d.n) *reinterpret_cast<float2 *>(d.geo + (size_t)p * 128 + frag_col(i, lane)) = make_float2(dd[i], dd[i + 1]);
+                }
+            }
+        }
+        // ---- the colour tiles 9..11 of the static schedule: wait for them and recycle their stages for the next batch ----
+#pragma unroll
+        for (int c = 9; c < 12; ++c) mbar_wait(&s.bar_full[c % W_NSTAGE], (c / W_NSTAGE) & 1);
+        __syncthreads();
+        if (warp == 0) {
+            if (elect_one()) issue_loads<SPLIT, 12, 3>(t, s);
+            __syncwarp();
+        }
+    }
+    for (uint32_t q = 0; q < W_NSTAGE; ++q) mbar_wait(&s.bar_full[q], 0);   // tiles 0..2 of a batch that never comes
+}
+
+cudaError_t launch_density_tc(const HeadArgs &a, const HeadTcArgs &t, const DensityArgs &d, cudaStream_t st) {
+    if (d.n == 0) return cudaSuccess;
+    auto kern = d.geo ? k_density_tc<true> : k_density_tc<false>;
+    const size_t smem = head_tc_smem_bytes(false);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (e != cudaSuccess) return e;
+    const uint32_t need = (d.n + TM - 1) / TM, cap = 2u * (uint32_t)sm_count();
+    kern<<<need < cap ? need : cap, NT, smem, st>>>(a, t, d);
+    return cudaGetLastError();
+}
+
 }  // namespace gfpp

@@ -134,14 +134,6 @@ __global__ void k_freq_encode(const float *__restrict__ inputs, uint32_t B, uint
 // ---- tight cell bounds of the occupied voxels (used to skip bit reads in known-empty space) ----
 // bounds[0..2] = min cell, bounds[3..5] = max cell over all cascades; initialised by the caller to
 // {INT_MAX.., -1..}.  Cells are decoded from the Morton bit index.
-__device__ __forceinline__ uint32_t compact3(uint32_t x) {
-    x &= 0x49249249u;
-    x = (x | (x >> 2)) & 0xC30C30C3u;
-    x = (x | (x >> 4)) & 0x0F00F00Fu;
-    x = (x | (x >> 8)) & 0xFF0000FFu;
-    x = (x | (x >> 16)) & 0x0000FFFFu;
-    return x;
-}
 
 __global__ void k_occupancy_bounds(const uint8_t *__restrict__ bits, uint32_t n_bytes, uint32_t H3, int *bounds) {
     int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {-1, -1, -1};

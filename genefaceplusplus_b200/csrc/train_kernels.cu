@@ -441,14 +441,6 @@ __global__ void k_grad_tv(GridMeta gm, const float *__restrict__ inputs, const f
 }
 
 // ---- update_extra_state helpers ----
-__device__ __forceinline__ uint32_t compact3(uint32_t x) {   // __morton3D_invert (raymarching.cu:74-81)
-    x &= 0x49249249u;
-    x = (x | (x >> 2)) & 0xC30C30C3u;
-    x = (x | (x >> 4)) & 0x0F00F00Fu;
-    x = (x | (x >> 8)) & 0xFF0000FFu;
-    x = (x | (x >> 16)) & 0x0000FFFFu;
-    return x;
-}
 
 __global__ void k_packbits(const float *__restrict__ grid, uint32_t N, float thresh, uint8_t *__restrict__ bitfield) {
     for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < N; n += gridDim.x * blockDim.x) {

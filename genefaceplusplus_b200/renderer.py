@@ -141,6 +141,10 @@ class RADNeRF(nn.Module):
         self.register_buffer("density_grid", torch.zeros([self.cascade, self.grid_size ** 3]))
         self.register_buffer("density_bitfield", torch.zeros(self.cascade * self.grid_size ** 3 // 8, dtype=torch.uint8))
         self.register_buffer("step_counter", torch.zeros(16, 2, dtype=torch.int32))
+        self.mean_density = 0
+        self.iter_density = 0
+        self.mean_count = 0
+        self.local_step = 0
         # --- RADNeRF.__init__ (modules/radnerfs/radnerf.py:14-86)
         if hp["cond_type"] == "esperanto":
             self.cond_in_dim = 44
@@ -443,6 +447,129 @@ class RADNeRF(nn.Module):
                                                            _capi.stream_ptr(dev)), "gfpp_debug_generate_rays")
         return ro, rd
 
+    # ------------------------------------------------------------------ occupancy grid (NeRFRenderer, renderer.py:117-284)
+    @torch.no_grad()
+    def density(self, position, cond_feat, e=None, cond_mask=None):
+        """radnerf.py:143-166: {'sigma': trunc_exp(h0) [N], 'geo_feat': h[1:129] [N,128]} for positions [N,3] in [-bound, bound]
+        and one conditioning vector [64].  libgfpp evaluates the field of the model's mode: fp16 models on wgmma with their fp16
+        operand images and tables, the other modes in fp32."""
+        _, _, model, _ = self._ensure_packed()
+        dev = self.density_bitfield.device
+        x = position.to(dev, torch.float32).reshape(-1, 3).contiguous()
+        c = cond_feat.to(dev, torch.float32).reshape(-1).contiguous()
+        if c.numel() != self.cond_out_dim:
+            raise ValueError(f"density() takes one conditioning vector of {self.cond_out_dim} values")
+        n = x.shape[0]
+        sigma = torch.empty(n, device=dev, dtype=torch.float32)
+        geo = torch.empty(n, self.geo_feat_dim, device=dev, dtype=torch.float32)
+        if n:
+            with torch.cuda.device(dev):
+                _capi.check(_capi.lib().gfpp_density_query(ctypes.byref(model), x.data_ptr(), n, c.data_ptr(), sigma.data_ptr(),
+                                                           geo.data_ptr(), _capi.stream_ptr(dev)), "gfpp_density_query")
+        return {"sigma": sigma, "geo_feat": geo}
+
+    def reset_extra_state(self):
+        """renderer.py:117-129."""
+        self.density_grid.zero_()
+        self.mean_density = 0
+        self.iter_density = 0
+        self.step_counter.zero_()
+        self.mean_count = 0
+        self.local_step = 0
+
+    def _cell_noise(self, S, dev):
+        """The reference's rand_like draws (renderer.py:238-258) as one [C,H,H,H,3] tensor: chunks of S cells per axis, x-major,
+        one [chunk, 3] draw per cascade inside each chunk."""
+        H, C = self.grid_size, self.cascade
+        if S >= H:
+            return torch.stack([torch.rand(H ** 3, 3, device=dev) for _ in range(C)]).view(C, H, H, H, 3)
+        noise = torch.empty(C, H, H, H, 3, device=dev)
+        for x0 in range(0, H, S):
+            for y0 in range(0, H, S):
+                for z0 in range(0, H, S):
+                    nx, ny, nz = min(S, H - x0), min(S, H - y0), min(S, H - z0)
+                    for cas in range(C):
+                        noise[cas, x0:x0 + nx, y0:y0 + ny, z0:z0 + nz] = torch.rand(nx * ny * nz, 3, device=dev).view(nx, ny, nz, 3)
+        return noise
+
+    def refresh_density_grid(self, cond_feat, noise, decay=0.95, tmp_grid=None):
+        """The device half of update_extra_state (renderer.py:230-278) in libgfpp, on the current stream, no host sync:
+        density_grid (EMA, in place), the bitfield and the packed model's derived occupancy.  Returns the device scalar
+        mean_density.  tmp_grid: optional [C, H^3] fp32 tensor that receives the raw (pre-dilation) densities."""
+        _, _, model, _ = self._ensure_packed()
+        dev = self.density_bitfield.device
+        L = _capi.lib()
+        C, H = self.cascade, self.grid_size
+        c = cond_feat.to(dev, torch.float32).reshape(-1).contiguous()
+        if c.numel() != self.cond_out_dim:
+            raise ValueError(f"the grid refresh takes one conditioning vector of {self.cond_out_dim} values")
+        noise = noise.to(dev, torch.float32).contiguous()
+        if noise.numel() != C * H ** 3 * 3:
+            raise ValueError(f"noise must be [{C},{H},{H},{H},3]")
+        g = self.density_grid
+        if g.dtype != torch.float32 or not g.is_contiguous():
+            raise ValueError("density_grid must be a contiguous fp32 buffer")
+        if tmp_grid is not None and (tmp_grid.dtype != torch.float32 or not tmp_grid.is_contiguous() or tmp_grid.numel() != C * H ** 3
+                                     or tmp_grid.device != dev):
+            raise ValueError(f"tmp_grid must be a contiguous fp32 [{C},{H ** 3}] tensor on {dev}")
+        need = L.gfpp_density_grid_workspace_bytes(C, H)
+        if need == 0:
+            raise _capi.GfppError(f"the grid refresh does not support cascade {C} / grid_size {H}")
+        ws = self.__dict__.get("_grid_ws")
+        if ws is None or ws.numel() < need or ws.device != dev:
+            ws = self.__dict__["_grid_ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+        mean = torch.empty(1, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            # writes density_bitfield through its pointer: its _version does not move, so the packed model stays valid (the
+            # call itself rebuilt the packed occupancy bounds and coarse bits)
+            _capi.check(L.gfpp_density_grid_update(ctypes.byref(model), c.data_ptr(), noise.data_ptr(), float(decay), float(self.density_thresh),
+                                                   g.data_ptr(), mean.data_ptr(), None if tmp_grid is None else tmp_grid.data_ptr(),
+                                                   ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_density_grid_update")
+        self.last_launch_count = int(L.gfpp_last_launch_count())
+        return mean
+
+    @torch.no_grad()
+    def update_extra_state(self, decay=0.95, S=128, *, cond_index=None, noise=None):
+        """renderer.py:201-284 (the to_heatmap branch is not supported, as in the reference's own density()).  The conditioning
+        window comes from `self.conds` at `cond_index` (default: random.randint, as the reference) and the cell jitter from
+        `noise` [C,H,H,H,3] in [0,1) (default: torch.rand in the reference's draw order for chunk size S)."""
+        import random
+        from .scene import cond_window
+        if self.hparams.get("to_heatmap", False):
+            raise NotImplementedError("to_heatmap: the reference's density() asserts against it (radnerf.py:147)")
+        dev = self.density_bitfield.device
+        if dev.type != "cuda":
+            raise _capi.GfppError("model is not on a CUDA device: libgfpp has no CPU path (call .cuda())")
+        if cond_index is None:
+            cond_index = random.randint(0, self.conds.shape[0] - 1)
+        cond = cond_window(self.conds, cond_index, self.smo_win_size).to(dev)
+        cond_feat = self.cal_cond_feat(cond)
+        if noise is None:
+            noise = self._cell_noise(S, dev)
+        mean = self.refresh_density_grid(cond_feat, noise, decay)
+        self.mean_density = mean.item()
+        self.iter_density += 1
+        total_step = min(16, self.local_step)
+        if total_step > 0:
+            self.mean_count = int(self.step_counter[:total_step, 0].sum().item() / total_step)
+        self.local_step = 0
+
+    @torch.no_grad()
+    def mark_untrained_grid(self, poses, intrinsic, S=64):
+        """renderer.py:131-199: cells of density_grid that no camera of poses [B,4,4] (c2w) sees become -1.  intrinsic =
+        (fx, fy, cx, cy), taken as Python floats like the reference.  S (the reference's chunk size) does not change the result."""
+        dev = self.density_grid.device
+        if dev.type != "cuda":
+            raise _capi.GfppError("model is not on a CUDA device: libgfpp has no CPU path (call .cuda())")
+        if isinstance(poses, np.ndarray):
+            poses = torch.from_numpy(poses)
+        P = poses.to(dev, torch.float32).reshape(-1, 16).contiguous()
+        fx, fy, cx, cy = [float(v) for v in intrinsic]
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_mark_untrained_grid(P.data_ptr(), P.shape[0], fx, fy, cx, cy, float(self.bound), self.cascade,
+                                                             self.grid_size, self.density_grid.data_ptr(), _capi.stream_ptr(dev)),
+                        "gfpp_mark_untrained_grid")
+
     # ------------------------------------------------------------------ the reference's render()
     @torch.no_grad()
     def render(self, rays_o, rays_d, cond, bg_coords, poses, index=0, dt_gamma=0, bg_color=None, perturb=False,
@@ -634,6 +761,9 @@ class RADNeRFTorsowithSR(RADNeRF):
         self.sr_net = Superresolution(channels=3)
         self.encoders = None      # _NativeEncoders (libgfpp per-op kernels) on first use.  Nothing in the package sets this: it is the
                                   # seam through which the CPU unit test of the host logic supplies the checker's encoders
+
+    def update_extra_state(self, decay=0.95, S=128, **kwargs):
+        raise NotImplementedError("the torso models refresh density_grid_torso (radnerf_torso_sr.py:246-288): not built in libgfpp yet")
 
     @staticmethod
     def _mlp(x, net):
@@ -912,6 +1042,9 @@ class RADNeRFTorso(RADNeRF):
         # mean_density_torso is a plain attribute that is NOT in the checkpoint (=> 0 after load, radnerf_torso.py:22,167)
         d.density_thresh_torso = float(min(self.density_thresh_torso, self.mean_density_torso))
         d.torso_shrink = float(self.torso_shrink)
+
+    def update_extra_state(self, decay=0.95, S=128, **kwargs):
+        raise NotImplementedError("the torso models refresh density_grid_torso (radnerf_torso.py:201-242): not built in libgfpp yet")
 
     def torso_mask(self, bg_coords):
         """radnerf_torso.py:166-169 (host-side helper used only to shape the `deform` result like the reference)."""

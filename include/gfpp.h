@@ -363,6 +363,40 @@ GFPP_API int gfpp_morton3D_invert(const int32_t *indices, uint32_t N, int32_t *c
 GFPP_API int gfpp_morton3D_dilation(const float *grid, uint32_t C, uint32_t H, float *grid_dilation, void *stream);
 GFPP_API int gfpp_sph_from_ray(const float *rays_o, const float *rays_d, float radius, uint32_t N, float *coords, void *stream);
 
+/* ------------------------------------------------------------------ (E) occupancy-grid maintenance (SURVEY.md 8(f) rank 4)
+ *
+ * The head model's density grid as NeRFRenderer maintains it during training (modules/radnerfs/renderer.py:131-278), on a
+ * packed model.  The density query evaluates the head field up to the sigma net (RADNeRF.density, radnerf.py:143-166) in the
+ * arithmetic of the model's mode: fp16 models on wgmma with their fp16 operand images and fp16 tables (what they render); fp32,
+ * bf16x3, bf16 and robust models with the fp32 weight chunks and fp32 tables.  Everything is enqueued on `stream` with
+ * no host synchronisation and no allocation, and is bit-identical from run to run (no atomics whose order reaches an output).
+ *
+ * gfpp_density_query: sigma [n] = trunc_exp(h0) (raw: density_scale is NOT applied, as in density()); geo_feat [n,128] = h[1:129]
+ *   or NULL.  xyzs [n,3] in [-bound, bound]; cond_feat [64].  cond_feat and geo_feat 16-byte aligned.
+ * gfpp_density_grid_update: update_extra_state's grid refresh (renderer.py:230-278) --
+ *   1. sigma * density_scale at every cell of every cascade into tmp [C, H^3] (Morton order), the cell positions computed from
+ *      noise [C,H,H,H,3] in [0,1) (the rand_like draws of renderer.py:258 in meshgrid(x,y,z) order) in fp32 exactly as the reference;
+ *   2. tmp = 6-neighbour dilation; where density_grid >= 0 and tmp >= 0: density_grid = max(density_grid * decay, tmp);
+ *   3. *mean_out = mean(clamp(density_grid, 0)) (double accumulation, fixed order; device scalar);
+ *   4. the model's bitfield = packbits(density_grid, min(*mean_out, density_thresh)), threshold read on the device;
+ *   5. the packed model's occupied-cell bounds and coarse occupancy are rebuilt in place: the next gfpp_render_frames on `model`
+ *      marches the new grid without a repack.
+ *   density_grid [C, H^3] (16-byte aligned) is updated in place; tmp_grid [C, H^3] receives the raw (pre-dilation) densities, or
+ *   NULL.  The bitfield is written on `stream`: a render that reads it on another stream must be ordered against this call.
+ *   Cascade and grid_size come from the model: cascade 1..8, grid_size a power of two in 8..512 (Morton codes below H^3 cover
+ *   the grid only then); workspace: gfpp_density_grid_workspace_bytes (0 = unsupported shape).
+ * gfpp_mark_untrained_grid: mark_untrained_grid (renderer.py:131-199): density_grid [C, H^3] cells that no camera of
+ *   poses_c2w [B,4,4] sees are set to -1, the others are left as they are.  Intrinsics and bound as the reference's Python
+ *   floats (double); the coverage test runs in fp32 in the reference's operation order. */
+GFPP_API int gfpp_density_query(const gfpp_model *model, const float *xyzs, uint32_t n, const float *cond_feat, float *sigma,
+                                float *geo_feat, void *stream);
+GFPP_API size_t gfpp_density_grid_workspace_bytes(uint32_t cascade, uint32_t grid_size);
+GFPP_API int gfpp_density_grid_update(const gfpp_model *model, const float *cond_feat, const float *noise, float decay,
+                                      float density_thresh, float *density_grid, float *mean_out, float *tmp_grid, void *workspace,
+                                      size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_mark_untrained_grid(const float *poses_c2w, uint32_t n_poses, double fx, double fy, double cx, double cy,
+                                      double bound, uint32_t cascade, uint32_t grid_size, float *density_grid, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
