@@ -24,6 +24,10 @@ class GfppError(RuntimeError):
     pass
 
 
+class GfppNoCpuPath(GfppError, NotImplementedError):
+    """A libgfpp entry point was called on a model that lives on the CPU: there is no CPU path."""
+
+
 class GridDesc(ctypes.Structure):
     _fields_ = [("embeddings", c_void_p), ("offsets_host", c_void_p), ("input_dim", c_u32), ("num_levels", c_u32),
                 ("base_resolution", c_u32), ("log2_per_level_scale", c_f), ("gridtype", c_u32), ("interp", c_u32),
@@ -95,6 +99,8 @@ EXPORTS = [
     "gfpp_composite_rays_train_backward", "gfpp_grid_encode_forward_dydx", "gfpp_grid_encode_backward", "gfpp_grad_total_variation",
     "gfpp_packbits", "gfpp_morton3D", "gfpp_morton3D_invert", "gfpp_morton3D_dilation", "gfpp_sph_from_ray",
     "gfpp_density_query", "gfpp_density_grid_workspace_bytes", "gfpp_density_grid_update", "gfpp_mark_untrained_grid",
+    "gfpp_torso_grid_workspace_bytes", "gfpp_torso_query_workspace_bytes", "gfpp_torso_query", "gfpp_torso_grid_update", "gfpp_torso_sr_grid_update",
+    "gfpp_model_set_torso_threshold", "gfpp_torso_sr_set_threshold",
 ]
 
 
@@ -161,6 +167,15 @@ def lib():
         L.gfpp_density_grid_workspace_bytes.argtypes = [c_u32, c_u32]
         L.gfpp_density_grid_update.argtypes = [ctypes.POINTER(Model), P, P, c_f, c_f, P, P, P, P, c_size_t, P]
         L.gfpp_mark_untrained_grid.argtypes = [P, c_u32, c_d, c_d, c_d, c_d, c_d, c_u32, c_u32, P, P]
+        L.gfpp_torso_grid_workspace_bytes.restype = c_size_t
+        L.gfpp_torso_grid_workspace_bytes.argtypes = [c_u32]
+        L.gfpp_torso_query_workspace_bytes.restype = c_size_t
+        L.gfpp_torso_query_workspace_bytes.argtypes = []
+        L.gfpp_torso_query.argtypes = [ctypes.POINTER(Model), P, c_u32, P, P, P, P, P, P, c_size_t, P]
+        L.gfpp_torso_grid_update.argtypes = [ctypes.POINTER(Model), P, P, P, c_f, P, P, P, P, c_size_t, P]
+        L.gfpp_torso_sr_grid_update.argtypes = [ctypes.POINTER(TorsoSrModel), P, P, P, c_f, P, P, P, P, c_size_t, P]
+        L.gfpp_model_set_torso_threshold.argtypes = [ctypes.POINTER(Model), c_f]
+        L.gfpp_torso_sr_set_threshold.argtypes = [ctypes.POINTER(TorsoSrModel), c_f]
         _lib = L
     return _lib
 

@@ -11,6 +11,7 @@
 #include "head_kernel.cuh"
 #include "launch.cuh"
 #include "sr_kernel.cuh"
+#include "torso_grid_kernel.cuh"
 #include "torso_kernel.cuh"
 #include "torso_sr_kernel.cuh"
 
@@ -56,6 +57,8 @@ uint32_t dilate_ema_blocks(uint32_t C, uint32_t H);
 cudaError_t launch_grid_refresh_tail(const float *, uint32_t, uint32_t, float, float, float *, double *, float *, float *, uint8_t *, int *,
                                      cudaStream_t);
 cudaError_t launch_mark_untrained(const float *, uint32_t, float, float, const float *, const float *, uint32_t, uint32_t, float *, cudaStream_t);
+uint32_t torso_dilate_ema_blocks(uint32_t H);
+cudaError_t launch_torso_grid_tail(const float *, uint32_t, float, float, float *, double *, float *, float *, int *, cudaStream_t);
 }  // namespace gfpp
 
 using namespace gfpp;
@@ -1268,6 +1271,174 @@ int gfpp_mark_untrained_grid(const float *poses_c2w, uint32_t n_poses, double fx
     g_launches = 0;
     CK(launch_mark_untrained(poses_c2w, n_poses, (float)(cx / fx), (float)(cy / fy), scale, pad, cascade, grid_size, density_grid,
                              (cudaStream_t)stream));
+    return GFPP_OK;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------ (F) torso occupancy grid (torso_grid_kernel.cu; grid_kernels.cu)
+namespace {
+
+constexpr uint32_t kTorsoGridMax = 4096;
+bool torso_grid_ok(uint32_t H) { return H >= 2 && H <= kTorsoGridMax; }   // the cell placement divides by H - 1
+
+struct TorsoGridWork {
+    size_t bias_def, bias_can, tmp, partial, thresh, total;
+};
+
+TorsoGridWork torso_grid_work_layout(uint32_t H) {
+    TorsoGridWork W;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
+    W.bias_def = take(64 * 4);
+    W.bias_can = take(32 * 4);
+    W.tmp = take((size_t)H * H * 4);
+    W.partial = take((size_t)torso_dilate_ema_blocks(H) * 8);
+    W.thresh = take(4);
+    W.total = o;
+    return W;
+}
+
+// the bias block that opens the refresh's workspace is the query's whole workspace
+size_t torso_query_work_bytes() { return torso_grid_work_layout(2).tmp; }
+
+// query arguments of the plain torso field of a packed model, bias vectors in the workspace
+TorsoQueryArgs torso_query_args(const ModelHost &m, char *ws, const TorsoGridWork &W) {
+    TorsoQueryArgs q;
+    memset(&q, 0, sizeof(q));
+    q.tor_gm = m.tor_gm; q.tor_tab = m.tor_tab;
+    q.w_def0 = m.wd0; q.w_def1 = m.wd1; q.w_def2 = m.wd2; q.w_can0 = m.wc0; q.w_can1 = m.wc1; q.w_can2 = m.wc2;
+    q.bias_def = (const float *)(ws + W.bias_def); q.bias_can = (const float *)(ws + W.bias_can);
+    q.torso_shrink = m.torso_shrink;
+    return q;
+}
+
+cudaError_t launch_plain_torso_bias(const ModelHost &m, const float *pose6, const float *code, char *ws, const TorsoGridWork &W,
+                                    cudaStream_t st) {
+    TorsoArgs t;
+    memset(&t, 0, sizeof(t));
+    t.n_frames = 1; t.pose6 = pose6;
+    return launch_torso_frame_bias(t, m.torso_def0_src, m.torso_can0_src, code, (int)m.torso_code_dim, (float *)(ws + W.bias_def),
+                                   (float *)(ws + W.bias_can), st);
+}
+
+// the cell query into tmp (the reference's y*H + x layout), then dilation + EMA into density_grid_torso and the mean
+int torso_refresh(TorsoQueryArgs q, bool sr, uint32_t H, const float *noise, float decay, float *grid, float *mean_out, float *tmp_grid,
+                  char *ws, const TorsoGridWork &W, cudaStream_t st) {
+    float *tmp = tmp_grid ? tmp_grid : (float *)(ws + W.tmp);
+    q.n = H * H; q.grid_size = H; q.noise = noise;
+    q.cell_scale = (float)(1.0 - 1.0 / (double)H); q.hgs = (float)(1.0 / (double)H);   // Python floats of radnerf_torso.py:219-227
+    q.alpha = tmp;
+    CK(sr ? launch_torso_sr_query(q, st) : launch_torso_query(q, st));
+    int nl = 0;
+    const cudaError_t e = launch_torso_grid_tail(tmp, H, decay, INFINITY, grid, (double *)(ws + W.partial), mean_out,
+                                                 (float *)(ws + W.thresh), &nl, st);
+    g_launches += nl;
+    if (e != cudaSuccess) return fail(GFPP_ERR_CUDA, "launch_torso_grid_tail: %s", cudaGetErrorString(e));
+    return GFPP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t gfpp_torso_grid_workspace_bytes(uint32_t grid_size) {
+    return torso_grid_ok(grid_size) ? torso_grid_work_layout(grid_size).total : 0;
+}
+
+size_t gfpp_torso_query_workspace_bytes(void) { return torso_query_work_bytes(); }
+
+int gfpp_torso_query(const gfpp_model *model, const float *xy, uint32_t n, const float *pose6, const float *code, float *alpha,
+                     float *color, float *deform, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!model || !xy || !pose6 || !alpha || !workspace) return fail(GFPP_ERR_INVALID, "torso_query: null pointer%s");
+    ModelHost m;
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "torso_query: model handle not initialised by gfpp_model_pack%s");
+    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "torso_query: the model was packed without a torso (has_torso = 0)%s");
+    if ((code == nullptr) != (m.torso_code_dim == 0)) return fail(GFPP_ERR_INVALID, "torso_query: code must be given iff torso_code_dim > 0%s");
+    if (n >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_query: n must be < 2^31%s");
+    if (workspace_bytes < torso_query_work_bytes()) return fail(GFPP_ERR_WORKSPACE, "torso_query: workspace too small%s");
+    const TorsoGridWork W = torso_grid_work_layout(2);   // only its bias block is used
+    cudaStream_t st = (cudaStream_t)stream;
+    char *ws = (char *)workspace;
+    g_launches = 0;
+    if (n == 0) return GFPP_OK;
+    CK(launch_plain_torso_bias(m, pose6, code, ws, W, st));
+    TorsoQueryArgs q = torso_query_args(m, ws, W);
+    q.n = n; q.xy = xy;
+    q.alpha = alpha; q.color = color; q.deform = deform;
+    CK(launch_torso_query(q, st));
+    return GFPP_OK;
+}
+
+int gfpp_torso_grid_update(const gfpp_model *model, const float *pose6, const float *code, const float *noise, float decay,
+                           float *density_grid_torso, float *mean_out, float *tmp_grid, void *workspace, size_t workspace_bytes,
+                           void *stream) {
+    if (!model || !pose6 || !noise || !density_grid_torso || !mean_out || !workspace)
+        return fail(GFPP_ERR_INVALID, "torso_grid_update: null pointer%s");
+    ModelHost m;
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "torso_grid_update: model handle not initialised by gfpp_model_pack%s");
+    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "torso_grid_update: the model was packed without a torso (has_torso = 0)%s");
+    if ((code == nullptr) != (m.torso_code_dim == 0))
+        return fail(GFPP_ERR_INVALID, "torso_grid_update: code must be given iff torso_code_dim > 0%s");
+    const uint32_t H = m.grid_size;
+    if (!torso_grid_ok(H)) return fail(GFPP_ERR_UNSUPPORTED, "torso_grid_update: grid_size must be in 2..4096%s");
+    const TorsoGridWork W = torso_grid_work_layout(H);
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "torso_grid_update: workspace too small%s");
+    cudaStream_t st = (cudaStream_t)stream;
+    char *ws = (char *)workspace;
+    g_launches = 0;
+    CK(launch_plain_torso_bias(m, pose6, code, ws, W, st));
+    return torso_refresh(torso_query_args(m, ws, W), false, H, noise, decay, density_grid_torso, mean_out, tmp_grid, ws, W, st);
+}
+
+int gfpp_torso_sr_grid_update(const gfpp_torso_sr_model *model, const float *lm68, const float *code, const float *noise, float decay,
+                              float *density_grid_torso, float *mean_out, float *tmp_grid, void *workspace, size_t workspace_bytes,
+                              void *stream) {
+    if (!model || !lm68 || !noise || !density_grid_torso || !mean_out || !workspace)
+        return fail(GFPP_ERR_INVALID, "torso_sr_grid_update: null pointer%s");
+    TorsoSrHost m;
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != kTorsoSrMagic) return fail(GFPP_ERR_INVALID, "torso_sr_grid_update: model handle not initialised by gfpp_torso_sr_pack%s");
+    if ((code == nullptr) != (m.code_dim == 0))
+        return fail(GFPP_ERR_INVALID, "torso_sr_grid_update: code must be given iff torso_code_dim > 0%s");
+    const uint32_t H = m.grid_size;
+    if (!torso_grid_ok(H)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_grid_update: grid_size must be in 2..4096%s");
+    const TorsoGridWork W = torso_grid_work_layout(H);
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "torso_sr_grid_update: workspace too small%s");
+    cudaStream_t st = (cudaStream_t)stream;
+    char *ws = (char *)workspace;
+    g_launches = 0;
+    CK(launch_torso_sr_frame_bias(lm68, 1, m.def0_src, m.can0_src, code, (int)m.code_dim, m.head_aware, (float *)(ws + W.bias_def),
+                                  (float *)(ws + W.bias_can), st));
+    TorsoQueryArgs q;
+    memset(&q, 0, sizeof(q));
+    q.tor_gm = m.tor_gm; q.tor_tab = m.tor_tab;
+    q.w_def0 = m.wd0; q.w_def1 = m.wd1; q.w_def2 = m.wd2; q.w_can0 = m.wc0; q.w_can1 = m.wc1; q.w_can2 = m.wc2; q.ha = m.ha;
+    q.bias_def = (const float *)(ws + W.bias_def); q.bias_can = (const float *)(ws + W.bias_can);
+    q.torso_shrink = m.torso_shrink;
+    return torso_refresh(q, true, H, noise, decay, density_grid_torso, mean_out, tmp_grid, ws, W, st);
+}
+
+int gfpp_model_set_torso_threshold(gfpp_model *model, float density_thresh_torso) {
+    if (!model) return fail(GFPP_ERR_INVALID, "model_set_torso_threshold: null pointer%s");
+    ModelHost m;
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "model_set_torso_threshold: model handle not initialised by gfpp_model_pack%s");
+    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "model_set_torso_threshold: the model was packed without a torso (has_torso = 0)%s");
+    m.density_thresh_torso = density_thresh_torso;
+    memcpy(model, &m, sizeof(m));
+    return GFPP_OK;
+}
+
+int gfpp_torso_sr_set_threshold(gfpp_torso_sr_model *model, float density_thresh_torso) {
+    if (!model) return fail(GFPP_ERR_INVALID, "torso_sr_set_threshold: null pointer%s");
+    TorsoSrHost m;
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != kTorsoSrMagic) return fail(GFPP_ERR_INVALID, "torso_sr_set_threshold: model handle not initialised by gfpp_torso_sr_pack%s");
+    m.density_thresh_torso = density_thresh_torso;
+    memcpy(model, &m, sizeof(m));
     return GFPP_OK;
 }
 

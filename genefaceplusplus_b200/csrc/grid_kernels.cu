@@ -1,6 +1,7 @@
 // grid_kernels.cu -- occupancy-grid maintenance behind gfpp.h section (E): the device half of NeRFRenderer.update_extra_state
 // (modules/radnerfs/renderer.py:201-278) after the density query (k_density, head_kernel.cu), and mark_untrained_grid
-// (renderer.py:131-199).  Everything is stream-ordered and deterministic: fixed work per block, fixed reduction trees, no atomics.
+// (renderer.py:131-199), and the torso grid's dilation + EMA + mean after the torso query (k_torso_query / k_torso_sr_query,
+// torso_grid_kernel.cu).  Everything is stream-ordered and deterministic: fixed work per block, fixed reduction trees, no atomics.
 #include "common.cuh"
 #include "launch.cuh"
 
@@ -52,6 +53,30 @@ __global__ void __launch_bounds__(RED_NT) k_dilate_ema(const float *__restrict__
             grid[n] = v;
         }
         acc += (double)fmaxf(v, 0.f);
+    }
+    const double s = block_sum(acc, sh);
+    if (threadIdx.x == 0) partial[blockIdx.x] = s;
+}
+
+// radnerf_torso.py:235-241: tmp = max_pool2d(tmp, 5, stride 1, padding 2) (out-of-range cells are -inf: skipped);
+// grid = max(grid * decay, tmp) everywhere (no untrained cells in the torso grid); then this block's share of sum(grid) in double
+// (no clamp: the torso mean is a plain mean).  tmp and grid are [H, H]; the 5x5 window is symmetric in x and y.
+__global__ void __launch_bounds__(RED_NT) k_torso_dilate_ema(const float *__restrict__ tmp, uint32_t H, float decay,
+                                                             float *__restrict__ grid, double *__restrict__ partial) {
+    __shared__ double sh[RED_NT / 32];
+    const uint32_t total = H * H;
+    double acc = 0.0;
+    const uint32_t base = blockIdx.x * RED_CELLS;
+    for (int k = 0; k < RED_PER_THREAD; ++k) {
+        const uint32_t n = base + k * RED_NT + threadIdx.x;
+        if (n >= total) break;
+        const int y = (int)(n / H), x = (int)(n - (uint32_t)y * H), h = (int)H;
+        float r = tmp[n];
+        for (int yy = max(y - 2, 0); yy <= min(y + 2, h - 1); ++yy)
+            for (int xx = max(x - 2, 0); xx <= min(x + 2, h - 1); ++xx) r = fmaxf(r, tmp[yy * h + xx]);
+        const float v = fmaxf(__fmul_rn(grid[n], decay), r);
+        grid[n] = v;
+        acc += (double)v;
     }
     const double s = block_sum(acc, sh);
     if (threadIdx.x == 0) partial[blockIdx.x] = s;
@@ -136,6 +161,22 @@ cudaError_t launch_grid_refresh_tail(const float *tmp, uint32_t C, uint32_t H, f
     ++*n_launches;
     const uint32_t nbytes = C * H * H * H / 8;
     k_packbits_dev<<<grid_for(nbytes, 256), 256, 0, st>>>(grid, nbytes, thresh_dev, bitfield);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) ++*n_launches;
+    return e;
+}
+
+uint32_t torso_dilate_ema_blocks(uint32_t H) { return (H * H + RED_CELLS - 1) / RED_CELLS; }
+
+cudaError_t launch_torso_grid_tail(const float *tmp, uint32_t H, float decay, float density_thresh, float *grid, double *partial,
+                                   float *mean_out, float *thresh_dev, int *n_launches, cudaStream_t st) {
+    *n_launches = 0;
+    const uint32_t nb = torso_dilate_ema_blocks(H);
+    k_torso_dilate_ema<<<nb, RED_NT, 0, st>>>(tmp, H, decay, grid, partial);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    ++*n_launches;
+    k_mean_thresh<<<1, RED_NT, 0, st>>>(partial, nb, H * H, density_thresh, mean_out, thresh_dev);
     e = cudaGetLastError();
     if (e == cudaSuccess) ++*n_launches;
     return e;

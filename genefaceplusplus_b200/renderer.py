@@ -719,7 +719,109 @@ class _NativeEncoders:
         return out.permute(1, 0, 2).reshape(B, Lv * C)
 
 
-class RADNeRFTorsowithSR(RADNeRF):
+class _TorsoGrid:
+    """density_grid_torso maintenance shared by the two torso classes: update_extra_state of radnerf_torso.py:201-242 and
+    radnerf_torso_sr.py:246-288 in libgfpp (gfpp.h section F).  Each class supplies `_torso_grid_condition(index, dev)` (what the
+    field is conditioned on for training pose `index`), `_torso_grid_call(...)` (its C entry point) and
+    `_set_torso_threshold(thr)` (writes the new mask threshold into its packed handle, no repack)."""
+
+    def _torso_cell_noise(self, S, dev):
+        """The reference's rand_like draws (radnerf_torso.py:216-227) as one [H,H,2] tensor: chunks of S cells along x, then y,
+        one [chunk, 2] draw per chunk in meshgrid(x, y) order."""
+        H = self.grid_size
+        noise = torch.empty(H, H, 2, device=dev)
+        for x0 in range(0, H, S):
+            for y0 in range(0, H, S):
+                nx, ny = min(S, H - x0), min(S, H - y0)
+                noise[x0:x0 + nx, y0:y0 + ny] = torch.rand(nx * ny, 2, device=dev).view(nx, ny, 2)
+        return noise
+
+    def _torso_grid_ws(self, dev, need=None):
+        """Device workspace of the refresh (default) or of `need` bytes (the torso query), kept across calls."""
+        if need is None:
+            need = _capi.lib().gfpp_torso_grid_workspace_bytes(self.grid_size)
+            if need == 0:
+                raise _capi.GfppError(f"the torso grid refresh does not support grid_size {self.grid_size}")
+        ws = self.__dict__.get("_torso_grid_ws_buf")
+        if ws is None or ws.numel() < need or ws.device != dev:
+            ws = self.__dict__["_torso_grid_ws_buf"] = torch.empty(need, dtype=torch.uint8, device=dev)
+        return ws
+
+    def _torso_code_row(self, index, dev):
+        """torso_individual_codes[index] as a contiguous fp32 device vector, or None without codes.  The index is checked here, on
+        the host: an out-of-range row never reaches the device."""
+        if self.torso_individual_embedding_dim == 0:
+            return None
+        n = self.torso_individual_codes.shape[0]
+        if not 0 <= index < n:
+            raise IndexError(f"torso code row {index} out of range for {n} torso_individual_codes")
+        return self.torso_individual_codes[index].detach().to(dev, torch.float32).contiguous()
+
+    def _require_cuda(self):
+        dev = self.density_bitfield.device
+        if dev.type != "cuda":
+            raise _capi.GfppNoCpuPath("model is not on a CUDA device: libgfpp has no CPU path (call .cuda())")
+        return dev
+
+    @torch.no_grad()
+    def refresh_torso_grid(self, cond, code, noise, decay=0.95, tmp_grid=None):
+        """The device half of update_extra_state in libgfpp, on the current stream, no host sync: density_grid_torso (dilated
+        EMA, in place).  Returns the device scalar mean_density_torso.  cond: pose6 [6] (RADNeRFTorso) or lm68 [136]
+        (RADNeRFTorsowithSR); code: a row of torso_individual_codes or None; noise [H,H,2] in [0,1); tmp_grid: optional [H*H]
+        fp32 tensor that receives the raw (pre-dilation) alphas at the reference's index y*H + x."""
+        dev = self._require_cuda()
+        H = self.grid_size
+        noise = noise.to(dev, torch.float32).contiguous()
+        if noise.numel() != H * H * 2:
+            raise ValueError(f"noise must be [{H},{H},2]")
+        g = self.density_grid_torso
+        if g.dtype != torch.float32 or not g.is_contiguous():
+            raise ValueError("density_grid_torso must be a contiguous fp32 buffer")
+        if tmp_grid is not None and (tmp_grid.dtype != torch.float32 or not tmp_grid.is_contiguous() or tmp_grid.numel() != H * H
+                                     or tmp_grid.device != dev):
+            raise ValueError(f"tmp_grid must be a contiguous fp32 [{H * H}] tensor on {dev}")
+        if (code is None) != (self.torso_individual_embedding_dim == 0):
+            raise ValueError("code must be given iff the model has torso_individual_codes")
+        if code is not None:
+            code = code.to(dev, torch.float32).reshape(-1).contiguous()
+        ws = self._torso_grid_ws(dev)
+        mean = torch.empty(1, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            # writes density_grid_torso through its pointer: its _version does not move, so the packed handles stay valid
+            self._torso_grid_call(cond, code, noise, float(decay), g.data_ptr(), mean.data_ptr(),
+                                  None if tmp_grid is None else tmp_grid.data_ptr(), ws)
+        self.last_launch_count = int(_capi.lib().gfpp_last_launch_count())
+        return mean
+
+    @torch.no_grad()
+    def update_extra_state(self, decay=0.95, S=128, *, pose_index=None, noise=None):
+        """radnerf_torso.py:201-242 / radnerf_torso_sr.py:246-288: refreshes density_grid_torso and mean_density_torso only.  The
+        field is conditioned on training pose `pose_index` of `self.poses` (and `self.lm68s`), which the training task sets, with
+        torso code row `pose_index` (default: random.randint, as the reference); the cell jitter comes from `noise` [H,H,2] in
+        [0,1) (default: torch.rand in the reference's draw order for chunk size S).  The next render masks with the new
+        min(density_thresh_torso, mean_density_torso) without a repack."""
+        import random
+        dev = self._require_cuda()
+        if pose_index is None:
+            pose_index = random.randint(0, len(self.poses) - 1)
+        if not 0 <= pose_index < len(self.poses):
+            raise IndexError(f"pose_index {pose_index} out of range for {len(self.poses)} training poses")
+        cond = self._torso_grid_condition(pose_index, dev)
+        code = self._torso_code_row(pose_index, dev)
+        if noise is None:
+            noise = self._torso_cell_noise(S, dev)
+        mean = self.refresh_torso_grid(cond, code, noise, decay)
+        self.mean_density_torso = mean.item()
+        self._set_torso_threshold(float(min(self.density_thresh_torso, self.mean_density_torso)))
+        # the head pack's cache key (RADNeRF._ensure_packed: density_scale, mean_density_torso, device, mlp_precision, versions)
+        # follows the new mean without a repack: RADNeRFTorso's handle has just been given the new threshold, and RADNeRFTorsowithSR
+        # packs the head field only (has_torso = 0), which the torso mean does not touch
+        if self._packed is not None:
+            key, packed, model, keep = self._packed
+            self._packed = ((key[0], self.mean_density_torso) + key[2:], packed, model, keep)
+
+
+class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
     """modules/radnerfs/radnerf_torso_sr.py:17-246 (the `lm3d_radnerf_torso_sr.yaml` checkpoints; SURVEY.md 8(f) rank 3).
 
     Same state (`density_grid_torso`, `torso_individual_codes`, `torso_embedder.*`, `head_color_weights_encoder.*`,
@@ -762,8 +864,26 @@ class RADNeRFTorsowithSR(RADNeRF):
         self.encoders = None      # _NativeEncoders (libgfpp per-op kernels) on first use.  Nothing in the package sets this: it is the
                                   # seam through which the CPU unit test of the host logic supplies the checker's encoders
 
-    def update_extra_state(self, decay=0.95, S=128, **kwargs):
-        raise NotImplementedError("the torso models refresh density_grid_torso (radnerf_torso_sr.py:246-288): not built in libgfpp yet")
+    # ---- density_grid_torso refresh (_TorsoGrid): the field conditioned on lm68s[index], head-aware inputs zero
+    def _torso_grid_condition(self, index, dev):
+        return self.lm68s[index].detach().to(dev, torch.float32).reshape(136).contiguous()
+
+    def _torso_grid_call(self, lm68, code, noise, decay, grid, mean, tmp, ws):
+        lm68 = lm68.to(self.density_bitfield.device, torch.float32).reshape(-1).contiguous()
+        if lm68.numel() != 136:
+            raise ValueError("the torso-SR refresh takes one lm68 row of 136 values")
+        st = self._torso_native_state()
+        dev = self.density_bitfield.device
+        _capi.check(_capi.lib().gfpp_torso_sr_grid_update(ctypes.byref(st["model"]), lm68.data_ptr(), None if code is None else code.data_ptr(),
+                                                          noise.data_ptr(), decay, grid, mean, tmp, ws.data_ptr(), ws.numel(),
+                                                          _capi.stream_ptr(dev)), "gfpp_torso_sr_grid_update")
+
+    def _set_torso_threshold(self, thr):
+        st = self.__dict__.get("_torso_native")
+        if st is None:
+            return                              # the next _torso_native_state() packs with the new threshold
+        _capi.check(_capi.lib().gfpp_torso_sr_set_threshold(ctypes.byref(st["model"]), thr), "gfpp_torso_sr_set_threshold")
+        st["key"] = (st["key"][0], thr, st["key"][2])   # (device, threshold, parameter pointers + versions)
 
     @staticmethod
     def _mlp(x, net):
@@ -1003,7 +1123,7 @@ class RADNeRFTorsowithSR(RADNeRF):
 
 
 # ------------------------------------------------------------------------------------------------ torso model
-class RADNeRFTorso(RADNeRF):
+class RADNeRFTorso(_TorsoGrid, RADNeRF):
     has_torso = True
     forwards_eye_area = False
 
@@ -1043,8 +1163,49 @@ class RADNeRFTorso(RADNeRF):
         d.density_thresh_torso = float(min(self.density_thresh_torso, self.mean_density_torso))
         d.torso_shrink = float(self.torso_shrink)
 
-    def update_extra_state(self, decay=0.95, S=128, **kwargs):
-        raise NotImplementedError("the torso models refresh density_grid_torso (radnerf_torso.py:201-242): not built in libgfpp yet")
+    @torch.no_grad()
+    def forward_torso(self, x, poses, c=None):
+        """radnerf_torso.py:51-84 in libgfpp (k_torso_query, fp32): x [n,2] in [-1,1], poses [1,6] (convert_poses of the head
+        pose), c [1,torso_code_dim] (a row of torso_individual_codes) or None without codes -> (alpha [n,1], color [n,3],
+        dx [n,2]).  Inference only: no autograd."""
+        dev = self._require_cuda()
+        _, _, model, _ = self._ensure_packed()
+        f32 = torch.float32
+        xy = x.to(dev, f32).reshape(-1, 2).contiguous()
+        pose6 = poses.to(dev, f32).reshape(-1).contiguous()
+        if pose6.numel() != 6:
+            raise ValueError("forward_torso takes one pose [1,6] (convert_poses)")
+        if (c is None) != (self.torso_individual_embedding_dim == 0):
+            raise ValueError("c must be given iff the model has torso_individual_codes")
+        code = None if c is None else c.to(dev, f32).reshape(-1).contiguous()
+        n = xy.shape[0]
+        alpha, color, dx = (torch.empty(n, k, device=dev, dtype=f32) for k in (1, 3, 2))
+        ws = self._torso_grid_ws(dev, _capi.lib().gfpp_torso_query_workspace_bytes())
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_torso_query(ctypes.byref(model), xy.data_ptr(), n, pose6.data_ptr(),
+                                                     None if code is None else code.data_ptr(), alpha.data_ptr(), color.data_ptr(),
+                                                     dx.data_ptr(), ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_torso_query")
+        return alpha, color, dx
+
+    # ---- density_grid_torso refresh (_TorsoGrid): the field conditioned on convert_poses(poses[index])
+    def _torso_grid_condition(self, index, dev):
+        from .scene import convert_poses
+        return convert_poses(self.poses[index].detach().cpu().float().reshape(1, 4, 4)).to(dev).reshape(6)
+
+    def _torso_grid_call(self, pose6, code, noise, decay, grid, mean, tmp, ws):
+        _, _, model, _ = self._ensure_packed()
+        dev = self.density_bitfield.device
+        pose6 = pose6.to(dev, torch.float32).reshape(-1).contiguous()
+        if pose6.numel() != 6:
+            raise ValueError("the torso refresh takes one pose6 of 6 values (convert_poses)")
+        _capi.check(_capi.lib().gfpp_torso_grid_update(ctypes.byref(model), pose6.data_ptr(), None if code is None else code.data_ptr(),
+                                                       noise.data_ptr(), decay, grid, mean, tmp, ws.data_ptr(), ws.numel(),
+                                                       _capi.stream_ptr(dev)), "gfpp_torso_grid_update")
+
+    def _set_torso_threshold(self, thr):
+        if self._packed is None:
+            return                              # the next _ensure_packed() packs with the new mean_density_torso
+        _capi.check(_capi.lib().gfpp_model_set_torso_threshold(ctypes.byref(self._packed[2]), thr), "gfpp_model_set_torso_threshold")
 
     def torso_mask(self, bg_coords):
         """radnerf_torso.py:166-169 (host-side helper used only to shape the `deform` result like the reference)."""

@@ -29,6 +29,10 @@
  *      gfpp_torso_sr_* (the torso field of radnerf_torso_sr.py), declared at the end of this file.
  *
  *  (D) the training-side native ops (SURVEY.md 8(f) rank 4), mirroring the reference's pybind functions like (A).
+ *
+ *  (E) occupancy-grid maintenance of the head models: density query, grid refresh, mark_untrained_grid.
+ *
+ *  (F) the torso models' occupancy grid: torso field query and density_grid_torso refresh, threshold setters.
  */
 #ifndef GFPP_H_
 #define GFPP_H_
@@ -396,6 +400,40 @@ GFPP_API int gfpp_density_grid_update(const gfpp_model *model, const float *cond
                                       size_t workspace_bytes, void *stream);
 GFPP_API int gfpp_mark_untrained_grid(const float *poses_c2w, uint32_t n_poses, double fx, double fy, double cx, double cy,
                                       double bound, uint32_t cascade, uint32_t grid_size, float *density_grid, void *stream);
+
+/* ------------------------------------------------------------------ (F) torso occupancy grid (SURVEY.md 8(f) rank 4)
+ *
+ * density_grid_torso [H*H] as the torso models maintain it during training (RADNeRFTorso.update_extra_state,
+ * radnerf_torso.py:201-242; RADNeRFTorsowithSR.update_extra_state, radnerf_torso_sr.py:246-288), H = the packed model's
+ * grid_size in 2..4096.  The torso fields run in fp32 FFMA, in the arithmetic of the render epilogues.  Everything is enqueued
+ * on `stream` with no host synchronisation and no allocation, and is bit-identical from run to run.  `code` is one row of
+ * torso_individual_codes [torso_code_dim] (the refresh uses row rand_idx, not row 0); it is NULL iff torso_code_dim == 0.
+ * Workspaces: gfpp_torso_grid_workspace_bytes(grid_size) for the refresh (0 = unsupported size), gfpp_torso_query_workspace_bytes()
+ * for the query (the two folded bias vectors only; a refresh workspace is large enough for it too).
+ *
+ * gfpp_torso_query: forward_torso (radnerf_torso.py:51-84) of a model packed with has_torso = 1 at xy [n,2] in [-1,1] for the
+ *   head pose pose6 [6] (convert_poses): alpha [n], color [n,3] or NULL, deform [n,2] (dx before the clamp) or NULL.
+ * gfpp_torso_grid_update / gfpp_torso_sr_grid_update: the refresh, for the plain torso model (pose6 [6]) and for the torso-SR
+ *   model (lm68 [136]; with head_aware its encoder sees image = weights_sum = 0, as the reference passes it) --
+ *   1. alpha at every cell into tmp [H*H] at the reference's transposed index y*H + x, the cell positions computed from
+ *      noise [H,H,2] in [0,1) (the rand_like draws in meshgrid(x, y) order) in fp32 exactly as the reference;
+ *   2. tmp = 5x5 max (max_pool2d, stride 1, padding 2); density_grid_torso = max(density_grid_torso * decay, tmp) in place;
+ *   3. *mean_out = mean(density_grid_torso) (no clamp; double accumulation, fixed order; device scalar).
+ *   tmp_grid [H*H] receives the raw (pre-dilation) alphas, or NULL.
+ * gfpp_model_set_torso_threshold / gfpp_torso_sr_set_threshold: host-only write of the mask threshold
+ *   min(density_thresh_torso, mean_density_torso) into the handle: the next render masks with it without a repack. */
+GFPP_API size_t gfpp_torso_grid_workspace_bytes(uint32_t grid_size);
+GFPP_API size_t gfpp_torso_query_workspace_bytes(void);
+GFPP_API int gfpp_torso_query(const gfpp_model *model, const float *xy, uint32_t n, const float *pose6, const float *code,
+                              float *alpha, float *color, float *deform, void *workspace, size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_torso_grid_update(const gfpp_model *model, const float *pose6, const float *code, const float *noise,
+                                    float decay, float *density_grid_torso, float *mean_out, float *tmp_grid, void *workspace,
+                                    size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_torso_sr_grid_update(const gfpp_torso_sr_model *model, const float *lm68, const float *code, const float *noise,
+                                       float decay, float *density_grid_torso, float *mean_out, float *tmp_grid, void *workspace,
+                                       size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_model_set_torso_threshold(gfpp_model *model, float density_thresh_torso);
+GFPP_API int gfpp_torso_sr_set_threshold(gfpp_torso_sr_model *model, float density_thresh_torso);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,13 @@ Legs (CUDA events, median of `reps` after one warm-up call; ms per call):
     per-op grid_encode_forward launches, then the per-op morton3D_dilation, the masked EMA, mean().item() and packbits -- once over
     libgfpp's per-op kernels and, where oracle/_ref was built, once over the reference's own compiled kernels.
 Algorithmic work of one refresh: C*H^3 points x (96*128 + 128*128 + 128*3 + 64*128 + 128*128 + 128*1) * 2 FLOP (the sigma column
-only) and 2 grids x 16 levels x 8 corners x 8 B = 2048 B of gathers per point."""
+only) and 2 grids x 16 levels x 8 corners x 8 B = 2048 B of gathers per point.
+Torso legs (the torso models' update_extra_state, radnerf_torso.py:201-242 / radnerf_torso_sr.py:246-288), 128^2 = 16 384 cells:
+  * native refresh of density_grid_torso for RADNeRFTorso and RADNeRFTorsowithSR (frame-bias fold -> k_torso_query /
+    k_torso_sr_query -> k_torso_dilate_ema -> k_mean_thresh), including the one .item() of mean_density_torso; launches per call;
+  * eager: the reference's procedure on the GPU -- forward_torso as PyTorch F.linear / ReLU over libgfpp's per-op freq / grid
+    encoder kernels, then max_pool2d, maximum, mean().item().
+  Algorithmic FLOP per cell: 2 x the multiply-adds of the deform and canonical nets (and the head-aware encoder), from the weights."""
 import argparse
 import json
 import os
@@ -99,6 +105,67 @@ def eager_refresh(model, ge, rm, cond_feat, noise, decay, autocast=True):
     return mean
 
 
+def _mlp(x, net):
+    for i, lin in enumerate(net.net):
+        x = F.linear(x, lin.weight)
+        if i != len(net.net) - 1:
+            x = F.relu(x)
+    return x
+
+
+def eager_torso_refresh(m, enc, cond, code, noise, decay):
+    """radnerf_torso.py:204-242 (radnerf_torso_sr.py:249-288 when m is a torso-SR model) with S >= grid_size: one chunk of cells,
+    forward_torso as PyTorch ops over libgfpp's per-op encoder kernels."""
+    H = m.grid_size
+    r = torch.arange(H, dtype=torch.int32, device="cuda")
+    xx, yy = torch.meshgrid(r, r, indexing="ij")
+    coords = torch.cat([xx.reshape(-1, 1), yy.reshape(-1, 1)], dim=-1)
+    idx = (coords[:, 1] * H + coords[:, 0]).long()
+    xys = (2 * coords.float() / (H - 1) - 1) * (1 - 1 / H) + (noise.view(-1, 2) * 2 - 1) * (1 / H)
+    if cond.numel() == 136:     # torso-SR model: its host-side forward_torso over the same per-op encoders (m.encoders)
+        alphas, _, _ = m.forward_torso(xys, None, code.view(1, -1), lm68=cond)
+    else:
+        x = xys * m.torso_shrink
+        n = x.shape[0]
+        h = torch.cat([enc.freq_encode(x, 10), enc.freq_encode(cond.view(1, 6), 4).expand(n, -1), code.view(1, -1).expand(n, -1)], -1)
+        dx = _mlp(h, m.torso_deform_net)
+        lay = m.torso_embedder.layout
+        xf = enc.grid_encode(((x + dx).clamp(-1, 1) + 1) / 2, m.torso_embedder.embeddings, m.torso_embedder.offsets, lay.per_level_scale,
+                             lay.base_resolution, 1, False, 0)
+        alphas = torch.sigmoid(_mlp(torch.cat([xf, h], -1), m.torso_canonicial_net)[..., :1])
+    tmp = torch.zeros(H * H, device="cuda")
+    tmp[idx] = alphas.squeeze(1).float()
+    tmp = F.max_pool2d(tmp.view(1, 1, H, H), kernel_size=5, stride=1, padding=2).view(-1)
+    m.density_grid_torso = torch.maximum(m.density_grid_torso * decay, tmp)
+    return torch.mean(m.density_grid_torso).item()
+
+
+def measure_torso(res, reps):
+    from genefaceplusplus_b200.renderer import RADNeRFTorso, RADNeRFTorsowithSR, _NativeEncoders
+    from genefaceplusplus_b200.scene import convert_poses
+    from oracle import make_torso_grid_golden as mtg
+    enc = _NativeEncoders()
+    for kind in ("torso", "torso_sr"):
+        inp = mtg.inputs(kind, 128)
+        m = (RADNeRFTorsowithSR if kind == "torso_sr" else RADNeRFTorso)(inp["hp"])
+        m.load_state_dict(inp["state"], strict=True)
+        m = m.cuda().eval()
+        m.encoders = enc
+        nets = [m.torso_deform_net, m.torso_canonicial_net] + ([m.head_color_weights_encoder] if kind == "torso_sr" else [])
+        macs = sum(p.numel() for net in nets for n_, p in net.named_parameters() if n_.endswith("weight"))
+        cond = (inp["lm68s"][mtg.POSE_INDEX] if kind == "torso_sr" else convert_poses(inp["poses"][mtg.POSE_INDEX].view(1, 4, 4)).view(6)).cuda()
+        code, noise = inp["code"].cuda(), inp["noise"].cuda()
+        g0 = m.density_grid_torso.clone()
+        ms = _median_ms(lambda: m.refresh_torso_grid(cond, code, noise, 0.95).item(), reps)
+        res[f"{kind}_cells"] = 128 * 128
+        res[f"{kind}_algorithmic_mflop"] = round(128 * 128 * 2 * macs / 1e6, 1)
+        res[f"{kind}_native_refresh_ms"] = round(ms, 3)
+        res[f"{kind}_native_launches_per_call"] = m.last_launch_count
+        m.density_grid_torso.copy_(g0)
+        with torch.no_grad():
+            res[f"{kind}_eager_libgfpp_ops_ms"] = round(_median_ms(lambda: eager_torso_refresh(m, enc, cond, code, noise, 0.95), reps), 3)
+
+
 def measure(reps=5):
     from genefaceplusplus_b200 import backend_shims
     from oracle import make_grid_golden as mg
@@ -134,6 +201,7 @@ def measure(reps=5):
         res["eager_reference_kernels_ms"] = round(_median_ms(lambda: eager_refresh(m, ref_ge, ref_rm, cf, noise, mg.DECAY), reps), 3)
     else:
         res["eager_reference_kernels_ms"] = "oracle/_ref/*.so not present"
+    measure_torso(res, reps)
     return res
 
 
