@@ -8,6 +8,7 @@
 
 #include "../../include/gfpp.h"
 #include "common.cuh"
+#include "field_train_kernel.cuh"
 #include "head_kernel.cuh"
 #include "launch.cuh"
 #include "sr_kernel.cuh"
@@ -1439,6 +1440,106 @@ int gfpp_torso_sr_set_threshold(gfpp_torso_sr_model *model, float density_thresh
     if (m.magic != kTorsoSrMagic) return fail(GFPP_ERR_INVALID, "torso_sr_set_threshold: model handle not initialised by gfpp_torso_sr_pack%s");
     m.density_thresh_torso = density_thresh_torso;
     memcpy(model, &m, sizeof(m));
+    return GFPP_OK;
+}
+
+// ---------------------------------------------------------------- (G) trainable head field
+static uint32_t field_ctas(uint32_t M) {
+    const uint32_t tiles = (M + FIELD_TP - 1) / FIELD_TP;
+    return tiles < (uint32_t)FIELD_CTAS ? tiles : (uint32_t)FIELD_CTAS;
+}
+static size_t field_wt_bytes() { return (FieldWt::total * 4 + 255) / 256 * 256; }
+
+// Validates the desc (everything the kernels read from it) and fills the model half of FieldArgs; no CUDA call.
+static int field_setup(const char *who, const gfpp_model_desc *d, FieldArgs &a) {
+    if (!d) return fail(GFPP_ERR_INVALID, "%s: null desc", who);
+    memset(&a, 0, sizeof(a));
+    const gfpp_grid_desc *gd[2] = {&d->position_grid, &d->ambient_grid};
+    GridMeta *gm[2] = {&a.pos_gm, &a.amb_gm};
+    for (int i = 0; i < 2; ++i) {
+        if (!gd[i]->embeddings || !gd[i]->offsets_host) return fail(GFPP_ERR_INVALID, "%s: null grid table or offsets", who);
+        if (gd[i]->num_levels != 16 ||
+            fill_grid_meta(*gm[i], gd[i]->offsets_host, gd[i]->input_dim, gd[i]->num_levels, gd[i]->log2_per_level_scale, gd[i]->base_resolution,
+                           gd[i]->gridtype, gd[i]->align_corners, gd[i]->interp) != 0)
+            return fail(GFPP_ERR_UNSUPPORTED, "%s: grids must have 16 levels x 2 features, 2-D or 3-D", who);
+        if (((uintptr_t)gd[i]->embeddings & 7u) != 0) return fail(GFPP_ERR_INVALID, "%s: grid tables must be 8-byte aligned", who);
+    }
+    if (a.pos_gm.dim != 3) return fail(GFPP_ERR_UNSUPPORTED, "%s: the position grid must be 3-D", who);
+    const float *w[8] = {d->ambient_w[0], d->ambient_w[1], d->ambient_w[2], d->sigma_w[0], d->sigma_w[1], d->sigma_w[2], d->color_w[0], d->color_w[1]};
+    for (int i = 0; i < 8; ++i) {
+        if (!w[i]) return fail(GFPP_ERR_INVALID, "%s: null weight", who);
+        if (!aligned16(w[i])) return fail(GFPP_ERR_INVALID, "%s: weights must be 16-byte aligned", who);
+        a.w[i] = w[i];
+    }
+    if (d->cond_dim != 64) return fail(GFPP_ERR_UNSUPPORTED, "%s: cond_dim must be 64", who);
+    if (d->ind_dim > 16 || d->ind_dim % 4 != 0) return fail(GFPP_ERR_UNSUPPORTED, "%s: ind_dim must be 0, 4, 8, 12 or 16", who);
+    if ((d->ind_dim > 0) != (d->individual_code != nullptr)) return fail(GFPP_ERR_INVALID, "%s: individual_code must be given iff ind_dim > 0", who);
+    if (d->mlp_precision != 0) return fail(GFPP_ERR_UNSUPPORTED, "%s: the training field runs in fp32 only (mlp_precision 0)", who);
+    a.pos_tab = (const float2 *)d->position_grid.embeddings;
+    a.amb_tab = (const float2 *)d->ambient_grid.embeddings;
+    a.code = d->individual_code;
+    a.ind_dim = (int)d->ind_dim;
+    a.amb_dim = (int)a.amb_gm.dim;
+    a.bound = d->bound;
+    return GFPP_OK;
+}
+
+size_t gfpp_field_backward_workspace_bytes(uint32_t M) {
+    if (M >= (1u << 30)) return 0;
+    return field_wt_bytes() + (size_t)field_ctas(M) * FieldPart::total * 4;
+}
+
+int gfpp_field_forward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat, float *sigma,
+                       float *color, float *ambient_pos, void *workspace, size_t workspace_bytes, void *stream) {
+    FieldArgs a;
+    const int rc = field_setup("field_forward", desc, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xyzs || !dirs || !cond_feat || !sigma || !color || !ambient_pos || !workspace) return fail(GFPP_ERR_INVALID, "field_forward: null pointer%s");
+    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "field_forward: M must be < 2^30%s");
+    if (workspace_bytes < field_wt_bytes()) return fail(GFPP_ERR_WORKSPACE, "field_forward: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "field_forward: workspace must be 256-byte aligned%s");
+    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    a.wt = (float *)workspace;
+    a.sigma = sigma; a.color = color; a.ambient = ambient_pos;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_field_relayout(a, st));
+    CK(launch_field_fwd(a, st));
+    return GFPP_OK;
+}
+
+int gfpp_field_backward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat,
+                        const float *grad_sigma, const float *grad_color, const float *grad_ambient_pos, float *const grad_w[8], float *grad_cond,
+                        float *grad_code, float *grad_position_table, float *grad_ambient_table, void *workspace, size_t workspace_bytes,
+                        void *stream) {
+    FieldArgs a;
+    const int rc = field_setup("field_backward", desc, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xyzs || !dirs || !cond_feat || !grad_sigma || !grad_color || !grad_ambient_pos || !grad_w || !grad_cond || !grad_position_table ||
+        !grad_ambient_table || !workspace || (a.ind_dim > 0 && !grad_code))
+        return fail(GFPP_ERR_INVALID, "field_backward: null pointer%s");
+    for (int i = 0; i < 8; ++i)
+        if (!grad_w[i]) return fail(GFPP_ERR_INVALID, "field_backward: null weight gradient%s");
+    if (((uintptr_t)grad_position_table & 7u) || ((uintptr_t)grad_ambient_table & 7u))
+        return fail(GFPP_ERR_INVALID, "field_backward: table gradients must be 8-byte aligned%s");
+    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "field_backward: M must be < 2^30%s");
+    if (workspace_bytes < gfpp_field_backward_workspace_bytes(M)) return fail(GFPP_ERR_WORKSPACE, "field_backward: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "field_backward: workspace must be 256-byte aligned%s");
+    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    a.wt = (float *)workspace;
+    a.part = (float *)((char *)workspace + field_wt_bytes());
+    a.n_cta = field_ctas(M);
+    a.g_sigma = grad_sigma; a.g_color = grad_color; a.g_ambient = grad_ambient_pos;
+    a.g_pos_tab = (float2 *)grad_position_table; a.g_amb_tab = (float2 *)grad_ambient_table;
+    for (int i = 0; i < 8; ++i) a.g_w[i] = grad_w[i];
+    a.g_cond = grad_cond; a.g_code = grad_code;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_field_relayout(a, st));
+    CK(launch_field_bwd(a, st));
+    CK(launch_field_reduce(a, st));
     return GFPP_OK;
 }
 

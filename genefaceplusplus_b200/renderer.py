@@ -9,7 +9,12 @@
   * same errors-as-exceptions behaviour.
 Everything under `render` runs in the fused sm_90a kernels of libgfpp.so through the C-ABI (include/gfpp.h).
 Only the tiny conditioning nets (AudioNet / AudioAttNet, cond_encoder.py:98-180: 5x204 -> 64) stay in PyTorch,
-as SURVEY.md 8(a) a4 prescribes.  Inference only: `self.training` raises (training is out of scope, SURVEY 2.1).
+as SURVEY.md 8(a) a4 prescribes.
+
+Training: `RADNeRF` in `.train()` mode runs the reference's training branch of `render` (renderer.py:319-339, 385-398) on libgfpp's
+training ops (train_ops.py) and its differentiable field, `RADNeRF.forward` (gfpp.h section G: fused fp32 forward and backward
+kernels), so `loss.backward()` reaches the MLP weights, both grid tables, the individual code and the conditioning nets.  The SR and
+torso classes are inference only: their `render` raises NotImplementedError in training mode.
 
 `render_clip` is the clip-level entry point (SURVEY.md 8(f) rank 1): a whole clip of poses + conditioning is
 rendered by a handful of persistent-kernel launches with rays generated in-kernel and frames kept on device.
@@ -570,10 +575,73 @@ class RADNeRF(nn.Module):
                                                              self.grid_size, self.density_grid.data_ptr(), _capi.stream_ptr(dev)),
                         "gfpp_mark_untrained_grid")
 
+    # ------------------------------------------------------------------ the differentiable field (training)
+    def forward(self, position, direction, cond_feat, individual_code, cond_mask=None):
+        """radnerf.py:108-141: (sigma [N] raw, color [N,3], ambient_pos [N,A]) at positions [N,3] in [-bound, bound] and directions
+        [N,3], for one conditioning vector [1,64] and one individual code [ind_dim] (or None).  Differentiable w.r.t. the eight MLP
+        weights, both grid tables, cond_feat and individual_code, through libgfpp's fused fp32 kernels (gfpp.h section G).  cond_mask
+        is accepted and ignored, as in the reference.  The field always runs in fp32 and returns fp32, also under torch.autocast (the
+        reference's amp: false arithmetic; its autocast field would round the MLP operands and tables to fp16)."""
+        if self.mlp_precision != "fp32":
+            raise NotImplementedError(f"the training field runs in fp32 only (mlp_precision is {self.mlp_precision!r})")
+        if position.requires_grad or direction.requires_grad:
+            raise NotImplementedError("gradients w.r.t. positions or directions (camera-pose optimisation) are not implemented")
+        if self.density_bitfield.device.type != "cuda":
+            raise _capi.GfppNoCpuPath("model is not on a CUDA device: libgfpp has no CPU path (call .cuda())")
+        from . import train_ops
+        params = ([self.ambient_net.net[i].weight for i in range(3)] + [self.sigma_net.net[i].weight for i in range(3)] +
+                  [self.color_net.net[i].weight for i in range(2)] + [self.position_embedder.embeddings, self.ambient_embedder.embeddings])
+        code = individual_code if self.individual_embedding_dim > 0 else None
+        with torch.autocast("cuda", enabled=False):
+            return train_ops.field(self, position, direction, cond_feat, code, *params)
+
+    def _render_train(self, rays_o, rays_d, cond, index, dt_gamma, bg_color, perturb, force_all_rays, max_steps, cond_mask, eye_area_percent):
+        """The training branch of renderer.py:286-339 plus the shared tail 385-398."""
+        from . import train_ops
+        dev = self.density_bitfield.device
+        if dev.type != "cuda":
+            raise _capi.GfppNoCpuPath("model is not on a CUDA device: libgfpp has no CPU path (call .cuda())")
+        prefix = rays_o.shape[:-1]
+        rays_o = rays_o.to(dev).contiguous().view(-1, 3)
+        rays_d = rays_d.to(dev).contiguous().view(-1, 3)
+        nears, fars = train_ops.near_far_from_aabb(rays_o, rays_d, self.aabb_train, self.min_near)
+        cond_feat = self.cal_cond_feat(cond.to(dev), eye_area_percent=eye_area_percent if self.forwards_eye_area else None)
+        ind_code = self.individual_embeddings[index] if self.individual_embedding_dim > 0 else None
+        counter = self.step_counter[self.local_step % 16]
+        counter.zero_()
+        self.local_step += 1
+        xyzs, dirs, deltas, rays = train_ops.march_rays_train(rays_o, rays_d, self.bound, self.density_bitfield, self.cascade, self.grid_size, nears,
+                                                              fars, counter, self.mean_count, perturb, 128, force_all_rays, dt_gamma, max_steps)
+        sigmas, rgbs, ambient = self.forward(xyzs, dirs, cond_feat, ind_code, cond_mask=cond_mask)
+        sigmas = self.density_scale * sigmas
+        weights_sum, ambient_sum, depth, image = train_ops.composite_rays_train(sigmas, rgbs, ambient.abs().sum(-1), deltas, rays)
+        results = {"weights_sum": weights_sum, "ambient": ambient_sum, "position": xyzs}
+        if bg_color is None:
+            bg_color = 1
+        elif torch.is_tensor(bg_color):
+            bg_color = bg_color.to(dev)
+        image = image + (1 - weights_sum).unsqueeze(-1) * bg_color
+        results["rgb_map"] = image.view(*prefix, 3).clamp(0, 1)
+        results["depth_map"] = (torch.clamp(depth - nears, min=0) / (fars - nears)).view(*prefix)
+        return results
+
     # ------------------------------------------------------------------ the reference's render()
-    @torch.no_grad()
+    trains_field = True   # render() has a training branch; the SR and torso subclasses do not
+
     def render(self, rays_o, rays_d, cond, bg_coords, poses, index=0, dt_gamma=0, bg_color=None, perturb=False,
                force_all_rays=False, max_steps=1024, T_thresh=1e-4, cond_mask=None, eye_area_percent=None, **kwargs):
+        """renderer.py:286-399.  In training mode: the differentiable training branch (T_thresh is not used there, as in the reference,
+        which calls composite_rays_train with its default); otherwise the fused inference renderer, without autograd."""
+        if self.training:
+            if not self.trains_field:
+                raise NotImplementedError(f"{type(self).__name__} renders for inference only; training covers the head field (RADNeRF)")
+            return self._render_train(rays_o, rays_d, cond, index, dt_gamma, bg_color, perturb, force_all_rays, max_steps, cond_mask,
+                                      eye_area_percent)
+        with torch.no_grad():
+            return self._render_eval(rays_o, rays_d, cond, bg_coords, poses, dt_gamma, bg_color, perturb, max_steps, T_thresh, cond_mask,
+                                     eye_area_percent)
+
+    def _render_eval(self, rays_o, rays_d, cond, bg_coords, poses, dt_gamma, bg_color, perturb, max_steps, T_thresh, cond_mask, eye_area_percent):
         if perturb:
             raise NotImplementedError("perturb=True is a training/GUI option; the inference driver passes False")
         # cond_mask: accepted and ignored, exactly like the reference -- its forward() / density() take the argument and never read
@@ -647,6 +715,7 @@ class RADNeRFwithSR(RADNeRF):
     the 256x256 image [1,3,256,256], `sr_rgb_map` the clamped 512x512 one (what the driver takes when `with_sr`,
     inference/genefacepp_infer.py:464-465, 480-481)."""
     sr_input_resolution = 256
+    trains_field = False
 
     def __init__(self, hparams):
         super().__init__(hparams)
@@ -1022,6 +1091,8 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
     @torch.no_grad()
     def render(self, rays_o, rays_d, cond, bg_coords, poses, index=0, dt_gamma=0, bg_color=None, perturb=False, force_all_rays=False,
                max_steps=1024, T_thresh=1e-4, upscale_torso=False, lm68=None, eye_area_percent=None, **kwargs):
+        if self.training:
+            raise NotImplementedError(f"{type(self).__name__} renders for inference only; training covers the head field (RADNeRF)")
         if perturb:
             raise NotImplementedError("perturb=True is a training/GUI option; the inference driver passes False")
         if lm68 is None:
@@ -1125,6 +1196,7 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
 # ------------------------------------------------------------------------------------------------ torso model
 class RADNeRFTorso(_TorsoGrid, RADNeRF):
     has_torso = True
+    trains_field = False
     forwards_eye_area = False
 
     def __init__(self, hparams):

@@ -7,6 +7,8 @@ meaning and autograd behaviour -- over csrc/train_kernels.cu through the C-ABI (
                                                             perturb, 128, force_all_rays, dt_gamma, max_steps)
     weights_sum, ambient_sum, depth, image = raymarching.composite_rays_train(sigmas, rgbs, ambient, deltas, rays, T_thresh)
 
+`field` is RADNeRF.forward with its gradient (include/gfpp.h section G, csrc/field_train_kernel.cu); RADNeRF.forward calls it.
+
 fp32 only (the reference casts with custom_fwd(cast_inputs=float32) as well); CUDA tensors only -- there is no CPU path.
 Differences from the reference, both deliberate: march_rays_train lays the samples out in ray order (deterministic; the
 reference's atomicAdd order changes from run to run, every consumer goes through `rays`), and nothing here calls
@@ -16,7 +18,9 @@ import numpy as np
 import torch
 from torch.autograd import Function
 
-from . import backend_shims
+import ctypes
+
+from . import _capi, backend_shims
 
 _mods = None
 
@@ -81,6 +85,16 @@ def morton3D_dilation(grid):
 
 
 # ------------------------------------------------------------------------------------------------ marching + compositing
+def near_far_from_aabb(rays_o, rays_d, aabb, min_near=0.2):
+    """raymarching.py:17-47: [N,3] x2 -> nears [N], fars [N] (both FLT_MAX on a miss)."""
+    rays_o, rays_d = _cuda_f32(rays_o).view(-1, 3), _cuda_f32(rays_d).view(-1, 3)
+    N = rays_o.shape[0]
+    nears = torch.empty(N, dtype=torch.float32, device=rays_o.device)
+    fars = torch.empty(N, dtype=torch.float32, device=rays_o.device)
+    _backend("_raymarching_face").near_far_from_aabb(rays_o, rays_d, _cuda_f32(aabb), N, min_near, nears, fars)
+    return nears, fars
+
+
 class _march_rays_train(Function):
     """raymarching.py:184-273."""
 
@@ -210,3 +224,109 @@ def grad_total_variation(embeddings, offsets, per_level_scale, base_resolution, 
         B = inputs.shape[0]
     _backend("_gridencoder").grad_total_variation(_cuda_f32(inputs), _cuda_f32(embeddings), embeddings.grad, offsets, weight, B, D, C, L,
                                                   float(np.log2(per_level_scale)), base_resolution, gridtype, align_corners)
+
+
+# ------------------------------------------------------------------------------------------------ the head field
+def _field_workspace(model, M):
+    need = _capi.lib().gfpp_field_backward_workspace_bytes(M)
+    if need == 0:
+        raise _capi.GfppError(f"the training field does not support {M} points per call")
+    dev = model.density_bitfield.device
+    ws = model.__dict__.get("_field_ws")
+    if ws is None or ws.numel() < need or ws.device != dev:
+        ws = model.__dict__["_field_ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+    return ws
+
+
+def _host_offsets(gp):
+    """The grid's level offsets as a host int32 array, copied from the device once per offsets buffer (they never change in training)."""
+    key = (gp.offsets.data_ptr(), gp.offsets._version)
+    cached = gp.__dict__.get("_host_offsets")
+    if cached is None or cached[0] != key:
+        cached = gp.__dict__["_host_offsets"] = (key, np.ascontiguousarray(gp.offsets.detach().cpu().numpy().astype(np.int32)))
+    return cached[1]
+
+
+def _field_desc(model, code, keep):
+    """The gfpp_model_desc fields section (G) reads -- grids, weights, code, cond_dim, bound, precision -- with no device-to-host copy."""
+    d = _capi.ModelDesc()
+    for name, gp in (("position_grid", model.position_embedder), ("ambient_grid", model.ambient_embedder)):
+        g = getattr(d, name)
+        lay = gp.layout
+        emb = _cuda_f32(gp.embeddings.detach())
+        off = _host_offsets(gp)
+        keep += [emb, off]
+        g.embeddings, g.offsets_host = emb.data_ptr(), off.ctypes.data
+        g.input_dim, g.num_levels, g.base_resolution = lay.input_dim, lay.num_levels, lay.base_resolution
+        g.log2_per_level_scale, g.gridtype, g.interp, g.align_corners = float(lay.S), lay.gridtype_id, lay.interp_id, int(lay.align_corners)
+    ws = [_cuda_f32(w.weight.detach()) for w in list(model.ambient_net.net) + list(model.sigma_net.net) + list(model.color_net.net)]
+    keep += ws
+    for i in range(3):
+        d.ambient_w[i], d.sigma_w[i] = ws[i].data_ptr(), ws[3 + i].data_ptr()
+    d.color_w[0], d.color_w[1] = ws[6].data_ptr(), ws[7].data_ptr()
+    d.individual_code = code.data_ptr() if code is not None else None
+    d.cond_dim, d.ind_dim = model.cond_out_dim, model.individual_embedding_dim
+    d.bound = float(model.bound)
+    d.mlp_precision = 0
+    return d
+
+
+class _field(Function):
+    """RADNeRF.forward (radnerf.py:108-141) over gfpp_field_forward / gfpp_field_backward: (xyzs [M,3], dirs [M,3], cond_feat [64] or
+    [1,64], code [ind_dim] or None) -> (sigma [M], color [M,3], ambient_pos [M,A]).  `params` are the eight MLP weights and the two grid
+    tables of `model`, passed so that autograd routes their gradients; the kernels read them in place.  No gradient reaches xyzs or
+    dirs (the caller rejects inputs that require one)."""
+
+    @staticmethod
+    def forward(ctx, model, xyzs, dirs, cond_feat, code, *params):
+        x, dr = _cuda_f32(xyzs).view(-1, 3), _cuda_f32(dirs).view(-1, 3)
+        if cond_feat.numel() != model.cond_out_dim:
+            raise ValueError(f"cond_feat must hold one conditioning vector of {model.cond_out_dim} values, got shape {tuple(cond_feat.shape)}")
+        if (code is None) != (model.individual_embedding_dim == 0) or (code is not None and code.numel() != model.individual_embedding_dim):
+            raise ValueError(f"individual_code must hold {model.individual_embedding_dim} values (None iff the model has no codes)")
+        c = _cuda_f32(cond_feat).reshape(-1)
+        cd = _cuda_f32(code).reshape(-1) if code is not None else None
+        M, A, dev = x.shape[0], model.ambient_coord_dim, x.device
+        sigma = torch.empty(M, dtype=torch.float32, device=dev)
+        color = torch.empty(M, 3, dtype=torch.float32, device=dev)
+        amb = torch.empty(M, A, dtype=torch.float32, device=dev)
+        keep = []
+        d = _field_desc(model, cd, keep)
+        ws = _field_workspace(model, 0)
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_field_forward(ctypes.byref(d), x.data_ptr(), dr.data_ptr(), M, c.data_ptr(), sigma.data_ptr(), color.data_ptr(),
+                                                       amb.data_ptr(), ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_field_forward")
+        ctx.model = model
+        ctx.shapes = (cond_feat.shape, None if code is None else code.shape)
+        ctx.save_for_backward(x, dr, c, cd if cd is not None else torch.empty(0, device=dev), *params)
+        return sigma, color, amb
+
+    @staticmethod
+    def backward(ctx, g_sigma, g_color, g_amb):
+        x, dr, c, cd, *params = ctx.saved_tensors
+        model = ctx.model
+        cond_shape, code_shape = ctx.shapes
+        M, dev = x.shape[0], x.device
+        g_sigma = torch.zeros(M, device=dev) if g_sigma is None else _cuda_f32(g_sigma)
+        g_color = torch.zeros(M, 3, device=dev) if g_color is None else _cuda_f32(g_color)
+        g_amb = torch.zeros(M, model.ambient_coord_dim, device=dev) if g_amb is None else _cuda_f32(g_amb)
+        alloc = torch.zeros if M == 0 else torch.empty
+        grad_w = [alloc(p.shape, dtype=torch.float32, device=dev) for p in params[:8]]
+        g_pos = torch.zeros(params[8].shape, dtype=torch.float32, device=dev)
+        g_tab = torch.zeros(params[9].shape, dtype=torch.float32, device=dev)
+        g_cond = alloc(c.shape, dtype=torch.float32, device=dev)
+        g_code = alloc(cd.shape, dtype=torch.float32, device=dev) if code_shape is not None else None
+        keep = []
+        d = _field_desc(model, cd if code_shape is not None else None, keep)
+        ws = _field_workspace(model, M)
+        ptrs = (ctypes.c_void_p * 8)(*[g.data_ptr() for g in grad_w])
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_field_backward(ctypes.byref(d), x.data_ptr(), dr.data_ptr(), M, c.data_ptr(), g_sigma.data_ptr(),
+                                                        g_color.data_ptr(), g_amb.data_ptr(), ctypes.byref(ptrs), g_cond.data_ptr(),
+                                                        None if g_code is None else g_code.data_ptr(), g_pos.data_ptr(), g_tab.data_ptr(),
+                                                        ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_field_backward")
+        grads = [g.to(p.dtype) for g, p in zip(grad_w + [g_pos, g_tab], params)]
+        return (None, None, None, g_cond.view(cond_shape), None if g_code is None else g_code.view(code_shape), *grads)
+
+
+field = _field.apply

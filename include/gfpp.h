@@ -33,6 +33,8 @@
  *  (E) occupancy-grid maintenance of the head models: density query, grid refresh, mark_untrained_grid.
  *
  *  (F) the torso models' occupancy grid: torso field query and density_grid_torso refresh, threshold setters.
+ *
+ *  (G) the trainable head field: RADNeRF.forward and its backward at explicit points, fp32.
  */
 #ifndef GFPP_H_
 #define GFPP_H_
@@ -434,6 +436,40 @@ GFPP_API int gfpp_torso_sr_grid_update(const gfpp_torso_sr_model *model, const f
                                        size_t workspace_bytes, void *stream);
 GFPP_API int gfpp_model_set_torso_threshold(gfpp_model *model, float density_thresh_torso);
 GFPP_API int gfpp_torso_sr_set_threshold(gfpp_torso_sr_model *model, float density_thresh_torso);
+
+/* ------------------------------------------------------------------ (G) trainable head field
+ *
+ * RADNeRF.forward (modules/radnerfs/radnerf.py:108-141) and its gradient for the training step, in fp32 FFMA arithmetic (the
+ * reference's amp: false), reading the parameters IN PLACE through a gfpp_model_desc -- no gfpp_model_pack: the weights change
+ * after every optimizer step.  Read from the desc: both grids (reference layout [entries,2] fp32, 8-byte aligned; 16 levels x 2;
+ * position 3-D, ambient 2-D or 3-D), the eight nn.Linear weights [out, in] (16-byte aligned; the May shapes of gfpp_model_pack),
+ * individual_code [ind_dim] (the training row individual_embeddings[index]; NULL iff ind_dim == 0; ind_dim 0, 4, 8, 12 or 16),
+ * cond_dim (64), bound and mlp_precision (must be 0).  Anything else returns GFPP_ERR_UNSUPPORTED or GFPP_ERR_INVALID.  The other
+ * desc fields are not read.  Every argument is validated before any CUDA call; M == 0 then returns GFPP_OK without touching the
+ * device (the data pointers may be NULL).  Everything is enqueued on `stream` with no host synchronisation and no allocation.
+ *
+ * Workspace (256-byte aligned): gfpp_field_backward_workspace_bytes(M) for the backward (0 = unsupported M); the forward needs
+ * gfpp_field_backward_workspace_bytes(0) bytes (the per-call k-major copy of the weights, ~320 KB), so a backward workspace fits both.
+ *
+ * gfpp_field_forward: for points xyzs [M,3] in [-bound, bound], dirs [M,3], one cond_feat [64]:
+ *   sigma [M] = exp(h0) raw (density_scale is the caller's, renderer.py:376), color [M,3] (sigmoid), ambient_pos [M,A] (tanh).
+ * gfpp_field_backward: given grad_sigma [M] (w.r.t. the raw sigma), grad_color [M,3] and grad_ambient_pos [M,A] (the ambient
+ *   regulariser's gradient enters there), recomputes the forward and writes
+ *     grad_w[0..7]  the gradients of ambient_w[0..2], sigma_w[0..2], color_w[0..1], same [out, in] layout (overwritten);
+ *     grad_cond [64] (cond_feat is repeated over the points: its gradient is the sum), grad_code [ind_dim] (NULL iff ind_dim == 0);
+ *     grad_position_table / grad_ambient_table [entries,2]: ACCUMULATED into (+=), as the reference's grid backward does.
+ *   trunc_exp' = exp(clamp(h0, -15, 15)); the ambient grid's input gradient goes through its dy_dx and the (x+1)/2 map of bound 1;
+ *   the position grid gets no input gradient (xyzs never requires grad in the reference).
+ * Determinism: the forward outputs, grad_w, grad_cond and grad_code are bit-identical from run to run (per-CTA partial sums in the
+ * workspace, reduced in a fixed order by one kernel; the partitioning depends only on M).  The two table gradients are scattered
+ * with float2 vector reductions, so their summation order is free. */
+GFPP_API size_t gfpp_field_backward_workspace_bytes(uint32_t M);
+GFPP_API int gfpp_field_forward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat,
+                                float *sigma, float *color, float *ambient_pos, void *workspace, size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_field_backward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat,
+                                 const float *grad_sigma, const float *grad_color, const float *grad_ambient_pos, float *const grad_w[8],
+                                 float *grad_cond, float *grad_code, float *grad_position_table, float *grad_ambient_table, void *workspace,
+                                 size_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }
