@@ -55,7 +55,7 @@ class Frames(ctypes.Structure):
                 ("poses_c2w", c_void_p), ("fx", c_f), ("fy", c_f), ("cx", c_f), ("cy", c_f),
                 ("img_h", c_u32), ("img_w", c_u32), ("cond_feat", c_void_p), ("torso_pose6", c_void_p),
                 ("bg_coords", c_void_p), ("bg_color", c_void_p), ("dt_gamma", c_f), ("max_steps", c_u32),
-                ("T_thresh", c_f)]
+                ("T_thresh", c_f), ("noises", c_void_p)]
 
 
 class SrDesc(ctypes.Structure):

@@ -656,6 +656,7 @@ int gfpp_render_frames(const gfpp_model *model, const gfpp_frames *fr, const gfp
     a.fx = fr->fx; a.fy = fr->fy; a.cx = fr->cx; a.cy = fr->cy; a.img_w = (int)fr->img_w;
     a.cond_feat = fr->cond_feat;
     a.max_steps = (int)fr->max_steps; a.T_thresh = fr->T_thresh;
+    a.noises = fr->noises;
     a.image = (float *)(ws + W.image);
     a.wsum = out->weights_sum ? out->weights_sum : (float *)(ws + W.wsum);
     a.depth = out->depth_map ? out->depth_map : (float *)(ws + W.depth);

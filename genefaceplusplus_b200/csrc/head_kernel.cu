@@ -548,7 +548,10 @@ __global__ void __launch_bounds__(256) k_ray_setup(const __grid_constant__ HeadA
         sl.frame = gid / a.n_rays;
         load_ray(a, sl.frame, gid - sl.frame * a.n_rays, sl.g);
         near_far(sl.g, a.aabb, a.min_near, sl.near, sl.far);
-        sl.t = sl.near;
+        // perturb: the reference jitters only the first round's start (renderer.py:370, raymarching.cu:873); every later round
+        // resumes from rays_t, so the whole ray is the continuous march from this start.  [near, far] stays the slab interval
+        // (depth normalisation, may_hit_occupied): the jittered segment lies inside it.
+        sl.t = a.noises ? __fadd_rn(sl.near, __fmul_rn(step_len(mc, sl.near), a.noises[gid])) : sl.near;
         int budget = 1 << 30;
         const bool hit = may_hit_occupied(have_box, occ_lo, occ_hi, sl.g, sl.near, sl.far, sl.far_m) &&
                          march_budget(mc, sl.g, sl.far_m, sl.t, budget) == 1;

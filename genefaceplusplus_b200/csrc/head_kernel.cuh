@@ -50,6 +50,8 @@ struct HeadArgs {
     int *valid_samples;             // [F] statistics (or nullptr)
     int pass;                       // 1 or 2
     unsigned long long *phase_cycles;  // optional [32]: per-phase cycle totals of thread 0 of every CTA (diagnostics)
+    // ---- appended last so the offsets above stay put ----
+    const float *noises;            // [F,N] in [0,1): jittered ray starts (k_ray_setup), or nullptr = start at near
 };
 
 // tensor-core variant: pre-swizzled 16-bit weight tiles (see pack_tc_weights in capi.cu)

@@ -341,10 +341,13 @@ class RADNeRF(nn.Module):
     # ------------------------------------------------------------------ core call
     def render_frames(self, cond_feat, *, rays_o=None, rays_d=None, poses_c2w=None, intrinsics=None, H=None, W=None,
                       pose6=None, bg_coords=None, bg_color=None, dt_gamma=0.0, max_steps=1024, T_thresh=1e-4,
-                      want_torso_maps=True, want_stats=False, rgb_out=None, u8_out=None, want_aux=True):
+                      want_torso_maps=True, want_stats=False, rgb_out=None, u8_out=None, want_aux=True, noise=None):
         """Render F frames with one call into libgfpp.  Returns a dict of device tensors with a leading F axis.
 
         Either (rays_o, rays_d) [F,N,3] or (poses_c2w [F,4,4], intrinsics, H, W) must be given.
+        noise: optional fp32 [F,N] (any shape of F*N values) in [0,1) on the model's device: jittered ray starts, ray i of frame f
+        begins marching at near + clamp(near*dt_gamma, dt_min, dt_max) * noise[f,i] (the first-round `noises` of the reference's
+        march_rays, raymarching.py:388-392).  None = start at near, as perturb=False does.
         rgb_out: optional contiguous fp32 [F,N,3] device view the kernel writes `rgb_map` into (e.g. a slice of the clip buffer:
         no copy afterwards); u8_out: optional contiguous uint8 [F,N,3] view that receives the video frame `(rgb*255).int()`
         straight from the epilogue kernel -- with u8_out and no rgb_out no fp32 frame is written at all.
@@ -399,6 +402,12 @@ class RADNeRF(nn.Module):
             fr.bg_color = bg_color.data_ptr()
             hold.append(bg_color)
         fr.dt_gamma, fr.max_steps, fr.T_thresh = float(dt_gamma), int(max_steps), float(T_thresh)
+        if noise is not None:
+            if not torch.is_tensor(noise) or noise.numel() != Fn * N:
+                raise ValueError(f"noise must hold {Fn}*{N} values (one per ray and frame)")
+            noise = noise.to(dev, f32).reshape(Fn, N).contiguous()
+            fr.noises = noise.data_ptr()
+            hold.append(noise)
 
         out = _capi.Outputs()
         res = {}
@@ -631,7 +640,9 @@ class RADNeRF(nn.Module):
     def render(self, rays_o, rays_d, cond, bg_coords, poses, index=0, dt_gamma=0, bg_color=None, perturb=False,
                force_all_rays=False, max_steps=1024, T_thresh=1e-4, cond_mask=None, eye_area_percent=None, **kwargs):
         """renderer.py:286-399.  In training mode: the differentiable training branch (T_thresh is not used there, as in the reference,
-        which calls composite_rays_train with its default); otherwise the fused inference renderer, without autograd."""
+        which calls composite_rays_train with its default); otherwise the fused inference renderer, without autograd.  perturb=True
+        outside training (the reference's validation_step) jitters each ray's start with one torch.rand(N) draw on the model's
+        device, as the reference's first march_rays round does (_ray_start_noise)."""
         if self.training:
             if not self.trains_field:
                 raise NotImplementedError(f"{type(self).__name__} renders for inference only; training covers the head field (RADNeRF)")
@@ -641,9 +652,18 @@ class RADNeRF(nn.Module):
             return self._render_eval(rays_o, rays_d, cond, bg_coords, poses, dt_gamma, bg_color, perturb, max_steps, T_thresh, cond_mask,
                                      eye_area_percent)
 
+    def _ray_start_noise(self, n_rays):
+        """perturb=True outside training (the reference's validation_step): the first round of renderer.py:354-384 passes
+        `perturb` to march_rays, which draws torch.rand(n_alive) with all N rays alive (raymarching.py:388-390); later rounds pass
+        False and draw nothing.  One draw of N values on the model's device, made before any later draw of the same call (the
+        SR head's random noise planes), so a seeded call consumes the generator exactly as the reference does."""
+        dev = self.density_bitfield.device
+        if dev.type != "cuda":
+            raise _capi.GfppNoCpuPath("model is not on a CUDA device: libgfpp has no CPU path (call .cuda())")
+        return torch.rand(n_rays, dtype=torch.float32, device=dev)
+
     def _render_eval(self, rays_o, rays_d, cond, bg_coords, poses, dt_gamma, bg_color, perturb, max_steps, T_thresh, cond_mask, eye_area_percent):
-        if perturb:
-            raise NotImplementedError("perturb=True is a training/GUI option; the inference driver passes False")
+        # perturb: jittered ray starts (_ray_start_noise); the jitter moves where each ray starts marching, nothing else
         # cond_mask: accepted and ignored, exactly like the reference -- its forward() / density() take the argument and never read
         # it (radnerf.py:108-141, 143-165); the only requirement renderer.py:371-372 puts on it is one entry per ray
         if cond_mask is not None and torch.is_tensor(cond_mask) and cond_mask.shape[0] != rays_o.numel() // 3:
@@ -653,9 +673,10 @@ class RADNeRF(nn.Module):
             raise ValueError("render() assumes B == 1 (renderer.py:287)")
         cond_feat = self.cal_cond_feat(cond.to(self.density_bitfield.device),
                                        eye_area_percent=eye_area_percent if self.forwards_eye_area else None)
+        noise = self._ray_start_noise(rays_o.numel() // 3) if perturb else None
         res = self.render_frames(cond_feat.reshape(1, -1), rays_o=rays_o.reshape(1, -1, 3), rays_d=rays_d.reshape(1, -1, 3),
                                  pose6=poses if self.has_torso else None, bg_coords=bg_coords if self.has_torso else None,
-                                 bg_color=bg_color, dt_gamma=dt_gamma, max_steps=max_steps, T_thresh=T_thresh)
+                                 bg_color=bg_color, dt_gamma=dt_gamma, max_steps=max_steps, T_thresh=T_thresh, noise=noise)
         results = {"depth_map": res["depth_map"].view(*prefix), "rgb_map": res["rgb_map"].view(*prefix, 3),
                    "weights_sum": res["weights_sum"].view(-1)}
         if self.has_torso:
@@ -1080,12 +1101,13 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
         del hold
         return res
 
-    def _head(self, rays_o, rays_d, cond_feat, dt_gamma, max_steps, T_thresh):
-        """Premultiplied head colour, alpha and normalised depth of one frame from libgfpp (background 0 => rgb_map == image)."""
+    def _head(self, rays_o, rays_d, cond_feat, dt_gamma, max_steps, T_thresh, noise=None):
+        """Premultiplied head colour, alpha and normalised depth of one frame from libgfpp (background 0 => rgb_map == image).
+        noise: optional [N] jittered ray starts (render_frames)."""
         N = rays_o.numel() // 3
         res = self.render_frames(cond_feat.reshape(1, -1), rays_o=rays_o.reshape(1, -1, 3), rays_d=rays_d.reshape(1, -1, 3),
                                  bg_color=torch.zeros(N, 3, device=self.density_bitfield.device), dt_gamma=dt_gamma,
-                                 max_steps=max_steps, T_thresh=T_thresh)
+                                 max_steps=max_steps, T_thresh=T_thresh, noise=noise)
         return res["rgb_map"].view(N, 3), res["weights_sum"].view(N), res["depth_map"].view(N)
 
     @torch.no_grad()
@@ -1093,8 +1115,6 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
                max_steps=1024, T_thresh=1e-4, upscale_torso=False, lm68=None, eye_area_percent=None, **kwargs):
         if self.training:
             raise NotImplementedError(f"{type(self).__name__} renders for inference only; training covers the head field (RADNeRF)")
-        if perturb:
-            raise NotImplementedError("perturb=True is a training/GUI option; the inference driver passes False")
         if lm68 is None:
             raise ValueError("the torso-SR field is conditioned on lm68 (radnerf_torso_sr.py:84)")
         R = self.sr_input_resolution
@@ -1107,7 +1127,9 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
         dev = self.density_bitfield.device
         with torch.autocast(dev.type, enabled=False):
             cond_feat = self.cal_cond_feat(cond.to(dev), eye_area_percent=eye_area_percent)
-            image, weights_sum, depth = self._head(rays_o.to(dev), rays_d.to(dev), cond_feat, dt_gamma, max_steps, T_thresh)
+            # perturb: the marching draw comes first, the SR head's noise planes after it (radnerf_torso_sr.py:166-181 marches first)
+            jitter = {"noise": self._ray_start_noise(N)} if perturb else {}
+            image, weights_sum, depth = self._head(rays_o.to(dev), rays_d.to(dev), cond_feat, dt_gamma, max_steps, T_thresh, **jitter)
             bg_coords = bg_coords.to(dev).contiguous().view(-1, 2)
             bg = 1 if bg_color is None else (bg_color.to(dev).reshape(-1, 3) if torch.is_tensor(bg_color) else bg_color)
             code = self.torso_individual_codes[0] if self.torso_individual_embedding_dim > 0 else None

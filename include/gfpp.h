@@ -181,6 +181,7 @@ typedef struct {
     float dt_gamma;
     uint32_t max_steps;
     float T_thresh;
+    const float *noises;          /* [F,N] in [0,1), or NULL = no jitter (renderer.py:370, raymarching.py:388-392) */
 } gfpp_frames;
 
 typedef struct {
