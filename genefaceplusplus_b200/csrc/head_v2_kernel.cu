@@ -12,7 +12,9 @@
 //   * the weight stream is SHARED: the loader warp copies each tile once (NSTAGE-deep ring) for all slots; a stage is refilled
 //     once every owner warp has arrived on `w_free`;
 //   * the 3-wide outputs and the sigma logit are N=16 MMAs against small RESIDENT tiles, handed to the row owners through a
-//     small buffer at the head of the slot's second operand tile.
+//     small buffer at the head of the slot's second operand tile (the sigma logit through a per-row buffer of its own);
+//   * the CTA is whole warpgroups: NSLOT owner warpgroups and one producer warpgroup, whose registers (setmaxnreg) go to
+//     the owners.
 //
 // Precision modes: FP16_X1 (the reference's autocast arithmetic) with 3 slots, and FP16_ROBUST with 2 slots: fp16 hi/lo
 // split (3 MMAs per k-step, ~22 mantissa bits) on the ambient net and a 16-bit fixed-point position table (gather8.cuh) --
@@ -42,7 +44,14 @@ struct Cfg {
     static constexpr int NSTAGE = 4;   // >= 4: a robust ambient layer waits for four tiles at once
     static constexpr int NTILE = ROBUST ? V2_NTILE_ROBUST : V2_NTILE_X1;
     static constexpr int NWORK = 4 * NSLOT;                 // row-owner warps
-    static constexpr int NT = 32 * (NWORK + 1);             // + loader warp
+    static constexpr int NT = 128 * (NSLOT + 1);            // + one producer warpgroup: its warp 0 is the loader
+    // register split (setmaxnreg): the owner warpgroups grow to OWNER_REGS, the producer warpgroup shrinks to PRODUCER_REGS.
+    // The launch allocates 65536 / NT per thread (128 | 168); the owners' increase is served by the producer's decrease.
+    static constexpr int OWNER_REGS = ROBUST ? 232 : 160, PRODUCER_REGS = ROBUST ? 40 : 24;
+    static constexpr int LAUNCH_REGS = (65536 / NT) & ~7;
+    static_assert(NSLOT * 128 * OWNER_REGS + 128 * PRODUCER_REGS <= 65536, "register split exceeds the register file");
+    static_assert(NSLOT * 128 * (OWNER_REGS - LAUNCH_REGS) <= 128 * (LAUNCH_REGS - PRODUCER_REGS), "owners grow by more than the producer frees");
+    static_assert(OWNER_REGS % 8 == 0 && PRODUCER_REGS % 8 == 0 && PRODUCER_REGS >= 24 && OWNER_REGS <= 256, "setmaxnreg operand");
     static constexpr int SLOT_BYTES = (ROBUST ? 4 : 2) * V2_TILE_BYTES + 4096;   // h0 h1 [l0 l1] sh
     static constexpr int OFF_W = NSLOT * SLOT_BYTES;
     static constexpr int OFF_RES = OFF_W + NSTAGE * V2_TILE_BYTES;
@@ -53,13 +62,20 @@ struct Misc {
     float cbias[128];                    // color L0 bias (individual code folded)
     uint32_t coarse[HEAD_COARSE_WORDS];
     uint4 lvl[2][2 * GFPP_MAX_LEVELS];
+    MarchConst mc;
+    float occ_lo[3], occ_hi[3];
+    bool have_box;
     unsigned long long w_full[4], w_free[4], res_full, batch_bar;
     volatile int stop;
     volatile int flag[2][16];            // per batch parity, per owner warp: "I have live rows"
 };
 
+// the sigma logits of a slot's rows, from sigma L2 to the row owners (TM floats per slot): the robust mode keeps them at the
+// head of the slot's residual tile l (idle from ambient out to the next batch's operand rows), fp16 behind Misc
 template <bool ROBUST>
-constexpr size_t smem_bytes() { return (size_t)Cfg<ROBUST>::OFF_MISC + sizeof(Misc) + 1024; }
+constexpr size_t slogit_bytes() { return ROBUST ? 0 : (size_t)Cfg<ROBUST>::NSLOT * TM * sizeof(float); }
+template <bool ROBUST>
+constexpr size_t smem_bytes() { return (size_t)Cfg<ROBUST>::OFF_MISC + sizeof(Misc) + slogit_bytes<ROBUST>() + 1024; }
 static_assert(smem_bytes<false>() <= 227 * 1024 && smem_bytes<true>() <= 227 * 1024, "v2 shared memory budget");
 
 // Epilogue of one M = 64 half (rows 64*half ..) of a 128-wide layer from the accumulator fragment: (+bias) -> (ReLU) ->
@@ -76,6 +92,12 @@ __device__ __forceinline__ void epilogue_half(const float (&d)[64], unsigned cha
         store_pair<false, LO>(h + (col >> 6) * V2_TILE_BYTES, l + (LO ? (col >> 6) * V2_TILE_BYTES : 0), row, col & 63, x0, x1);
     }
 }
+
+// per-thread register budget of the executing warpgroup (all four warps, converged)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 __device__ __forceinline__ float2 unpack_h2(uint32_t h) { return __half22float2(*reinterpret_cast<const __half2 *>(&h)); }
 
@@ -122,16 +144,15 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
     // ---------------- one-time setup ----------------
-    MarchConst mc = a.mc;
-    float occ_lo[3] = {0.f, 0.f, 0.f}, occ_hi[3] = {0.f, 0.f, 0.f};
-    const bool have_box = setup_occupancy(a, mc, occ_lo, occ_hi);
-    if (a.coarse_bits && a.coarse_words <= HEAD_COARSE_WORDS) {
+    const bool coarse_in_smem = a.coarse_bits && a.coarse_words <= HEAD_COARSE_WORDS;
+    if (coarse_in_smem)
         for (int i = tid; i < a.coarse_words; i += C::NT) ms.coarse[i] = a.coarse_bits[i];
-        mc.coarse = ms.coarse;
-    } else {
-        mc.coarse = a.coarse_bits;
-    }
     if (tid == 0) {
+        // marching constants and the occupied box in shared memory, not in ~25 registers of every owner thread
+        ms.mc = a.mc;
+        for (int k = 0; k < 3; ++k) { ms.occ_lo[k] = 0.f; ms.occ_hi[k] = 0.f; }
+        ms.have_box = setup_occupancy(a, ms.mc, ms.occ_lo, ms.occ_hi);
+        ms.mc.coarse = coarse_in_smem ? ms.coarse : a.coarse_bits;
         for (int i = 0; i < 4; ++i) { mbar_init(&ms.w_full[i], 1); mbar_init(&ms.w_free[i], NWORK); }
         mbar_init(&ms.res_full, 1);
         mbar_init(&ms.batch_bar, NWORK);
@@ -147,6 +168,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
     const int total = (a.pass == 1) ? *a.n_hits : *a.n_survivors;
 
     if (warp < NWORK) {
+        setmaxnreg_inc<C::OWNER_REGS>();
         // =====================================================================================================
         // ROW OWNER: thread `row` of slot `s`
         //
@@ -158,10 +180,12 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         // =====================================================================================================
         const int s = warp >> 2, row = tid & (TM - 1), wwarp = warp & 3;
         unsigned char *h = sm + s * C::SLOT_BYTES, *l = h + 2 * V2_TILE_BYTES, *sht = h + (ROBUST ? 4 : 2) * V2_TILE_BYTES;
-        // live columns of the N = 16 layers, [4][TM] floats at the head of tile h1: they only overlap operand rows 0-15 of h1,
+        // live columns of the N = 16 layers, [3][TM] floats at the head of tile h1: they only overlap operand rows 0-15 of h1,
         // which half 0 has consumed before they are written and which are rewritten only after the owners have read them
         float *outc = reinterpret_cast<float *>(h + V2_TILE_BYTES);
+        float *slogit = ROBUST ? reinterpret_cast<float *>(l) : reinterpret_cast<float *>(sm + C::OFF_MISC + sizeof(Misc)) + s * TM;
         const uint32_t h_u = smem_u32(h), l_u = smem_u32(l), sh_u = smem_u32(sht), res_u = smem_u32(res), ring_u = smem_u32(wring);
+        const MarchConst &mc = ms.mc;
         uint32_t wc = 0;            // streamed tiles consumed so far (the same sequence in every slot)
         const bool smooth_p = a.pos_gm.interp == 1, smooth_a = a.amb_gm.interp == 1;
         Slot sl;
@@ -268,7 +292,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                         sl.t = a.rays_t[g]; sl.ws = a.wsum[g]; sl.depth = a.depth[g];
                         sl.r = a.image[3 * g]; sl.gch = a.image[3 * g + 1]; sl.b = a.image[3 * g + 2];
                         sl.nsamp = a.max_steps; sl.cap = a.B_total[sl.frame];
-                        (void)may_hit_occupied(have_box, occ_lo, occ_hi, sl.g, sl.near, sl.far, sl.far_m);
+                        (void)may_hit_occupied(ms.have_box, ms.occ_lo, ms.occ_hi, sl.g, sl.near, sl.far, sl.far_m);
                         live = sl.nsamp < sl.cap && march_next(mc, sl.g, sl.far_m, sl.t, sl.px, sl.py, sl.pz, sl.dt);
                         if (!live) finalize_ray(a, sl, true);
                     }
@@ -467,10 +491,9 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
             }, [&](const float (&d)[64], int hf) { epilogue_half<true, false, false>(d, h, h, hf, lane, wwarp, nullptr); });
             ARRIVE_A();   // -> sigma L2
             PH(11)  // MMA + epilogue: sigma L1
-            float slogit[2][2];   // sigma logit of fragment rows r, r+8 of each half (lanes with lane % 4 == 0)
             {   // sigma L2: 128 geo rows (streamed) + the sigma row (resident N = 16 tile)
                 const uint32_t w0 = tile(0), w1 = tile(1);
-#pragma unroll
+#pragma unroll 1
                 for (int hf = 0; hf < 2; ++hf) {
                     const uint32_t o = (uint32_t)hf * SW128_HALF;
                     float d[64], d16[8];
@@ -482,8 +505,10 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                     wg_wait<0>();
                     acc_fence(d);
                     acc_fence(d16);
-                    slogit[hf][0] = d16[0];
-                    slogit[hf][1] = d16[2];
+                    if ((lane & 3) == 0) {   // the sigma logit (column 0) of fragment rows r, r+8
+                        slogit[64 * hf + frag_row(0, lane, wwarp)] = d16[0];
+                        slogit[64 * hf + frag_row(2, lane, wwarp)] = d16[2];
+                    }
                     epilogue_half<false, false, false>(d, h, h, hf, lane, wwarp, nullptr);   // geo features (no activation) -> color-net input
                 }
                 release(2);
@@ -501,7 +526,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
             ARRIVE_A();   // -> color out (N = 16)
             PH(13)  // MMA + epilogue: color L0
 #pragma unroll
-            for (int hf = 0; hf < 2; ++hf) {   // color out: N = 16 group; the sigma logits join the rgb logits in the hand-over buffer
+            for (int hf = 0; hf < 2; ++hf) {   // color out: N = 16 group -> the hand-over buffer
                 const uint32_t o = (uint32_t)hf * SW128_HALF;
                 float d[8];
                 wg_fence();
@@ -510,15 +535,11 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                 wg_wait<0>();
                 acc_fence(d);
                 put_cols<3>(d, outc, 0, hf, lane, wwarp);
-                if ((lane & 3) == 0) {
-                    outc[3 * TM + 64 * hf + frag_row(0, lane, wwarp)] = slogit[hf][0];
-                    outc[3 * TM + 64 * hf + frag_row(2, lane, wwarp)] = slogit[hf][1];
-                }
             }
             wg_sync(1 + s);
             PH(14)  // MMA: color out
             // trunc_exp forward (utils.py:36-49) * density_scale (renderer.py:365)
-            const float sigma = a.density_scale * expf(outc[3 * TM + row]);
+            const float sigma = a.density_scale * expf(slogit[row]);
             const float cr = 1.0f / (1.0f + expf(-outc[row]));
             const float cg = 1.0f / (1.0f + expf(-outc[TM + row]));
             const float cb = 1.0f / (1.0f + expf(-outc[2 * TM + row]));
@@ -586,8 +607,12 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         __syncwarp();
     } else {
         // =====================================================================================================
-        // LOADER WARP: resident tiles once, then the weight stream, NSTAGE tiles ahead of the issue warp
+        // PRODUCER WARPGROUP: hands its registers to the owners; warp 0 is the LOADER, the other three leave.  No barrier
+        // counts them: `w_free` and `batch_bar` count owner warps, the named barriers the 128 threads of one slot.
         // =====================================================================================================
+        setmaxnreg_dec<C::PRODUCER_REGS>();
+        if (warp != NWORK) return;
+        // LOADER: resident tiles once, then the weight stream, NSTAGE tiles ahead of the issue warp
         if (elect_one()) {
             mbar_expect_tx(&ms.res_full, V2_RES_BYTES);
             bulk_g2s(res, t.w_res, V2_RES_BYTES, &ms.res_full);
