@@ -15,6 +15,7 @@
 #include "torso_grid_kernel.cuh"
 #include "torso_kernel.cuh"
 #include "torso_sr_kernel.cuh"
+#include "torso_train_kernel.cuh"
 
 namespace gfpp {
 // ops_kernels.cu
@@ -1541,6 +1542,107 @@ int gfpp_field_backward(const gfpp_model_desc *desc, const float *xyzs, const fl
     CK(launch_field_relayout(a, st));
     CK(launch_field_bwd(a, st));
     CK(launch_field_reduce(a, st));
+    return GFPP_OK;
+}
+
+// ---------------------------------------------------------------- (H) trainable torso field
+static uint32_t torso_field_ctas(uint32_t M) {
+    const uint32_t tiles = (M + TORSO_TRAIN_TP - 1) / TORSO_TRAIN_TP;
+    return tiles < (uint32_t)TORSO_TRAIN_CTAS ? tiles : (uint32_t)TORSO_TRAIN_CTAS;
+}
+static size_t torso_wt_bytes() { return (TorsoWt::total * 4 + 255) / 256 * 256; }
+
+// Validates the desc's torso fields, pose6 and code (everything the kernels read besides the points) and fills the model half of
+// TorsoTrainArgs; no CUDA call.
+static int torso_field_setup(const char *who, const gfpp_model_desc *d, const float *pose6, const float *code, TorsoTrainArgs &a) {
+    if (!d) return fail(GFPP_ERR_INVALID, "%s: null desc", who);
+    memset(&a, 0, sizeof(a));
+    const gfpp_grid_desc &g = d->torso_grid;
+    if (!g.embeddings || !g.offsets_host) return fail(GFPP_ERR_INVALID, "%s: null torso grid table or offsets", who);
+    if (g.num_levels != 16 ||
+        fill_grid_meta(a.gm, g.offsets_host, g.input_dim, g.num_levels, g.log2_per_level_scale, g.base_resolution, g.gridtype,
+                       g.align_corners, g.interp) != 0 || a.gm.dim != 2)
+        return fail(GFPP_ERR_UNSUPPORTED, "%s: the torso grid must be 2-D with 16 levels x 2 features", who);
+    if (((uintptr_t)g.embeddings & 7u) != 0) return fail(GFPP_ERR_INVALID, "%s: the torso grid table must be 8-byte aligned", who);
+    for (int i = 0; i < 3; ++i) {
+        if (!d->torso_deform_w[i] || !d->torso_canon_w[i]) return fail(GFPP_ERR_INVALID, "%s: null torso weight", who);
+        a.w_def[i] = d->torso_deform_w[i];
+        a.w_can[i] = d->torso_canon_w[i];
+    }
+    if (d->torso_code_dim > 10) return fail(GFPP_ERR_UNSUPPORTED, "%s: torso_code_dim must be <= 10", who);
+    if ((code == nullptr) != (d->torso_code_dim == 0)) return fail(GFPP_ERR_INVALID, "%s: code must be given iff torso_code_dim > 0", who);
+    if (!pose6) return fail(GFPP_ERR_INVALID, "%s: null pose6", who);
+    a.tab = (const float2 *)g.embeddings;
+    a.pose6 = pose6;
+    a.code = code;
+    a.code_dim = (int)d->torso_code_dim;
+    a.shrink = d->torso_shrink;
+    return GFPP_OK;
+}
+
+size_t gfpp_torso_field_workspace_bytes(uint32_t M) {
+    if (M >= (1u << 31)) return 0;
+    return torso_wt_bytes() + (size_t)torso_field_ctas(M) * TorsoPart::total * 4;
+}
+
+int gfpp_torso_field_forward(const gfpp_model_desc *desc, const float *xy, uint32_t M, const float *pose6, const float *code, float *alpha,
+                             float *color, float *deform, void *workspace, size_t workspace_bytes, void *stream) {
+    TorsoTrainArgs a;
+    const int rc = torso_field_setup("torso_field_forward", desc, pose6, code, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xy || !alpha || !color || !deform || !workspace) return fail(GFPP_ERR_INVALID, "torso_field_forward: null pointer%s");
+    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_field_forward: M must be < 2^31%s");
+    if (workspace_bytes < torso_wt_bytes()) return fail(GFPP_ERR_WORKSPACE, "torso_field_forward: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_field_forward: workspace must be 256-byte aligned%s");
+    a.wt = (float *)workspace;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_torso_field_relayout(a, st));
+    // the inference query's kernel on the re-laid-out weights: the same values as gfpp_torso_query at the same parameters
+    TorsoQueryArgs q;
+    memset(&q, 0, sizeof(q));
+    q.tor_gm = a.gm; q.tor_tab = a.tab;
+    q.w_def0 = a.wt + TorsoWt::wd0; q.w_def1 = a.wt + TorsoWt::wd1; q.w_def2 = a.wt + TorsoWt::wd2;
+    q.w_can0 = a.wt + TorsoWt::wc0; q.w_can1 = a.wt + TorsoWt::wc1; q.w_can2 = a.wt + TorsoWt::wc2;
+    q.bias_def = a.wt + TorsoWt::bias_def; q.bias_can = a.wt + TorsoWt::bias_can;
+    q.torso_shrink = a.shrink;
+    q.n = M; q.xy = xy;
+    q.alpha = alpha; q.color = color; q.deform = deform;
+    CK(launch_torso_query(q, st));
+    return GFPP_OK;
+}
+
+int gfpp_torso_field_backward(const gfpp_model_desc *desc, const float *xy, uint32_t M, const float *pose6, const float *code,
+                              const float *grad_alpha, const float *grad_color, const float *grad_deform, float *const grad_deform_w[3],
+                              float *const grad_canon_w[3], float *grad_code, float *grad_torso_table, void *workspace, size_t workspace_bytes,
+                              void *stream) {
+    TorsoTrainArgs a;
+    const int rc = torso_field_setup("torso_field_backward", desc, pose6, code, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xy || !grad_alpha || !grad_color || !grad_deform || !grad_deform_w || !grad_canon_w || !grad_torso_table || !workspace ||
+        (a.code_dim > 0 && !grad_code))
+        return fail(GFPP_ERR_INVALID, "torso_field_backward: null pointer%s");
+    for (int i = 0; i < 3; ++i)
+        if (!grad_deform_w[i] || !grad_canon_w[i]) return fail(GFPP_ERR_INVALID, "torso_field_backward: null weight gradient%s");
+    if (((uintptr_t)grad_torso_table & 7u) != 0) return fail(GFPP_ERR_INVALID, "torso_field_backward: the table gradient must be 8-byte aligned%s");
+    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_field_backward: M must be < 2^31%s");
+    if (workspace_bytes < gfpp_torso_field_workspace_bytes(M)) return fail(GFPP_ERR_WORKSPACE, "torso_field_backward: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_field_backward: workspace must be 256-byte aligned%s");
+    a.M = M; a.xy = xy;
+    a.wt = (float *)workspace;
+    a.part = (float *)((char *)workspace + torso_wt_bytes());
+    a.n_cta = torso_field_ctas(M);
+    a.g_alpha = grad_alpha; a.g_color = grad_color; a.g_deform = grad_deform;
+    a.g_tab = (float2 *)grad_torso_table;
+    for (int i = 0; i < 3; ++i) { a.g_def[i] = grad_deform_w[i]; a.g_can[i] = grad_canon_w[i]; }
+    a.g_code = grad_code;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_torso_field_relayout(a, st));
+    CK(launch_torso_field_bwd(a, st));
+    CK(launch_torso_field_reduce(a, st));
     return GFPP_OK;
 }
 

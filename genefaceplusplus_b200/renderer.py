@@ -14,7 +14,9 @@ as SURVEY.md 8(a) a4 prescribes.
 Training: `RADNeRF` in `.train()` mode runs the reference's training branch of `render` (renderer.py:319-339, 385-398) on libgfpp's
 training ops (train_ops.py) and its differentiable field, `RADNeRF.forward` (gfpp.h section G: fused fp32 forward and backward
 kernels), so `loss.backward()` reaches the MLP weights, both grid tables, the individual code and the conditioning nets.  The SR and
-torso classes are inference only: their `render` raises NotImplementedError in training mode.
+torso classes are inference only: their `render` raises NotImplementedError in training mode.  `RADNeRFTorso.forward_torso` is
+differentiable in training mode (gfpp.h section H), so the torso training step can be assembled from it and the training ops
+(README.md shows the recipe).
 
 `render_clip` is the clip-level entry point (SURVEY.md 8(f) rank 1): a whole clip of poses + conditioning is
 rendered by a handful of persistent-kernel launches with rays generated in-kernel and frames kept on device.
@@ -1257,12 +1259,26 @@ class RADNeRFTorso(_TorsoGrid, RADNeRF):
         d.density_thresh_torso = float(min(self.density_thresh_torso, self.mean_density_torso))
         d.torso_shrink = float(self.torso_shrink)
 
-    @torch.no_grad()
     def forward_torso(self, x, poses, c=None):
-        """radnerf_torso.py:51-84 in libgfpp (k_torso_query, fp32): x [n,2] in [-1,1], poses [1,6] (convert_poses of the head
-        pose), c [1,torso_code_dim] (a row of torso_individual_codes) or None without codes -> (alpha [n,1], color [n,3],
-        dx [n,2]).  Inference only: no autograd."""
+        """radnerf_torso.py:51-84 in libgfpp (fp32): x [n,2] in [-1,1], poses [1,6] (convert_poses of the head pose), c
+        [1,torso_code_dim] (a row of torso_individual_codes) or None without codes -> (alpha [n,1], color [n,3], dx [n,2]).
+        In training mode it is differentiable w.r.t. the six torso MLP weights, the torso grid table and c (gfpp.h section H: fused
+        fp32 forward and backward reading the parameters in place; with c = torso_individual_codes[index] only that row gets a
+        gradient), and returns fp32 also under torch.autocast; its values are bit-identical to the eval-mode query's.  In eval mode
+        it is the packed model's query (k_torso_query), without autograd."""
         dev = self._require_cuda()
+        if self.training:
+            if (torch.is_tensor(x) and x.requires_grad) or (torch.is_tensor(poses) and poses.requires_grad):
+                raise NotImplementedError("gradients w.r.t. the torso positions or the head pose are not implemented")
+            from . import train_ops
+            params = ([self.torso_deform_net.net[i].weight for i in range(3)] + [self.torso_canonicial_net.net[i].weight for i in range(3)] +
+                      [self.torso_embedder.embeddings])
+            with torch.autocast("cuda", enabled=False):
+                return train_ops.torso_field(self, x.to(dev), poses.to(dev), None if c is None else c.to(dev), *params)
+        with torch.no_grad():
+            return self._forward_torso_eval(x, poses, c, dev)
+
+    def _forward_torso_eval(self, x, poses, c, dev):
         _, _, model, _ = self._ensure_packed()
         f32 = torch.float32
         xy = x.to(dev, f32).reshape(-1, 2).contiguous()

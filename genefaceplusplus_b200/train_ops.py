@@ -8,6 +8,8 @@ meaning and autograd behaviour -- over csrc/train_kernels.cu through the C-ABI (
     weights_sum, ambient_sum, depth, image = raymarching.composite_rays_train(sigmas, rgbs, ambient, deltas, rays, T_thresh)
 
 `field` is RADNeRF.forward with its gradient (include/gfpp.h section G, csrc/field_train_kernel.cu); RADNeRF.forward calls it.
+`torso_field` is RADNeRFTorso.forward_torso with its gradient (section H, csrc/torso_train_kernel.cu); forward_torso calls it in
+training mode.
 
 fp32 only (the reference casts with custom_fwd(cast_inputs=float32) as well); CUDA tensors only -- there is no CPU path.
 Differences from the reference, both deliberate: march_rays_train lays the samples out in ray order (deterministic; the
@@ -330,3 +332,100 @@ class _field(Function):
 
 
 field = _field.apply
+
+
+# ------------------------------------------------------------------------------------------------ the torso field
+def _torso_field_workspace(model, M):
+    need = _capi.lib().gfpp_torso_field_workspace_bytes(M)
+    if need == 0:
+        raise _capi.GfppError(f"the torso training field does not support {M} points per call")
+    dev = model.density_bitfield.device
+    ws = model.__dict__.get("_torso_field_ws")
+    if ws is None or ws.numel() < need or ws.device != dev:
+        ws = model.__dict__["_torso_field_ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+    return ws
+
+
+def _torso_field_desc(model, keep):
+    """The gfpp_model_desc fields section (H) reads -- torso grid, the six torso weights, torso_code_dim, torso_shrink -- with no
+    device-to-host copy."""
+    d = _capi.ModelDesc()
+    gp = model.torso_embedder
+    lay = gp.layout
+    emb = _cuda_f32(gp.embeddings.detach())
+    off = _host_offsets(gp)
+    keep += [emb, off]
+    g = d.torso_grid
+    g.embeddings, g.offsets_host = emb.data_ptr(), off.ctypes.data
+    g.input_dim, g.num_levels, g.base_resolution = lay.input_dim, lay.num_levels, lay.base_resolution
+    g.log2_per_level_scale, g.gridtype, g.interp, g.align_corners = float(lay.S), lay.gridtype_id, lay.interp_id, int(lay.align_corners)
+    ws = [_cuda_f32(w.weight.detach()) for w in list(model.torso_deform_net.net) + list(model.torso_canonicial_net.net)]
+    keep += ws
+    for i in range(3):
+        d.torso_deform_w[i], d.torso_canon_w[i] = ws[i].data_ptr(), ws[3 + i].data_ptr()
+    d.torso_code_dim = model.torso_individual_embedding_dim
+    d.torso_shrink = float(model.torso_shrink)
+    return d
+
+
+class _torso_field(Function):
+    """RADNeRFTorso.forward_torso (radnerf_torso.py:51-84) over gfpp_torso_field_forward / gfpp_torso_field_backward: (x [M,2] in
+    [-1,1], pose6 [6] or [1,6], code [torso_code_dim] or [1,torso_code_dim] or None) -> (alpha [M,1], color [M,3], dx [M,2]).  `params`
+    are the six torso MLP weights and the torso grid table of `model`, passed so that autograd routes their gradients; the kernels
+    read them in place.  `code` may be a view such as torso_individual_codes[index]: autograd then routes its gradient to that row
+    only.  No gradient reaches x or the pose (the caller rejects inputs that require one)."""
+
+    @staticmethod
+    def forward(ctx, model, x, pose6, code, *params):
+        xy = _cuda_f32(x).view(-1, 2)
+        p6 = _cuda_f32(pose6).reshape(-1)
+        if p6.numel() != 6:
+            raise ValueError(f"forward_torso takes one pose [1,6] (convert_poses), got shape {tuple(pose6.shape)}")
+        cdim = model.torso_individual_embedding_dim
+        if (code is None) != (cdim == 0) or (code is not None and code.numel() != cdim):
+            raise ValueError(f"c must hold {cdim} values (None iff the model has no torso_individual_codes)")
+        cd = _cuda_f32(code).reshape(-1) if code is not None else None
+        M, dev = xy.shape[0], xy.device
+        alpha = torch.empty(M, 1, dtype=torch.float32, device=dev)
+        color = torch.empty(M, 3, dtype=torch.float32, device=dev)
+        dx = torch.empty(M, 2, dtype=torch.float32, device=dev)
+        keep = []
+        d = _torso_field_desc(model, keep)
+        ws = _torso_field_workspace(model, 0)
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_torso_field_forward(ctypes.byref(d), xy.data_ptr(), M, p6.data_ptr(), None if cd is None else cd.data_ptr(),
+                                                             alpha.data_ptr(), color.data_ptr(), dx.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                             _capi.stream_ptr(dev)), "gfpp_torso_field_forward")
+        ctx.model = model
+        ctx.code_shape = None if code is None else code.shape
+        ctx.save_for_backward(xy, p6, cd if cd is not None else torch.empty(0, device=dev), *params)
+        return alpha, color, dx
+
+    @staticmethod
+    def backward(ctx, g_alpha, g_color, g_dx):
+        xy, p6, cd, *params = ctx.saved_tensors
+        model, code_shape = ctx.model, ctx.code_shape
+        M, dev = xy.shape[0], xy.device
+        g_alpha = torch.zeros(M, device=dev) if g_alpha is None else _cuda_f32(g_alpha).reshape(-1)
+        g_color = torch.zeros(M, 3, device=dev) if g_color is None else _cuda_f32(g_color)
+        g_dx = torch.zeros(M, 2, device=dev) if g_dx is None else _cuda_f32(g_dx)
+        alloc = torch.zeros if M == 0 else torch.empty
+        grad_w = [alloc(p.shape, dtype=torch.float32, device=dev) for p in params[:6]]
+        g_tab = torch.zeros(params[6].shape, dtype=torch.float32, device=dev)
+        g_code = alloc(cd.shape, dtype=torch.float32, device=dev) if code_shape is not None else None
+        keep = []
+        d = _torso_field_desc(model, keep)
+        ws = _torso_field_workspace(model, M)
+        p_def = (ctypes.c_void_p * 3)(*[g.data_ptr() for g in grad_w[:3]])
+        p_can = (ctypes.c_void_p * 3)(*[g.data_ptr() for g in grad_w[3:]])
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_torso_field_backward(ctypes.byref(d), xy.data_ptr(), M, p6.data_ptr(),
+                                                              None if code_shape is None else cd.data_ptr(), g_alpha.data_ptr(),
+                                                              g_color.data_ptr(), g_dx.data_ptr(), ctypes.byref(p_def), ctypes.byref(p_can),
+                                                              None if g_code is None else g_code.data_ptr(), g_tab.data_ptr(), ws.data_ptr(),
+                                                              ws.numel(), _capi.stream_ptr(dev)), "gfpp_torso_field_backward")
+        grads = [g.to(p.dtype) for g, p in zip(grad_w + [g_tab], params)]
+        return (None, None, None, None if g_code is None else g_code.view(code_shape), *grads)
+
+
+torso_field = _torso_field.apply

@@ -35,6 +35,8 @@
  *  (F) the torso models' occupancy grid: torso field query and density_grid_torso refresh, threshold setters.
  *
  *  (G) the trainable head field: RADNeRF.forward and its backward at explicit points, fp32.
+ *
+ *  (H) the trainable torso field: RADNeRFTorso.forward_torso and its backward at explicit points, fp32.
  */
 #ifndef GFPP_H_
 #define GFPP_H_
@@ -471,6 +473,38 @@ GFPP_API int gfpp_field_backward(const gfpp_model_desc *desc, const float *xyzs,
                                  const float *grad_sigma, const float *grad_color, const float *grad_ambient_pos, float *const grad_w[8],
                                  float *grad_cond, float *grad_code, float *grad_position_table, float *grad_ambient_table, void *workspace,
                                  size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------ (H) trainable torso field
+ *
+ * RADNeRFTorso.forward_torso (modules/radnerfs/radnerf_torso.py:51-84) and its gradient for the torso training step, in fp32 FFMA
+ * arithmetic, reading the parameters IN PLACE through a gfpp_model_desc -- no gfpp_model_pack.  Read from the desc: torso_grid
+ * (2-D, 16 levels x 2, reference layout [entries,2] fp32, 8-byte aligned), torso_deform_w (64,din) (64,64) (2,64), torso_canon_w
+ * (32,32+din) (32,32) (4,32) with din = 42 + 54 + torso_code_dim, torso_code_dim (<= 10) and torso_shrink.  The other desc fields
+ * are not read (has_torso and torso_code neither: `code` is an explicit argument, the training row torso_individual_codes[index];
+ * it is NULL iff torso_code_dim == 0).  pose6 [6] is the head pose (convert_poses).  Every argument is validated before any CUDA
+ * call; M == 0 then returns GFPP_OK without touching the device (the point and output pointers may be NULL).  Everything is enqueued
+ * on `stream` with no host synchronisation and no allocation.
+ *
+ * Workspace (256-byte aligned): gfpp_torso_field_workspace_bytes(M) for the backward (0 = unsupported M); the forward needs
+ * gfpp_torso_field_workspace_bytes(0) bytes (the per-call k-major copy of the weights and the two folded bias vectors, ~42 KB).
+ *
+ * gfpp_torso_field_forward: for points xy [M,2] in [-1,1]: alpha [M], color [M,3] (sigmoid), deform [M,2] (dx, before the clamp).
+ *   Bit-identical to gfpp_torso_query of a model packed from the same parameters, with the same pose6 and code.
+ * gfpp_torso_field_backward: given grad_alpha [M], grad_color [M,3] and grad_deform [M,2] (w.r.t. dx), recomputes the forward and
+ *   writes grad_deform_w[0..2], grad_canon_w[0..2] (same [out, in] layouts; overwritten) and grad_code [torso_code_dim] (the code
+ *   is repeated over the points: its gradient is the sum; NULL iff torso_code_dim == 0); grad_torso_table [entries,2] is
+ *   ACCUMULATED into (+=), as the reference's grid backward does.  The grid's input gradient goes through its dy_dx, the (x+1)/2
+ *   map of bound 1 and the clamp (which passes the gradient on [-1, 1] inclusive); the pose gets no gradient, xy neither.
+ * Determinism: the forward outputs, grad_deform_w, grad_canon_w and grad_code are bit-identical from run to run (per-CTA partial
+ * sums in the workspace, reduced in a fixed order by one kernel; the partitioning depends only on M).  The table gradient is
+ * scattered with float2 vector reductions, so its summation order is free. */
+GFPP_API size_t gfpp_torso_field_workspace_bytes(uint32_t M);
+GFPP_API int gfpp_torso_field_forward(const gfpp_model_desc *desc, const float *xy, uint32_t M, const float *pose6, const float *code,
+                                      float *alpha, float *color, float *deform, void *workspace, size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_torso_field_backward(const gfpp_model_desc *desc, const float *xy, uint32_t M, const float *pose6, const float *code,
+                                       const float *grad_alpha, const float *grad_color, const float *grad_deform,
+                                       float *const grad_deform_w[3], float *const grad_canon_w[3], float *grad_code,
+                                       float *grad_torso_table, void *workspace, size_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }
