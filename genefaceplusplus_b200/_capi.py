@@ -103,6 +103,7 @@ EXPORTS = [
     "gfpp_model_set_torso_threshold", "gfpp_torso_sr_set_threshold",
     "gfpp_field_backward_workspace_bytes", "gfpp_field_forward", "gfpp_field_backward",
     "gfpp_torso_field_workspace_bytes", "gfpp_torso_field_forward", "gfpp_torso_field_backward",
+    "gfpp_torso_sr_field_workspace_bytes", "gfpp_torso_sr_field_forward", "gfpp_torso_sr_field_backward",
 ]
 
 
@@ -187,6 +188,11 @@ def lib():
         L.gfpp_torso_field_forward.argtypes = [ctypes.POINTER(ModelDesc), P, c_u32, P, P, P, P, P, P, c_size_t, P]
         L.gfpp_torso_field_backward.argtypes = [ctypes.POINTER(ModelDesc), P, c_u32, P, P, P, P, P, ctypes.POINTER(P * 3),
                                                 ctypes.POINTER(P * 3), P, P, P, c_size_t, P]
+        L.gfpp_torso_sr_field_workspace_bytes.restype = c_size_t
+        L.gfpp_torso_sr_field_workspace_bytes.argtypes = [c_u32]
+        L.gfpp_torso_sr_field_forward.argtypes = [ctypes.POINTER(TorsoSrDesc), P, c_u32, P, P, P, P, P, P, P, P, c_size_t, P]
+        L.gfpp_torso_sr_field_backward.argtypes = [ctypes.POINTER(TorsoSrDesc), P, c_u32, P, P, P, P, P, P, P, ctypes.POINTER(P * 3),
+                                                   ctypes.POINTER(P * 3), ctypes.POINTER(P * 3), ctypes.POINTER(P * 3), P, P, P, c_size_t, P]
         _lib = L
     return _lib
 

@@ -15,6 +15,7 @@
 #include "torso_grid_kernel.cuh"
 #include "torso_kernel.cuh"
 #include "torso_sr_kernel.cuh"
+#include "torso_sr_train_kernel.cuh"
 #include "torso_train_kernel.cuh"
 
 namespace gfpp {
@@ -1643,6 +1644,134 @@ int gfpp_torso_field_backward(const gfpp_model_desc *desc, const float *xy, uint
     CK(launch_torso_field_relayout(a, st));
     CK(launch_torso_field_bwd(a, st));
     CK(launch_torso_field_reduce(a, st));
+    return GFPP_OK;
+}
+
+// ---------------------------------------------------------------- (I) trainable torso-SR field
+static uint32_t torso_sr_field_ctas(uint32_t M) {
+    const uint32_t tiles = (M + TORSO_SR_TRAIN_TP - 1) / TORSO_SR_TRAIN_TP;
+    return tiles < (uint32_t)TORSO_SR_TRAIN_CTAS ? tiles : (uint32_t)TORSO_SR_TRAIN_CTAS;
+}
+static size_t torso_sr_wt_bytes() { return (TorsoSrWt::total * 4 + 255) / 256 * 256; }
+
+// Validates the desc's torso fields, lm68, code and the head-aware inputs (everything the kernels read besides the points) and fills
+// the model half of TorsoSrTrainArgs; no CUDA call.
+static int torso_sr_field_setup(const char *who, const gfpp_torso_sr_desc *d, const float *lm68, const float *code, const float *image,
+                                const float *weights_sum, TorsoSrTrainArgs &a) {
+    if (!d) return fail(GFPP_ERR_INVALID, "%s: null desc", who);
+    memset(&a, 0, sizeof(a));
+    const gfpp_grid_desc &g = d->torso_grid;
+    if (!g.embeddings || !g.offsets_host) return fail(GFPP_ERR_INVALID, "%s: null torso grid table or offsets", who);
+    if (g.num_levels != 16 ||
+        fill_grid_meta(a.gm, g.offsets_host, g.input_dim, g.num_levels, g.log2_per_level_scale, g.base_resolution, g.gridtype,
+                       g.align_corners, g.interp) != 0 || a.gm.dim != 2)
+        return fail(GFPP_ERR_UNSUPPORTED, "%s: the torso grid must be 2-D with 16 levels x 2 features", who);
+    if (((uintptr_t)g.embeddings & 7u) != 0) return fail(GFPP_ERR_INVALID, "%s: the torso grid table must be 8-byte aligned", who);
+    for (int i = 0; i < 3; ++i) {
+        if (!d->torso_deform_w[i] || !d->torso_canon_w[i]) return fail(GFPP_ERR_INVALID, "%s: null torso weight", who);
+        a.w_def[i] = d->torso_deform_w[i];
+        a.w_can[i] = d->torso_canon_w[i];
+    }
+    if (d->torso_code_dim > 10) return fail(GFPP_ERR_UNSUPPORTED, "%s: torso_code_dim must be <= 10", who);
+    if ((code == nullptr) != (d->torso_code_dim == 0)) return fail(GFPP_ERR_INVALID, "%s: code must be given iff torso_code_dim > 0", who);
+    if (!lm68) return fail(GFPP_ERR_INVALID, "%s: null lm68", who);
+    if ((image == nullptr) != (weights_sum == nullptr)) return fail(GFPP_ERR_INVALID, "%s: image and weights_sum must both be given or both be NULL", who);
+    if (d->head_aware) {
+        for (int i = 0; i < 3; ++i) {
+            if (!d->ha_w[i] || !d->ha_b[i]) return fail(GFPP_ERR_INVALID, "%s: null head-aware encoder weight", who);
+            a.ha_w[i] = d->ha_w[i];
+            a.ha_b[i] = d->ha_b[i];
+        }
+    } else if (image) {
+        return fail(GFPP_ERR_INVALID, "%s: image and weights_sum are only read with head_aware", who);
+    }
+    a.head_aware = d->head_aware ? 1 : 0;
+    a.tab = (const float2 *)g.embeddings;
+    a.lm68 = lm68;
+    a.code = code;
+    a.code_dim = (int)d->torso_code_dim;
+    a.shrink = d->torso_shrink;
+    a.image = image;
+    a.wsum = weights_sum;
+    return GFPP_OK;
+}
+
+size_t gfpp_torso_sr_field_workspace_bytes(uint32_t M) {
+    if (M >= (1u << 31)) return 0;
+    return torso_sr_wt_bytes() + (size_t)torso_sr_field_ctas(M) * TorsoSrPart::total * 4;
+}
+
+int gfpp_torso_sr_field_forward(const gfpp_torso_sr_desc *desc, const float *xy, uint32_t M, const float *lm68, const float *code,
+                                const float *image, const float *weights_sum, float *alpha, float *color, float *deform, void *workspace,
+                                size_t workspace_bytes, void *stream) {
+    TorsoSrTrainArgs a;
+    const int rc = torso_sr_field_setup("torso_sr_field_forward", desc, lm68, code, image, weights_sum, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xy || !alpha || !color || !deform || !workspace) return fail(GFPP_ERR_INVALID, "torso_sr_field_forward: null pointer%s");
+    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_field_forward: M must be < 2^31%s");
+    if (workspace_bytes < torso_sr_wt_bytes()) return fail(GFPP_ERR_WORKSPACE, "torso_sr_field_forward: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_sr_field_forward: workspace must be 256-byte aligned%s");
+    a.wt = (float *)workspace;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_torso_sr_field_relayout(a, st));
+    // k_torso_sr's field in its point mode on the re-laid-out weights: the same values as the render epilogue at the same parameters
+    TorsoSrArgs t;
+    memset(&t, 0, sizeof(t));
+    t.tor_gm = a.gm; t.tor_tab = a.tab;
+    t.w_def0 = a.wt + TorsoSrWt::wd0; t.w_def1 = a.wt + TorsoSrWt::wd1; t.w_def2 = a.wt + TorsoSrWt::wd2;
+    t.w_can0 = a.wt + TorsoSrWt::wc0; t.w_can1 = a.wt + TorsoSrWt::wc1; t.w_can2 = a.wt + TorsoSrWt::wc2;
+    t.ha = a.head_aware ? a.wt + TorsoSrWt::ha : nullptr;
+    t.bias_def = a.wt + TorsoSrWt::bias_def; t.bias_can = a.wt + TorsoSrWt::bias_can;
+    t.torso_shrink = a.shrink;
+    t.bg_coords = xy;
+    t.n_frames = 1; t.n_rays = (int)M;
+    t.image = image; t.wsum = weights_sum;
+    t.torso_alpha = alpha; t.torso_rgb = color; t.deform = deform;
+    CK(launch_torso_sr_points(t, st));
+    return GFPP_OK;
+}
+
+int gfpp_torso_sr_field_backward(const gfpp_torso_sr_desc *desc, const float *xy, uint32_t M, const float *lm68, const float *code,
+                                 const float *image, const float *weights_sum, const float *grad_alpha, const float *grad_color,
+                                 const float *grad_deform, float *const grad_deform_w[3], float *const grad_canon_w[3],
+                                 float *const grad_ha_w[3], float *const grad_ha_b[3], float *grad_code, float *grad_torso_table,
+                                 void *workspace, size_t workspace_bytes, void *stream) {
+    TorsoSrTrainArgs a;
+    const int rc = torso_sr_field_setup("torso_sr_field_backward", desc, lm68, code, image, weights_sum, a);
+    if (rc != GFPP_OK) return rc;
+    if ((grad_ha_w == nullptr) != (a.head_aware == 0) || (grad_ha_b == nullptr) != (a.head_aware == 0))
+        return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: grad_ha_w / grad_ha_b must be given iff head_aware%s");
+    if (a.head_aware)
+        for (int i = 0; i < 3; ++i)
+            if (!grad_ha_w[i] || !grad_ha_b[i]) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: null head-aware gradient%s");
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xy || !grad_alpha || !grad_color || !grad_deform || !grad_deform_w || !grad_canon_w || !grad_torso_table || !workspace ||
+        (a.code_dim > 0 && !grad_code))
+        return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: null pointer%s");
+    for (int i = 0; i < 3; ++i)
+        if (!grad_deform_w[i] || !grad_canon_w[i]) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: null weight gradient%s");
+    if (((uintptr_t)grad_torso_table & 7u) != 0) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: the table gradient must be 8-byte aligned%s");
+    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_field_backward: M must be < 2^31%s");
+    if (workspace_bytes < gfpp_torso_sr_field_workspace_bytes(M)) return fail(GFPP_ERR_WORKSPACE, "torso_sr_field_backward: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: workspace must be 256-byte aligned%s");
+    a.M = M; a.xy = xy;
+    a.wt = (float *)workspace;
+    a.part = (float *)((char *)workspace + torso_sr_wt_bytes());
+    a.n_cta = torso_sr_field_ctas(M);
+    a.g_alpha = grad_alpha; a.g_color = grad_color; a.g_deform = grad_deform;
+    a.g_tab = (float2 *)grad_torso_table;
+    for (int i = 0; i < 3; ++i) {
+        a.g_def[i] = grad_deform_w[i]; a.g_can[i] = grad_canon_w[i];
+        if (a.head_aware) { a.g_ha_w[i] = grad_ha_w[i]; a.g_ha_b[i] = grad_ha_b[i]; }
+    }
+    a.g_code = grad_code;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_torso_sr_field_relayout(a, st));
+    CK(launch_torso_sr_field_bwd(a, st));
+    CK(launch_torso_sr_field_reduce(a, st));
     return GFPP_OK;
 }
 

@@ -11,35 +11,13 @@
 // skip the MLPs; fp32 FFMA tile GEMMs out of shared memory; accurate sinf; grid_sample restated.
 #include "launch.cuh"
 #include "torso_common.cuh"
+#include "torso_sr_field.cuh"
 #include "torso_sr_kernel.cuh"
 
 namespace gfpp {
 
 using namespace torsoc;
-
-namespace {
-
-constexpr int TP = 128;    // pixels per tile
-constexpr int NT = 256;
-constexpr int KD0 = TORSO_SR_KD0, KC0 = TORSO_SR_KC0;
-constexpr int LDT = 100;   // A-tile stride (>= 92, 16-byte aligned rows)
-constexpr int LDE = 60;    // copy of the deform input (enc_x + head-aware encoding) for the canonical net
-constexpr int NJAW = 14, NLM = NJAW + NJAW * 2 * 4;   // 126
-
-struct Smem {
-    float A[TP * LDT];
-    float E[TP * LDE];
-    float wd0[KD0 * 64], wd1[64 * 64], wc0[KC0 * 32], wc1[32 * 32];
-    float wd2[2 * 64], wc2[4 * 32];
-    float ha[TORSO_SR_HA_FLOATS];
-    float x2[2 * TP];
-    float alpha[TP], col[3 * TP], dxy[2 * TP];
-    int mask[TP];
-};
-
-__device__ __forceinline__ float leaky002(float x) { return x > 0.f ? x : 0.02f * x; }
-
-}  // namespace
+using namespace tsr;
 
 // per-frame bias vectors: columns [code | freq4(jaw landmarks)] of the first deform / canonical layers
 __global__ void k_torso_sr_frame_bias(const float *__restrict__ lm68 /*[F,136]*/, const float *__restrict__ w_def0 /*[64,din]*/,
@@ -65,187 +43,8 @@ __global__ void k_torso_sr_frame_bias(const float *__restrict__ lm68 /*[F,136]*/
 }
 
 __global__ void __launch_bounds__(256, 1) k_torso_sr(const __grid_constant__ TorsoSrArgs a) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    Smem &s = *reinterpret_cast<Smem *>(smem_raw);
-    const int tid = threadIdx.x;
-    const int tiles_per_frame = (a.n_rays + TP - 1) / TP;
-    const int n_tiles = a.n_frames * tiles_per_frame;
-    for (int i = tid; i < KD0 * 64; i += NT) s.wd0[i] = a.w_def0[i];
-    for (int i = tid; i < 64 * 64; i += NT) s.wd1[i] = a.w_def1[i];
-    for (int i = tid; i < KC0 * 32; i += NT) s.wc0[i] = a.w_can0[i];
-    for (int i = tid; i < 32 * 32; i += NT) s.wc1[i] = a.w_can1[i];
-    for (int i = tid; i < 2 * 64; i += NT) s.wd2[i] = a.w_def2[i];
-    for (int i = tid; i < 4 * 32; i += NT) s.wc2[i] = a.w_can2[i];
-    for (int i = tid; i < TORSO_SR_HA_FLOATS; i += NT) s.ha[i] = a.ha ? a.ha[i] : 0.f;
-    __syncthreads();
-    const int ty = tid >> 4, tx = tid & 15;
-    const int slot = tid & (TP - 1), lg = tid >> 7;
-
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int f = tile / tiles_per_frame;
-        const int n0 = (tile - f * tiles_per_frame) * TP;
-        const int n = n0 + slot;
-        const bool in_range = n < a.n_rays;
-        const size_t g = (size_t)f * a.n_rays + (in_range ? n : 0);
-        int m = 0;
-        if (tid < TP && in_range) {
-            const float occ = sample_density(a.density_grid_torso, a.grid_size, a.bg_coords[2 * n], a.bg_coords[2 * n + 1]);
-            m = occ > a.density_thresh_torso ? 1 : 0;
-        }
-        if (tid < TP) s.mask[tid] = m;
-        const int any = __syncthreads_or(m);
-        if (any) {
-            // ---- deform input: enc_x = freq10(shrink * bg_coord) -> cols 0..41, head-aware encoding -> cols 42..57, pad 58,59 ----
-            {
-                float x[2] = {0.f, 0.f};
-                if (in_range) { x[0] = __fmul_rn(a.bg_coords[2 * n], a.torso_shrink); x[1] = __fmul_rn(a.bg_coords[2 * n + 1], a.torso_shrink); }
-                for (int c = lg * 30; c < lg * 30 + 30; ++c) {
-                    if (c >= 42 && c < 58) continue;
-                    const float v = c < 42 ? freq_entry(x, 2, c) : 0.f;
-                    s.E[slot * LDE + c] = v;
-                    s.A[slot * LDT + c] = v;
-                }
-                if (lg == 0) {
-                    s.x2[slot] = x[0]; s.x2[TP + slot] = x[1];
-                    // head_color_weights_encoder(cat[image, weights_sum]) (radnerf_torso_sr.py:45-52, 98-100)
-                    float o[16];
-                    if (a.ha) {
-                        float in4[4] = {0.f, 0.f, 0.f, 0.f};
-                        if (in_range) { in4[0] = a.image[3 * g]; in4[1] = a.image[3 * g + 1]; in4[2] = a.image[3 * g + 2]; in4[3] = a.wsum[g]; }
-                        float h1[16], h2[32];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            float t = s.ha[TORSO_SR_HA_B0 + j];
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) t = fmaf(in4[k], s.ha[TORSO_SR_HA_W0 + k * 16 + j], t);
-                            h1[j] = leaky002(t);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) h2[j] = s.ha[TORSO_SR_HA_B1 + j];
-#pragma unroll
-                        for (int k = 0; k < 16; ++k) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) h2[j] = fmaf(h1[k], s.ha[TORSO_SR_HA_W1 + k * 32 + j], h2[j]);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) o[j] = s.ha[TORSO_SR_HA_B2 + j];
-#pragma unroll
-                        for (int k = 0; k < 32; ++k) {
-                            const float hk = leaky002(h2[k]);
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) o[j] = fmaf(hk, s.ha[TORSO_SR_HA_W2 + k * 16 + j], o[j]);
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) o[j] = 0.f;
-                    }
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        s.E[slot * LDE + 42 + j] = o[j];
-                        s.A[slot * LDT + 42 + j] = o[j];
-                    }
-                }
-            }
-            __syncthreads();
-            // ---- deform net din -> 64 -> 64 -> 2 ----
-            {
-                float acc[8][4] = {};
-                small_gemm<4, KD0, LDT>(acc, s.A, s.wd0, ty, tx);
-                __syncthreads();
-                store_relu<4, LDT>(acc, s.A, a.bias_def + (size_t)f * 64, ty, tx);
-                __syncthreads();
-            }
-            {
-                float acc[8][4] = {};
-                small_gemm<4, 64, LDT>(acc, s.A, s.wd1, ty, tx);
-                __syncthreads();
-                store_relu<4, LDT>(acc, s.A, nullptr, ty, tx);
-                __syncthreads();
-            }
-            {
-                const int row = tid >> 1, half = tid & 1;
-                float v0 = 0.f, v1 = 0.f;
-                for (int k = half * 32; k < half * 32 + 32; ++k) {
-                    const float xk = s.A[row * LDT + k];
-                    v0 = fmaf(xk, s.wd2[k], v0);
-                    v1 = fmaf(xk, s.wd2[64 + k], v1);
-                }
-                v0 += __shfl_xor_sync(0xffffffffu, v0, 1);
-                v1 += __shfl_xor_sync(0xffffffffu, v1, 1);
-                if (half == 0) {
-                    s.dxy[row] = v0; s.dxy[TP + row] = v1;
-                    s.x2[row] = fminf(fmaxf(s.x2[row] + v0, -1.f), 1.f);           // x = (x + dx).clamp(-1, 1)
-                    s.x2[TP + row] = fminf(fmaxf(s.x2[TP + row] + v1, -1.f), 1.f);
-                }
-            }
-            __syncthreads();
-            // ---- canonical input: [tiled2D(x) 32 | enc_x 42 | head-aware 16 | pad 2] ----
-            {
-                const float u = __fdiv_rn(__fadd_rn(s.x2[slot], 1.0f), 2.0f), v = __fdiv_rn(__fadd_rn(s.x2[TP + slot], 1.0f), 2.0f);
-#pragma unroll 2
-                for (int l = lg * 8; l < lg * 8 + 8; ++l)
-                    *reinterpret_cast<float2 *>(s.A + slot * LDT + 2 * l) = grid_lookup2(a.tor_gm, a.tor_tab, l, u, v);
-                for (int c = lg * 30; c < lg * 30 + 30; ++c) s.A[slot * LDT + 32 + c] = s.E[slot * LDE + c];
-            }
-            __syncthreads();
-            // ---- canonical net -> 32 -> 32 -> 4, sigmoid ----
-            {
-                float acc[8][2] = {};
-                small_gemm<2, KC0, LDT>(acc, s.A, s.wc0, ty, tx);
-                __syncthreads();
-                store_relu<2, LDT>(acc, s.A, a.bias_can + (size_t)f * 32, ty, tx);
-                __syncthreads();
-            }
-            {
-                float acc[8][2] = {};
-                small_gemm<2, 32, LDT>(acc, s.A, s.wc1, ty, tx);
-                __syncthreads();
-                store_relu<2, LDT>(acc, s.A, nullptr, ty, tx);
-                __syncthreads();
-            }
-            {
-                const int row = tid >> 1, half = tid & 1;
-                float v[4] = {0.f, 0.f, 0.f, 0.f};
-                for (int k = half * 16; k < half * 16 + 16; ++k) {
-                    const float xk = s.A[row * LDT + k];
-#pragma unroll
-                    for (int o = 0; o < 4; ++o) v[o] = fmaf(xk, s.wc2[o * 32 + k], v[o]);
-                }
-#pragma unroll
-                for (int o = 0; o < 4; ++o) v[o] += __shfl_xor_sync(0xffffffffu, v[o], 1);
-                if (half == 0) {
-                    s.alpha[row] = 1.0f / (1.0f + expf(-v[0]));
-                    s.col[row] = 1.0f / (1.0f + expf(-v[1]));
-                    s.col[TP + row] = 1.0f / (1.0f + expf(-v[2]));
-                    s.col[2 * TP + row] = 1.0f / (1.0f + expf(-v[3]));
-                }
-            }
-            __syncthreads();
-        }
-        // ---- composite (radnerf_torso_sr.py:214-221) ----
-        if (tid < TP && in_range) {
-            float ta = 0.f, tc[3] = {0.f, 0.f, 0.f}, dx = 0.f, dy = 0.f;
-            if (any && s.mask[tid]) {
-                ta = s.alpha[tid];
-                tc[0] = s.col[tid]; tc[1] = s.col[TP + tid]; tc[2] = s.col[2 * TP + tid];
-                dx = s.dxy[tid]; dy = s.dxy[TP + tid];
-            }
-            const float ws = a.wsum[g];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float bgc = a.bg_color ? a.bg_color[3 * (size_t)n + c] : 1.0f;
-                // torso_bg = torso_color * alpha + bg * (1 - alpha); image = image + (1 - ws) * torso_bg; clamp(0, 1)
-                const float bg = __fadd_rn(__fmul_rn(tc[c], ta), __fmul_rn(bgc, __fsub_rn(1.0f, ta)));
-                const float v = __fadd_rn(a.image[3 * g + c], __fmul_rn(__fsub_rn(1.0f, ws), bg));
-                a.rgb_map[3 * g + c] = fminf(fmaxf(v, 0.f), 1.f);
-                if (a.torso_rgb) a.torso_rgb[3 * g + c] = bg;
-            }
-            if (a.torso_alpha) a.torso_alpha[g] = ta;
-            if (a.deform) { a.deform[2 * g] = dx; a.deform[2 * g + 1] = dy; }
-            if (a.P_count && any && s.mask[tid]) atomicAdd(a.P_count + f, 1);
-        }
-        __syncthreads();
-    }
+    constexpr bool POINTS = false;
+#include "torso_sr_body.inc"
 }
 
 cudaError_t launch_torso_sr_frame_bias(const float *lm68, int n_frames, const float *w_def0, const float *w_can0, const float *code,

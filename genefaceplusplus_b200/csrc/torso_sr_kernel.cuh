@@ -40,5 +40,8 @@ constexpr int TORSO_SR_KD0 = 60, TORSO_SR_KC0 = 92;
 cudaError_t launch_torso_sr_frame_bias(const float *lm68, int n_frames, const float *w_def0, const float *w_can0, const float *code,
                                        int code_dim, int head_aware, float *bias_def, float *bias_can, cudaStream_t st);
 cudaError_t launch_torso_sr(const TorsoSrArgs &a, cudaStream_t st);
+// k_torso_sr's field at explicit points (n_frames 1, bg_coords = the points, no mask, image / wsum per point or both nullptr):
+// writes torso_alpha [n], torso_rgb [n,3] (the field's colour) and deform [n,2]; no composite.
+cudaError_t launch_torso_sr_points(const TorsoSrArgs &a, cudaStream_t st);
 
 }  // namespace gfpp

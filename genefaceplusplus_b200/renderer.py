@@ -986,7 +986,23 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
         return x
 
     def forward_torso(self, x, poses, c=None, image=None, weights_sum=None, lm68=None):
-        """radnerf_torso_sr.py:73-113 (`poses` is accepted and unused there too)."""
+        """radnerf_torso_sr.py:73-113 (`poses` is accepted and unused there too): x [n,2] in [-1,1], c [1,torso_code_dim] (a row of
+        torso_individual_codes) or None without codes, image [n,3] / weights_sum [n,1] the head colour and alpha at the points (None:
+        zeros; read only with torso_head_aware), lm68 (136 values) -> (alpha [n,1], color [n,3], dx [n,2]).
+        In training mode it runs libgfpp's fused fp32 field (gfpp.h section I) and is differentiable w.r.t. the six torso MLP weights,
+        the torso grid table, head_color_weights_encoder and c (with c = torso_individual_codes[index] only that row gets a gradient);
+        it returns fp32 also under torch.autocast, and its values are bit-identical to the render epilogue's at the same inputs.  In
+        eval mode it is the host-side field over `encoders`, without autograd."""
+        if self.training:
+            dev = self._require_cuda()
+            if any(torch.is_tensor(t) and t.requires_grad for t in (x, image, weights_sum, lm68)):
+                raise NotImplementedError("gradients w.r.t. the torso positions, the head image, weights_sum or lm68 are not implemented")
+            if lm68 is None:
+                raise ValueError("the torso-SR field is conditioned on lm68 (radnerf_torso_sr.py:84)")
+            from . import train_ops
+            to = (lambda t: None if t is None else t.to(dev))
+            with torch.autocast("cuda", enabled=False):
+                return train_ops.torso_sr_field(self, x.to(dev), lm68.to(dev), to(c), to(image), to(weights_sum), *train_ops.torso_sr_params(self))
         enc = self.encoders
         x = x * self.torso_shrink
         enc_x = enc.freq_encode(x, 10)

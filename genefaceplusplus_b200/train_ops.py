@@ -9,7 +9,7 @@ meaning and autograd behaviour -- over csrc/train_kernels.cu through the C-ABI (
 
 `field` is RADNeRF.forward with its gradient (include/gfpp.h section G, csrc/field_train_kernel.cu); RADNeRF.forward calls it.
 `torso_field` is RADNeRFTorso.forward_torso with its gradient (section H, csrc/torso_train_kernel.cu); forward_torso calls it in
-training mode.
+training mode.  `torso_sr_field` is the same for RADNeRFTorsowithSR.forward_torso (section I, csrc/torso_sr_train_kernel.cu).
 
 fp32 only (the reference casts with custom_fwd(cast_inputs=float32) as well); CUDA tensors only -- there is no CPU path.
 Differences from the reference, both deliberate: march_rays_train lays the samples out in ray order (deterministic; the
@@ -429,3 +429,129 @@ class _torso_field(Function):
 
 
 torso_field = _torso_field.apply
+
+
+# ------------------------------------------------------------------------------------------------ the torso-SR field
+def _torso_sr_field_workspace(model, M):
+    need = _capi.lib().gfpp_torso_sr_field_workspace_bytes(M)
+    if need == 0:
+        raise _capi.GfppError(f"the torso-SR training field does not support {M} points per call")
+    dev = model.density_bitfield.device
+    ws = model.__dict__.get("_torso_sr_field_ws")
+    if ws is None or ws.numel() < need or ws.device != dev:
+        ws = model.__dict__["_torso_sr_field_ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+    return ws
+
+
+def torso_sr_params(model):
+    """The parameters of RADNeRFTorsowithSR's torso field in the order torso_sr_field takes them: the six torso MLP weights, the torso
+    grid table and, with torso_head_aware, the three weights then the three biases of head_color_weights_encoder."""
+    p = ([model.torso_deform_net.net[i].weight for i in range(3)] + [model.torso_canonicial_net.net[i].weight for i in range(3)] +
+         [model.torso_embedder.embeddings])
+    if model.torso_head_aware:
+        lins = [model.head_color_weights_encoder[i] for i in (0, 2, 4)]
+        p += [lin.weight for lin in lins] + [lin.bias for lin in lins]
+    return p
+
+
+def _torso_sr_field_desc(model, params, keep):
+    """The gfpp_torso_sr_desc fields section (I) reads -- torso grid, the six torso weights, torso_code_dim, head_aware and the
+    encoder, torso_shrink -- from `params` (torso_sr_params order), with no device-to-host copy."""
+    d = _capi.TorsoSrDesc()
+    gp = model.torso_embedder
+    lay = gp.layout
+    ws = [_cuda_f32(p.detach()) for p in params]
+    off = _host_offsets(gp)
+    keep += ws + [off]
+    g = d.torso_grid
+    g.embeddings, g.offsets_host = ws[6].data_ptr(), off.ctypes.data
+    g.input_dim, g.num_levels, g.base_resolution = lay.input_dim, lay.num_levels, lay.base_resolution
+    g.log2_per_level_scale, g.gridtype, g.interp, g.align_corners = float(lay.S), lay.gridtype_id, lay.interp_id, int(lay.align_corners)
+    for i in range(3):
+        d.torso_deform_w[i], d.torso_canon_w[i] = ws[i].data_ptr(), ws[3 + i].data_ptr()
+    d.torso_code_dim = model.torso_individual_embedding_dim
+    d.head_aware = int(model.torso_head_aware)
+    if model.torso_head_aware:
+        for i in range(3):
+            d.ha_w[i], d.ha_b[i] = ws[7 + i].data_ptr(), ws[10 + i].data_ptr()
+    d.torso_shrink = float(model.torso_shrink)
+    return d
+
+
+class _torso_sr_field(Function):
+    """RADNeRFTorsowithSR.forward_torso (radnerf_torso_sr.py:75-114) over gfpp_torso_sr_field_forward / gfpp_torso_sr_field_backward:
+    (x [M,2] in [-1,1], lm68 (136 values), code [torso_code_dim] or [1,torso_code_dim] or None, image [M,3] and weights_sum [M,1] /
+    [M] or both None) -> (alpha [M,1], color [M,3], dx [M,2]).  image and weights_sum are read only with torso_head_aware (None:
+    zeros, the reference's image=None path).  `params` are the model's torso_sr_params, passed so that autograd routes their
+    gradients; the kernels read them in place.  `code` may be a view such as torso_individual_codes[index]: autograd then routes
+    its gradient to that row only.  No gradient reaches x, lm68, image or weights_sum (the caller rejects inputs that require one)."""
+
+    @staticmethod
+    def forward(ctx, model, x, lm68, code, image, weights_sum, *params):
+        xy = _cuda_f32(x).view(-1, 2)
+        lm = _cuda_f32(lm68).reshape(-1)
+        if lm.numel() != 136:
+            raise ValueError(f"lm68 must hold the 68 2-D landmarks of one frame (136 values), got shape {tuple(lm68.shape)}")
+        cdim = model.torso_individual_embedding_dim
+        if (code is None) != (cdim == 0) or (code is not None and code.numel() != cdim):
+            raise ValueError(f"c must hold {cdim} values (None iff the model has no torso_individual_codes)")
+        M, dev = xy.shape[0], xy.device
+        if not model.torso_head_aware:
+            image = weights_sum = None                      # the reference ignores them without torso_head_aware
+        if (image is None) != (weights_sum is None):
+            raise ValueError("image and weights_sum must both be given or both be None")
+        img = ws_ = None
+        if image is not None:
+            img, ws_ = _cuda_f32(image).reshape(-1, 3), _cuda_f32(weights_sum).reshape(-1)
+            if img.shape[0] != M or ws_.numel() != M:
+                raise ValueError(f"image must be [{M},3] and weights_sum [{M},1], got {tuple(image.shape)} and {tuple(weights_sum.shape)}")
+        cd = _cuda_f32(code).reshape(-1) if code is not None else None
+        alpha = torch.empty(M, 1, dtype=torch.float32, device=dev)
+        color = torch.empty(M, 3, dtype=torch.float32, device=dev)
+        dx = torch.empty(M, 2, dtype=torch.float32, device=dev)
+        keep = []
+        d = _torso_sr_field_desc(model, params, keep)
+        ws = _torso_sr_field_workspace(model, 0)
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_torso_sr_field_forward(ctypes.byref(d), xy.data_ptr(), M, lm.data_ptr(), None if cd is None else cd.data_ptr(),
+                                                                None if img is None else img.data_ptr(), None if ws_ is None else ws_.data_ptr(),
+                                                                alpha.data_ptr(), color.data_ptr(), dx.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                                _capi.stream_ptr(dev)), "gfpp_torso_sr_field_forward")
+        ctx.model = model
+        ctx.code_shape = None if code is None else code.shape
+        ctx.has_image = img is not None
+        empty = torch.empty(0, device=dev)
+        ctx.save_for_backward(xy, lm, cd if cd is not None else empty, img if img is not None else empty, ws_ if ws_ is not None else empty, *params)
+        return alpha, color, dx
+
+    @staticmethod
+    def backward(ctx, g_alpha, g_color, g_dx):
+        xy, lm, cd, img, ws_, *params = ctx.saved_tensors
+        model, code_shape = ctx.model, ctx.code_shape
+        M, dev = xy.shape[0], xy.device
+        g_alpha = torch.zeros(M, device=dev) if g_alpha is None else _cuda_f32(g_alpha).reshape(-1)
+        g_color = torch.zeros(M, 3, device=dev) if g_color is None else _cuda_f32(g_color)
+        g_dx = torch.zeros(M, 2, device=dev) if g_dx is None else _cuda_f32(g_dx)
+        alloc = torch.zeros if M == 0 else torch.empty
+        grads = [alloc(p.shape, dtype=torch.float32, device=dev) for p in params]
+        grads[6] = torch.zeros(params[6].shape, dtype=torch.float32, device=dev)      # the table gradient is accumulated into
+        g_code = alloc(cd.shape, dtype=torch.float32, device=dev) if code_shape is not None else None
+        keep = []
+        d = _torso_sr_field_desc(model, params, keep)
+        ws = _torso_sr_field_workspace(model, M)
+        P3 = ctypes.c_void_p * 3
+        p_def, p_can = P3(*[g.data_ptr() for g in grads[:3]]), P3(*[g.data_ptr() for g in grads[3:6]])
+        p_haw = P3(*[g.data_ptr() for g in grads[7:10]]) if len(grads) > 7 else None
+        p_hab = P3(*[g.data_ptr() for g in grads[10:13]]) if len(grads) > 7 else None
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_torso_sr_field_backward(
+                ctypes.byref(d), xy.data_ptr(), M, lm.data_ptr(), None if code_shape is None else cd.data_ptr(),
+                img.data_ptr() if ctx.has_image else None, ws_.data_ptr() if ctx.has_image else None, g_alpha.data_ptr(), g_color.data_ptr(),
+                g_dx.data_ptr(), ctypes.byref(p_def), ctypes.byref(p_can), None if p_haw is None else ctypes.byref(p_haw),
+                None if p_hab is None else ctypes.byref(p_hab), None if g_code is None else g_code.data_ptr(), grads[6].data_ptr(),
+                ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_torso_sr_field_backward")
+        grads = [g.to(p.dtype) for g, p in zip(grads, params)]
+        return (None, None, None, None if g_code is None else g_code.view(code_shape), None, None, *grads)
+
+
+torso_sr_field = _torso_sr_field.apply

@@ -37,6 +37,8 @@
  *  (G) the trainable head field: RADNeRF.forward and its backward at explicit points, fp32.
  *
  *  (H) the trainable torso field: RADNeRFTorso.forward_torso and its backward at explicit points, fp32.
+ *
+ *  (I) the trainable torso-SR field: RADNeRFTorsowithSR.forward_torso and its backward at explicit points, fp32.
  */
 #ifndef GFPP_H_
 #define GFPP_H_
@@ -505,6 +507,47 @@ GFPP_API int gfpp_torso_field_backward(const gfpp_model_desc *desc, const float 
                                        const float *grad_alpha, const float *grad_color, const float *grad_deform,
                                        float *const grad_deform_w[3], float *const grad_canon_w[3], float *grad_code,
                                        float *grad_torso_table, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------ (I) trainable torso-SR field
+ *
+ * RADNeRFTorsowithSR.forward_torso (modules/radnerfs/radnerf_torso_sr.py:75-114) and its gradient for the torso training step
+ * (on_train_torso_nerf), in fp32 FFMA arithmetic, reading the parameters IN PLACE through a gfpp_torso_sr_desc -- no
+ * gfpp_torso_sr_pack.  Read from the desc: torso_grid (2-D, 16 levels x 2, reference layout [entries,2] fp32, 8-byte aligned),
+ * torso_deform_w (64,din) (64,64) (2,64), torso_canon_w (32,32+din) (32,32) (4,32) with din = 42 + torso_code_dim + 126 (+ 16 with
+ * head_aware), torso_code_dim (<= 10), head_aware, ha_w / ha_b (head_color_weights_encoder (16,4) (32,16) (16,32) and its biases;
+ * read iff head_aware) and torso_shrink.  The other desc fields are not read (torso_code neither: `code` is an explicit argument,
+ * the training row torso_individual_codes[index]; it is NULL iff torso_code_dim == 0).  lm68 [136] are the frame's landmarks
+ * (points 5..11 are used).  image [M,3] and weights_sum [M] are the head colour and alpha at the points that the head-aware encoder
+ * sees; both NULL means zeros (the reference's image=None path).  Passing only one of them, or passing them without head_aware, is
+ * invalid.  Every argument is validated before any CUDA call; M == 0 then returns GFPP_OK without touching the device (the point
+ * and output pointers may be NULL).  Everything is enqueued on `stream` with no host synchronisation and no allocation.
+ *
+ * Workspace (256-byte aligned): gfpp_torso_sr_field_workspace_bytes(M) for the backward (0 = unsupported M); the forward needs
+ * gfpp_torso_sr_field_workspace_bytes(0) bytes (the per-call k-major copy of the weights and the encoder and the two folded bias
+ * vectors, ~52 KB).
+ *
+ * gfpp_torso_sr_field_forward: for points xy [M,2] in [-1,1]: alpha [M], color [M,3] (sigmoid), deform [M,2] (dx, before the clamp).
+ *   It is the render epilogue's own field code (k_torso_sr) on these points: bit-identical to gfpp_torso_sr_composite's
+ *   torso_alpha_map and torso_deform at its masked pixels, for the same parameters, code, lm68, image and weights_sum.
+ * gfpp_torso_sr_field_backward: given grad_alpha [M], grad_color [M,3] and grad_deform [M,2] (w.r.t. dx), recomputes the forward and
+ *   writes grad_deform_w[0..2], grad_canon_w[0..2], grad_ha_w[0..2], grad_ha_b[0..2] (same layouts as the parameters; overwritten;
+ *   the grad_ha_* arrays are NULL iff head_aware == 0) and grad_code [torso_code_dim] (the code is repeated over the points: its
+ *   gradient is the sum; NULL iff torso_code_dim == 0); grad_torso_table [entries,2] is ACCUMULATED into (+=), as the reference's grid
+ *   backward does.  The grid's input gradient goes through its dy_dx, the (x+1)/2 map of bound 1 and the clamp (which passes the
+ *   gradient on [-1, 1] inclusive); the head-aware encoding's gradient is the sum over both first layers' encoding columns, then
+ *   through the encoder (LeakyReLU slope 0.02 where its output is <= 0).  lm68, xy, image and weights_sum get no gradient.
+ * Determinism: the forward outputs and every gradient except the table's are bit-identical from run to run (per-CTA partial sums in
+ * the workspace, reduced in a fixed order by one kernel; the partitioning depends only on M).  The table gradient is scattered with
+ * float2 vector reductions, so its summation order is free. */
+GFPP_API size_t gfpp_torso_sr_field_workspace_bytes(uint32_t M);
+GFPP_API int gfpp_torso_sr_field_forward(const gfpp_torso_sr_desc *desc, const float *xy, uint32_t M, const float *lm68, const float *code,
+                                         const float *image, const float *weights_sum, float *alpha, float *color, float *deform,
+                                         void *workspace, size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_torso_sr_field_backward(const gfpp_torso_sr_desc *desc, const float *xy, uint32_t M, const float *lm68, const float *code,
+                                          const float *image, const float *weights_sum, const float *grad_alpha, const float *grad_color,
+                                          const float *grad_deform, float *const grad_deform_w[3], float *const grad_canon_w[3],
+                                          float *const grad_ha_w[3], float *const grad_ha_b[3], float *grad_code, float *grad_torso_table,
+                                          void *workspace, size_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }
