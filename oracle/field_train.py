@@ -139,19 +139,24 @@ class _CompositeTrain(Function):
         return gs, gr, ga, None, None, None
 
 
-def render_train(params, hp, state, rays_o, rays_d, cond_feat, individual_code, bg_color, density_scale, max_steps, dt_gamma=0.0):
-    """The training branch of render() with mean_count 0 (all samples kept, truncated to the count rounded up to 128, as
-    march_rays_train does), perturb False and composite_rays_train's default T_thresh."""
+def render_train(params, hp, state, rays_o, rays_d, cond_feat, individual_code, bg_color, density_scale, max_steps, dt_gamma=0.0,
+                 mean_count=0):
+    """The training branch of render() with perturb False and composite_rays_train's default T_thresh.  mean_count <= 0 (the first
+    steps): all samples kept, truncated to the count rounded up to 128.  mean_count > 0 (every step after update_extra_state): the
+    sample buffer has M = mean_count rounded up to 128 rows (raymarching.py:201-204: a multiple of 128 still gains 128), and a ray
+    whose samples would pass M keeps its `rays` row but gets none, so it composites to weights_sum = ambient = 0 and the background."""
     bound = hp["bound"]
     cascade = 1 + int(np.ceil(np.log2(bound)))
     prefix = rays_o.shape[:-1]
     ro, rd = rays_o.reshape(-1, 3).float().contiguous(), rays_d.reshape(-1, 3).float().contiguous()
     nears, fars = ops.near_far_from_aabb(ro, rd, state["aabb_train"], hp["min_near"])
+    M = None if mean_count <= 0 else mean_count + 128 - mean_count % 128
     xyzs, dirs, deltas, rays, counter = ops.march_rays_train(ro, rd, bound, state["density_bitfield"], cascade, hp["grid_size"], nears, fars,
-                                                             dt_gamma=dt_gamma, max_steps=max_steps)
-    m = int(counter[0])
-    m += 128 - m % 128
-    xyzs, dirs, deltas = xyzs[:m], dirs[:m], deltas[:m]
+                                                             M=M, dt_gamma=dt_gamma, max_steps=max_steps)
+    if M is None:
+        m = int(counter[0])
+        m += 128 - m % 128
+        xyzs, dirs, deltas = xyzs[:m], dirs[:m], deltas[:m]
     sigmas, rgbs, ambient = field_forward(params, hp, xyzs, dirs, cond_feat, individual_code)
     sigmas = density_scale * sigmas
     ws, asum, depth, image = _CompositeTrain.apply(sigmas, rgbs, ambient.abs().sum(-1), deltas, rays, 1e-4)
