@@ -15,7 +15,6 @@
 #include "torso_grid_kernel.cuh"
 #include "torso_kernel.cuh"
 #include "torso_sr_kernel.cuh"
-#include "torso_sr_train_kernel.cuh"
 #include "torso_train_kernel.cuh"
 
 namespace gfpp {
@@ -1546,16 +1545,22 @@ int gfpp_field_backward(const gfpp_model_desc *desc, const float *xyzs, const fl
     return GFPP_OK;
 }
 
-// ---------------------------------------------------------------- (H) trainable torso field
+// ---------------------------------------------------------------- (H) and (I) trainable torso fields
+// Both fields run the kernels of torso_train_kernel.cu: SR = false for the plain torso (H), SR = true for the torso-SR model (I).
+extern "C++" {   // the helpers are templates
 static uint32_t torso_field_ctas(uint32_t M) {
     const uint32_t tiles = (M + TORSO_TRAIN_TP - 1) / TORSO_TRAIN_TP;
     return tiles < (uint32_t)TORSO_TRAIN_CTAS ? tiles : (uint32_t)TORSO_TRAIN_CTAS;
 }
-static size_t torso_wt_bytes() { return (TorsoWt::total * 4 + 255) / 256 * 256; }
+template <bool SR> static size_t torso_wt_bytes() { return (TorsoWt<SR>::total * 4 + 255) / 256 * 256; }
+template <bool SR> static size_t torso_field_ws_bytes(uint32_t M) {
+    if (M >= (1u << 31)) return 0;
+    return torso_wt_bytes<SR>() + (size_t)torso_field_ctas(M) * TorsoPart<SR>::total * 4;
+}
 
-// Validates the desc's torso fields, pose6 and code (everything the kernels read besides the points) and fills the model half of
-// TorsoTrainArgs; no CUDA call.
-static int torso_field_setup(const char *who, const gfpp_model_desc *d, const float *pose6, const float *code, TorsoTrainArgs &a) {
+// Validates what both fields' descs hold -- the torso grid, the six weights, torso_code_dim -- and the code, and fills that part of
+// TorsoTrainArgs; no CUDA call.  Desc is gfpp_model_desc (H) or gfpp_torso_sr_desc (I).
+template <class Desc> static int torso_field_setup(const char *who, const Desc *d, const float *code, TorsoTrainArgs &a) {
     if (!d) return fail(GFPP_ERR_INVALID, "%s: null desc", who);
     memset(&a, 0, sizeof(a));
     const gfpp_grid_desc &g = d->torso_grid;
@@ -1572,108 +1577,18 @@ static int torso_field_setup(const char *who, const gfpp_model_desc *d, const fl
     }
     if (d->torso_code_dim > 10) return fail(GFPP_ERR_UNSUPPORTED, "%s: torso_code_dim must be <= 10", who);
     if ((code == nullptr) != (d->torso_code_dim == 0)) return fail(GFPP_ERR_INVALID, "%s: code must be given iff torso_code_dim > 0", who);
-    if (!pose6) return fail(GFPP_ERR_INVALID, "%s: null pose6", who);
     a.tab = (const float2 *)g.embeddings;
-    a.pose6 = pose6;
     a.code = code;
     a.code_dim = (int)d->torso_code_dim;
     a.shrink = d->torso_shrink;
     return GFPP_OK;
 }
 
-size_t gfpp_torso_field_workspace_bytes(uint32_t M) {
-    if (M >= (1u << 31)) return 0;
-    return torso_wt_bytes() + (size_t)torso_field_ctas(M) * TorsoPart::total * 4;
-}
-
-int gfpp_torso_field_forward(const gfpp_model_desc *desc, const float *xy, uint32_t M, const float *pose6, const float *code, float *alpha,
-                             float *color, float *deform, void *workspace, size_t workspace_bytes, void *stream) {
-    TorsoTrainArgs a;
-    const int rc = torso_field_setup("torso_field_forward", desc, pose6, code, a);
-    if (rc != GFPP_OK) return rc;
-    g_launches = 0;
-    if (M == 0) return GFPP_OK;
-    if (!xy || !alpha || !color || !deform || !workspace) return fail(GFPP_ERR_INVALID, "torso_field_forward: null pointer%s");
-    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_field_forward: M must be < 2^31%s");
-    if (workspace_bytes < torso_wt_bytes()) return fail(GFPP_ERR_WORKSPACE, "torso_field_forward: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_field_forward: workspace must be 256-byte aligned%s");
-    a.wt = (float *)workspace;
-    cudaStream_t st = (cudaStream_t)stream;
-    CK(launch_torso_field_relayout(a, st));
-    // the inference query's kernel on the re-laid-out weights: the same values as gfpp_torso_query at the same parameters
-    TorsoQueryArgs q;
-    memset(&q, 0, sizeof(q));
-    q.tor_gm = a.gm; q.tor_tab = a.tab;
-    q.w_def0 = a.wt + TorsoWt::wd0; q.w_def1 = a.wt + TorsoWt::wd1; q.w_def2 = a.wt + TorsoWt::wd2;
-    q.w_can0 = a.wt + TorsoWt::wc0; q.w_can1 = a.wt + TorsoWt::wc1; q.w_can2 = a.wt + TorsoWt::wc2;
-    q.bias_def = a.wt + TorsoWt::bias_def; q.bias_can = a.wt + TorsoWt::bias_can;
-    q.torso_shrink = a.shrink;
-    q.n = M; q.xy = xy;
-    q.alpha = alpha; q.color = color; q.deform = deform;
-    CK(launch_torso_query(q, st));
-    return GFPP_OK;
-}
-
-int gfpp_torso_field_backward(const gfpp_model_desc *desc, const float *xy, uint32_t M, const float *pose6, const float *code,
-                              const float *grad_alpha, const float *grad_color, const float *grad_deform, float *const grad_deform_w[3],
-                              float *const grad_canon_w[3], float *grad_code, float *grad_torso_table, void *workspace, size_t workspace_bytes,
-                              void *stream) {
-    TorsoTrainArgs a;
-    const int rc = torso_field_setup("torso_field_backward", desc, pose6, code, a);
-    if (rc != GFPP_OK) return rc;
-    g_launches = 0;
-    if (M == 0) return GFPP_OK;
-    if (!xy || !grad_alpha || !grad_color || !grad_deform || !grad_deform_w || !grad_canon_w || !grad_torso_table || !workspace ||
-        (a.code_dim > 0 && !grad_code))
-        return fail(GFPP_ERR_INVALID, "torso_field_backward: null pointer%s");
-    for (int i = 0; i < 3; ++i)
-        if (!grad_deform_w[i] || !grad_canon_w[i]) return fail(GFPP_ERR_INVALID, "torso_field_backward: null weight gradient%s");
-    if (((uintptr_t)grad_torso_table & 7u) != 0) return fail(GFPP_ERR_INVALID, "torso_field_backward: the table gradient must be 8-byte aligned%s");
-    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_field_backward: M must be < 2^31%s");
-    if (workspace_bytes < gfpp_torso_field_workspace_bytes(M)) return fail(GFPP_ERR_WORKSPACE, "torso_field_backward: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_field_backward: workspace must be 256-byte aligned%s");
-    a.M = M; a.xy = xy;
-    a.wt = (float *)workspace;
-    a.part = (float *)((char *)workspace + torso_wt_bytes());
-    a.n_cta = torso_field_ctas(M);
-    a.g_alpha = grad_alpha; a.g_color = grad_color; a.g_deform = grad_deform;
-    a.g_tab = (float2 *)grad_torso_table;
-    for (int i = 0; i < 3; ++i) { a.g_def[i] = grad_deform_w[i]; a.g_can[i] = grad_canon_w[i]; }
-    a.g_code = grad_code;
-    cudaStream_t st = (cudaStream_t)stream;
-    CK(launch_torso_field_relayout(a, st));
-    CK(launch_torso_field_bwd(a, st));
-    CK(launch_torso_field_reduce(a, st));
-    return GFPP_OK;
-}
-
-// ---------------------------------------------------------------- (I) trainable torso-SR field
-static uint32_t torso_sr_field_ctas(uint32_t M) {
-    const uint32_t tiles = (M + TORSO_SR_TRAIN_TP - 1) / TORSO_SR_TRAIN_TP;
-    return tiles < (uint32_t)TORSO_SR_TRAIN_CTAS ? tiles : (uint32_t)TORSO_SR_TRAIN_CTAS;
-}
-static size_t torso_sr_wt_bytes() { return (TorsoSrWt::total * 4 + 255) / 256 * 256; }
-
-// Validates the desc's torso fields, lm68, code and the head-aware inputs (everything the kernels read besides the points) and fills
-// the model half of TorsoSrTrainArgs; no CUDA call.
+// The section (I) setup: the shared part, then lm68, the head-aware encoder and its image / weights_sum inputs.
 static int torso_sr_field_setup(const char *who, const gfpp_torso_sr_desc *d, const float *lm68, const float *code, const float *image,
-                                const float *weights_sum, TorsoSrTrainArgs &a) {
-    if (!d) return fail(GFPP_ERR_INVALID, "%s: null desc", who);
-    memset(&a, 0, sizeof(a));
-    const gfpp_grid_desc &g = d->torso_grid;
-    if (!g.embeddings || !g.offsets_host) return fail(GFPP_ERR_INVALID, "%s: null torso grid table or offsets", who);
-    if (g.num_levels != 16 ||
-        fill_grid_meta(a.gm, g.offsets_host, g.input_dim, g.num_levels, g.log2_per_level_scale, g.base_resolution, g.gridtype,
-                       g.align_corners, g.interp) != 0 || a.gm.dim != 2)
-        return fail(GFPP_ERR_UNSUPPORTED, "%s: the torso grid must be 2-D with 16 levels x 2 features", who);
-    if (((uintptr_t)g.embeddings & 7u) != 0) return fail(GFPP_ERR_INVALID, "%s: the torso grid table must be 8-byte aligned", who);
-    for (int i = 0; i < 3; ++i) {
-        if (!d->torso_deform_w[i] || !d->torso_canon_w[i]) return fail(GFPP_ERR_INVALID, "%s: null torso weight", who);
-        a.w_def[i] = d->torso_deform_w[i];
-        a.w_can[i] = d->torso_canon_w[i];
-    }
-    if (d->torso_code_dim > 10) return fail(GFPP_ERR_UNSUPPORTED, "%s: torso_code_dim must be <= 10", who);
-    if ((code == nullptr) != (d->torso_code_dim == 0)) return fail(GFPP_ERR_INVALID, "%s: code must be given iff torso_code_dim > 0", who);
+                                const float *weights_sum, TorsoTrainArgs &a) {
+    const int rc = torso_field_setup(who, d, code, a);
+    if (rc != GFPP_OK) return rc;
     if (!lm68) return fail(GFPP_ERR_INVALID, "%s: null lm68", who);
     if ((image == nullptr) != (weights_sum == nullptr)) return fail(GFPP_ERR_INVALID, "%s: image and weights_sum must both be given or both be NULL", who);
     if (d->head_aware) {
@@ -1686,44 +1601,123 @@ static int torso_sr_field_setup(const char *who, const gfpp_torso_sr_desc *d, co
         return fail(GFPP_ERR_INVALID, "%s: image and weights_sum are only read with head_aware", who);
     }
     a.head_aware = d->head_aware ? 1 : 0;
-    a.tab = (const float2 *)g.embeddings;
-    a.lm68 = lm68;
-    a.code = code;
-    a.code_dim = (int)d->torso_code_dim;
-    a.shrink = d->torso_shrink;
+    a.cond = lm68;
     a.image = image;
     a.wsum = weights_sum;
     return GFPP_OK;
 }
 
-size_t gfpp_torso_sr_field_workspace_bytes(uint32_t M) {
-    if (M >= (1u << 31)) return 0;
-    return torso_sr_wt_bytes() + (size_t)torso_sr_field_ctas(M) * TorsoSrPart::total * 4;
+// The forward's checks after the setup, then the relayout into the workspace; M = 0 returns before it.
+template <bool SR>
+static int torso_field_relayout(const char *who, TorsoTrainArgs &a, const float *xy, uint32_t M, const float *alpha, const float *color,
+                                const float *deform, void *workspace, size_t workspace_bytes, cudaStream_t st) {
+    if (!xy || !alpha || !color || !deform || !workspace) return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
+    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: M must be < 2^31", who);
+    if (workspace_bytes < torso_wt_bytes<SR>()) return fail(GFPP_ERR_WORKSPACE, "%s: workspace too small", who);
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
+    a.wt = (float *)workspace;
+    CK(launch_torso_field_relayout<SR>(a, st));
+    return GFPP_OK;
 }
+
+// The backward after the setup: the checks both fields share, then relayout, backward and reduce.
+template <bool SR>
+static int torso_field_backward(const char *who, TorsoTrainArgs &a, const float *xy, uint32_t M, const float *grad_alpha,
+                                const float *grad_color, const float *grad_deform, float *const grad_deform_w[3],
+                                float *const grad_canon_w[3], float *grad_code, float *grad_torso_table, void *workspace,
+                                size_t workspace_bytes, void *stream) {
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xy || !grad_alpha || !grad_color || !grad_deform || !grad_deform_w || !grad_canon_w || !grad_torso_table || !workspace ||
+        (a.code_dim > 0 && !grad_code))
+        return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
+    for (int i = 0; i < 3; ++i)
+        if (!grad_deform_w[i] || !grad_canon_w[i]) return fail(GFPP_ERR_INVALID, "%s: null weight gradient", who);
+    if (((uintptr_t)grad_torso_table & 7u) != 0) return fail(GFPP_ERR_INVALID, "%s: the table gradient must be 8-byte aligned", who);
+    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: M must be < 2^31", who);
+    if (workspace_bytes < torso_field_ws_bytes<SR>(M)) return fail(GFPP_ERR_WORKSPACE, "%s: workspace too small", who);
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
+    a.M = M; a.xy = xy;
+    a.wt = (float *)workspace;
+    a.part = (float *)((char *)workspace + torso_wt_bytes<SR>());
+    a.n_cta = torso_field_ctas(M);
+    a.g_alpha = grad_alpha; a.g_color = grad_color; a.g_deform = grad_deform;
+    a.g_tab = (float2 *)grad_torso_table;
+    for (int i = 0; i < 3; ++i) { a.g_def[i] = grad_deform_w[i]; a.g_can[i] = grad_canon_w[i]; }
+    a.g_code = grad_code;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_torso_field_relayout<SR>(a, st));
+    CK(launch_torso_field_bwd<SR>(a, st));
+    CK(launch_torso_field_reduce<SR>(a, st));
+    return GFPP_OK;
+}
+
+}  // extern "C++"
+
+size_t gfpp_torso_field_workspace_bytes(uint32_t M) { return torso_field_ws_bytes<false>(M); }
+
+int gfpp_torso_field_forward(const gfpp_model_desc *desc, const float *xy, uint32_t M, const float *pose6, const float *code, float *alpha,
+                             float *color, float *deform, void *workspace, size_t workspace_bytes, void *stream) {
+    TorsoTrainArgs a;
+    int rc = torso_field_setup("torso_field_forward", desc, code, a);
+    if (rc != GFPP_OK) return rc;
+    if (!pose6) return fail(GFPP_ERR_INVALID, "torso_field_forward: null pose6%s");
+    a.cond = pose6;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    rc = torso_field_relayout<false>("torso_field_forward", a, xy, M, alpha, color, deform, workspace, workspace_bytes, st);
+    if (rc != GFPP_OK) return rc;
+    // the inference query's kernel on the re-laid-out weights: the same values as gfpp_torso_query at the same parameters
+    using W = TorsoWt<false>;
+    TorsoQueryArgs q;
+    memset(&q, 0, sizeof(q));
+    q.tor_gm = a.gm; q.tor_tab = a.tab;
+    q.w_def0 = a.wt + W::wd0; q.w_def1 = a.wt + W::wd1; q.w_def2 = a.wt + W::wd2;
+    q.w_can0 = a.wt + W::wc0; q.w_can1 = a.wt + W::wc1; q.w_can2 = a.wt + W::wc2;
+    q.bias_def = a.wt + W::bias_def; q.bias_can = a.wt + W::bias_can;
+    q.torso_shrink = a.shrink;
+    q.n = M; q.xy = xy;
+    q.alpha = alpha; q.color = color; q.deform = deform;
+    CK(launch_torso_query(q, st));
+    return GFPP_OK;
+}
+
+int gfpp_torso_field_backward(const gfpp_model_desc *desc, const float *xy, uint32_t M, const float *pose6, const float *code,
+                              const float *grad_alpha, const float *grad_color, const float *grad_deform, float *const grad_deform_w[3],
+                              float *const grad_canon_w[3], float *grad_code, float *grad_torso_table, void *workspace, size_t workspace_bytes,
+                              void *stream) {
+    TorsoTrainArgs a;
+    const int rc = torso_field_setup("torso_field_backward", desc, code, a);
+    if (rc != GFPP_OK) return rc;
+    if (!pose6) return fail(GFPP_ERR_INVALID, "torso_field_backward: null pose6%s");
+    a.cond = pose6;
+    return torso_field_backward<false>("torso_field_backward", a, xy, M, grad_alpha, grad_color, grad_deform, grad_deform_w, grad_canon_w,
+                                       grad_code, grad_torso_table, workspace, workspace_bytes, stream);
+}
+
+size_t gfpp_torso_sr_field_workspace_bytes(uint32_t M) { return torso_field_ws_bytes<true>(M); }
 
 int gfpp_torso_sr_field_forward(const gfpp_torso_sr_desc *desc, const float *xy, uint32_t M, const float *lm68, const float *code,
                                 const float *image, const float *weights_sum, float *alpha, float *color, float *deform, void *workspace,
                                 size_t workspace_bytes, void *stream) {
-    TorsoSrTrainArgs a;
-    const int rc = torso_sr_field_setup("torso_sr_field_forward", desc, lm68, code, image, weights_sum, a);
+    TorsoTrainArgs a;
+    int rc = torso_sr_field_setup("torso_sr_field_forward", desc, lm68, code, image, weights_sum, a);
     if (rc != GFPP_OK) return rc;
     g_launches = 0;
     if (M == 0) return GFPP_OK;
-    if (!xy || !alpha || !color || !deform || !workspace) return fail(GFPP_ERR_INVALID, "torso_sr_field_forward: null pointer%s");
-    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_field_forward: M must be < 2^31%s");
-    if (workspace_bytes < torso_sr_wt_bytes()) return fail(GFPP_ERR_WORKSPACE, "torso_sr_field_forward: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_sr_field_forward: workspace must be 256-byte aligned%s");
-    a.wt = (float *)workspace;
     cudaStream_t st = (cudaStream_t)stream;
-    CK(launch_torso_sr_field_relayout(a, st));
+    rc = torso_field_relayout<true>("torso_sr_field_forward", a, xy, M, alpha, color, deform, workspace, workspace_bytes, st);
+    if (rc != GFPP_OK) return rc;
     // k_torso_sr's field in its point mode on the re-laid-out weights: the same values as the render epilogue at the same parameters
+    using W = TorsoWt<true>;
     TorsoSrArgs t;
     memset(&t, 0, sizeof(t));
     t.tor_gm = a.gm; t.tor_tab = a.tab;
-    t.w_def0 = a.wt + TorsoSrWt::wd0; t.w_def1 = a.wt + TorsoSrWt::wd1; t.w_def2 = a.wt + TorsoSrWt::wd2;
-    t.w_can0 = a.wt + TorsoSrWt::wc0; t.w_can1 = a.wt + TorsoSrWt::wc1; t.w_can2 = a.wt + TorsoSrWt::wc2;
-    t.ha = a.head_aware ? a.wt + TorsoSrWt::ha : nullptr;
-    t.bias_def = a.wt + TorsoSrWt::bias_def; t.bias_can = a.wt + TorsoSrWt::bias_can;
+    t.w_def0 = a.wt + W::wd0; t.w_def1 = a.wt + W::wd1; t.w_def2 = a.wt + W::wd2;
+    t.w_can0 = a.wt + W::wc0; t.w_can1 = a.wt + W::wc1; t.w_can2 = a.wt + W::wc2;
+    t.ha = a.head_aware ? a.wt + W::ha : nullptr;
+    t.bias_def = a.wt + W::bias_def; t.bias_can = a.wt + W::bias_can;
     t.torso_shrink = a.shrink;
     t.bg_coords = xy;
     t.n_frames = 1; t.n_rays = (int)M;
@@ -1738,41 +1732,19 @@ int gfpp_torso_sr_field_backward(const gfpp_torso_sr_desc *desc, const float *xy
                                  const float *grad_deform, float *const grad_deform_w[3], float *const grad_canon_w[3],
                                  float *const grad_ha_w[3], float *const grad_ha_b[3], float *grad_code, float *grad_torso_table,
                                  void *workspace, size_t workspace_bytes, void *stream) {
-    TorsoSrTrainArgs a;
+    TorsoTrainArgs a;
     const int rc = torso_sr_field_setup("torso_sr_field_backward", desc, lm68, code, image, weights_sum, a);
     if (rc != GFPP_OK) return rc;
     if ((grad_ha_w == nullptr) != (a.head_aware == 0) || (grad_ha_b == nullptr) != (a.head_aware == 0))
         return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: grad_ha_w / grad_ha_b must be given iff head_aware%s");
     if (a.head_aware)
-        for (int i = 0; i < 3; ++i)
+        for (int i = 0; i < 3; ++i) {
             if (!grad_ha_w[i] || !grad_ha_b[i]) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: null head-aware gradient%s");
-    g_launches = 0;
-    if (M == 0) return GFPP_OK;
-    if (!xy || !grad_alpha || !grad_color || !grad_deform || !grad_deform_w || !grad_canon_w || !grad_torso_table || !workspace ||
-        (a.code_dim > 0 && !grad_code))
-        return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: null pointer%s");
-    for (int i = 0; i < 3; ++i)
-        if (!grad_deform_w[i] || !grad_canon_w[i]) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: null weight gradient%s");
-    if (((uintptr_t)grad_torso_table & 7u) != 0) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: the table gradient must be 8-byte aligned%s");
-    if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_field_backward: M must be < 2^31%s");
-    if (workspace_bytes < gfpp_torso_sr_field_workspace_bytes(M)) return fail(GFPP_ERR_WORKSPACE, "torso_sr_field_backward: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: workspace must be 256-byte aligned%s");
-    a.M = M; a.xy = xy;
-    a.wt = (float *)workspace;
-    a.part = (float *)((char *)workspace + torso_sr_wt_bytes());
-    a.n_cta = torso_sr_field_ctas(M);
-    a.g_alpha = grad_alpha; a.g_color = grad_color; a.g_deform = grad_deform;
-    a.g_tab = (float2 *)grad_torso_table;
-    for (int i = 0; i < 3; ++i) {
-        a.g_def[i] = grad_deform_w[i]; a.g_can[i] = grad_canon_w[i];
-        if (a.head_aware) { a.g_ha_w[i] = grad_ha_w[i]; a.g_ha_b[i] = grad_ha_b[i]; }
-    }
-    a.g_code = grad_code;
-    cudaStream_t st = (cudaStream_t)stream;
-    CK(launch_torso_sr_field_relayout(a, st));
-    CK(launch_torso_sr_field_bwd(a, st));
-    CK(launch_torso_sr_field_reduce(a, st));
-    return GFPP_OK;
+            a.g_ha_w[i] = grad_ha_w[i];
+            a.g_ha_b[i] = grad_ha_b[i];
+        }
+    return torso_field_backward<true>("torso_sr_field_backward", a, xy, M, grad_alpha, grad_color, grad_deform, grad_deform_w, grad_canon_w,
+                                      grad_code, grad_torso_table, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

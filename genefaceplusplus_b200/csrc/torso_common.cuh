@@ -14,6 +14,9 @@ __device__ __forceinline__ float freq_entry(const float *x, int D, int c) {
     return sinf(__fadd_rn(scalbnf(x[d], f), (float)(col % 2) * (3.141592653589793f / 2)));
 }
 
+// LeakyReLU(0.02) of the torso-SR model's head-aware encoder
+__device__ __forceinline__ float leaky002(float x) { return x > 0.f ? x : 0.02f * x; }
+
 // acc[i][j] += A[row_i][k] * W[k][col_j], rows ty*4+i / 64+ty*4+(i-4), cols tx*NC+j; W is [K][N], N = 16*NC
 template <int NC, int K, int LDT>
 __device__ __forceinline__ void small_gemm(float (&acc)[8][NC], const float *__restrict__ sA, const float *__restrict__ sW,

@@ -38,8 +38,6 @@ template <bool SR> struct QSmem {
     float h2[32], hae[16];
 };
 
-__device__ __forceinline__ float leaky002(float x) { return x > 0.f ? x : 0.02f * x; }
-
 // point p in torso-grid coordinates [-1,1]^2: xy[p], or cell (p % H, p / H) jittered as radnerf_torso.py:221-227 does in fp32:
 // xys = (2*c/(H-1) - 1) * (1 - 1/H) + (noise*2 - 1) * (1/H)
 __device__ __forceinline__ void query_point(const TorsoQueryArgs &q, uint32_t p, float (&pos)[2]) {

@@ -25,8 +25,5 @@ struct Smem {
     int mask[TP];
 };
 
-__device__ __forceinline__ float leaky002(float x) { return x > 0.f ? x : 0.02f * x; }
-
-
 }  // namespace tsr
 }  // namespace gfpp

@@ -8,8 +8,9 @@ meaning and autograd behaviour -- over csrc/train_kernels.cu through the C-ABI (
     weights_sum, ambient_sum, depth, image = raymarching.composite_rays_train(sigmas, rgbs, ambient, deltas, rays, T_thresh)
 
 `field` is RADNeRF.forward with its gradient (include/gfpp.h section G, csrc/field_train_kernel.cu); RADNeRF.forward calls it.
-`torso_field` is RADNeRFTorso.forward_torso with its gradient (section H, csrc/torso_train_kernel.cu); forward_torso calls it in
-training mode.  `torso_sr_field` is the same for RADNeRFTorsowithSR.forward_torso (section I, csrc/torso_sr_train_kernel.cu).
+`torso_field` is RADNeRFTorso.forward_torso with its gradient (section H); forward_torso calls it in training mode.
+`torso_sr_field` is the same for RADNeRFTorsowithSR.forward_torso (section I).  Both run csrc/torso_train_kernel.cu, one source
+instantiated for each field.
 
 fp32 only (the reference casts with custom_fwd(cast_inputs=float32) as well); CUDA tensors only -- there is no CPU path.
 Differences from the reference, both deliberate: march_rays_train lays the samples out in ray order (deterministic; the
@@ -228,15 +229,16 @@ def grad_total_variation(embeddings, offsets, per_level_scale, base_resolution, 
                                                   float(np.log2(per_level_scale)), base_resolution, gridtype, align_corners)
 
 
-# ------------------------------------------------------------------------------------------------ the head field
-def _field_workspace(model, M):
-    need = _capi.lib().gfpp_field_backward_workspace_bytes(M)
+# ------------------------------------------------------------------------------------------------ shared by the training fields
+def _workspace(model, attr, bytes_fn, M, what):
+    """The device workspace of `bytes_fn(M)` bytes, cached on the model as `attr` and regrown when too small."""
+    need = bytes_fn(M)
     if need == 0:
-        raise _capi.GfppError(f"the training field does not support {M} points per call")
+        raise _capi.GfppError(f"{what} does not support {M} points per call")
     dev = model.density_bitfield.device
-    ws = model.__dict__.get("_field_ws")
+    ws = model.__dict__.get(attr)
     if ws is None or ws.numel() < need or ws.device != dev:
-        ws = model.__dict__["_field_ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+        ws = model.__dict__[attr] = torch.empty(need, dtype=torch.uint8, device=dev)
     return ws
 
 
@@ -249,18 +251,39 @@ def _host_offsets(gp):
     return cached[1]
 
 
+def _fill_grid(g, gp, emb, keep):
+    """Fills the gfpp_grid_desc `g` for the _GridParams `gp` with table `emb` and the cached host offsets."""
+    lay = gp.layout
+    off = _host_offsets(gp)
+    keep += [emb, off]
+    g.embeddings, g.offsets_host = emb.data_ptr(), off.ctypes.data
+    g.input_dim, g.num_levels, g.base_resolution = lay.input_dim, lay.num_levels, lay.base_resolution
+    g.log2_per_level_scale, g.gridtype, g.interp, g.align_corners = float(lay.S), lay.gridtype_id, lay.interp_id, int(lay.align_corners)
+
+
+def _backward_buffers(M, dev, upstream, shapes, targets, code, tables):
+    """The common start of the fields' backward: the upstream gradients as contiguous fp32 of `shapes` (zeros where autograd passes
+    None), and fp32 gradient buffers shaped like `targets` and like `code` (None without a code).  The kernels write every element
+    of these buffers except the grid tables' (indices `tables` of `targets`), which they accumulate into; with M = 0 no kernel
+    runs, so all of them are zeros."""
+    up = [torch.zeros(s, device=dev) if g is None else _cuda_f32(g).reshape(s) for g, s in zip(upstream, shapes)]
+
+    def buf(t, accumulated=False):
+        return (torch.zeros if M == 0 or accumulated else torch.empty)(t.shape, dtype=torch.float32, device=dev)
+
+    return up, [buf(t, i in tables) for i, t in enumerate(targets)], None if code is None else buf(code)
+
+
+# ------------------------------------------------------------------------------------------------ the head field
+def _field_workspace(model, M):
+    return _workspace(model, "_field_ws", _capi.lib().gfpp_field_backward_workspace_bytes, M, "the training field")
+
+
 def _field_desc(model, code, keep):
     """The gfpp_model_desc fields section (G) reads -- grids, weights, code, cond_dim, bound, precision -- with no device-to-host copy."""
     d = _capi.ModelDesc()
     for name, gp in (("position_grid", model.position_embedder), ("ambient_grid", model.ambient_embedder)):
-        g = getattr(d, name)
-        lay = gp.layout
-        emb = _cuda_f32(gp.embeddings.detach())
-        off = _host_offsets(gp)
-        keep += [emb, off]
-        g.embeddings, g.offsets_host = emb.data_ptr(), off.ctypes.data
-        g.input_dim, g.num_levels, g.base_resolution = lay.input_dim, lay.num_levels, lay.base_resolution
-        g.log2_per_level_scale, g.gridtype, g.interp, g.align_corners = float(lay.S), lay.gridtype_id, lay.interp_id, int(lay.align_corners)
+        _fill_grid(getattr(d, name), gp, _cuda_f32(gp.embeddings.detach()), keep)
     ws = [_cuda_f32(w.weight.detach()) for w in list(model.ambient_net.net) + list(model.sigma_net.net) + list(model.color_net.net)]
     keep += ws
     for i in range(3):
@@ -309,15 +332,9 @@ class _field(Function):
         model = ctx.model
         cond_shape, code_shape = ctx.shapes
         M, dev = x.shape[0], x.device
-        g_sigma = torch.zeros(M, device=dev) if g_sigma is None else _cuda_f32(g_sigma)
-        g_color = torch.zeros(M, 3, device=dev) if g_color is None else _cuda_f32(g_color)
-        g_amb = torch.zeros(M, model.ambient_coord_dim, device=dev) if g_amb is None else _cuda_f32(g_amb)
-        alloc = torch.zeros if M == 0 else torch.empty
-        grad_w = [alloc(p.shape, dtype=torch.float32, device=dev) for p in params[:8]]
-        g_pos = torch.zeros(params[8].shape, dtype=torch.float32, device=dev)
-        g_tab = torch.zeros(params[9].shape, dtype=torch.float32, device=dev)
-        g_cond = alloc(c.shape, dtype=torch.float32, device=dev)
-        g_code = alloc(cd.shape, dtype=torch.float32, device=dev) if code_shape is not None else None
+        (g_sigma, g_color, g_amb), grads, g_code = _backward_buffers(M, dev, (g_sigma, g_color, g_amb), ((M,), (M, 3), (M, model.ambient_coord_dim)),
+                                                                     [*params, c], None if code_shape is None else cd, tables=(8, 9))
+        grad_w, g_pos, g_tab, g_cond = grads[:8], grads[8], grads[9], grads[10]
         keep = []
         d = _field_desc(model, cd if code_shape is not None else None, keep)
         ws = _field_workspace(model, M)
@@ -327,7 +344,7 @@ class _field(Function):
                                                         g_color.data_ptr(), g_amb.data_ptr(), ctypes.byref(ptrs), g_cond.data_ptr(),
                                                         None if g_code is None else g_code.data_ptr(), g_pos.data_ptr(), g_tab.data_ptr(),
                                                         ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_field_backward")
-        grads = [g.to(p.dtype) for g, p in zip(grad_w + [g_pos, g_tab], params)]
+        grads = [g.to(p.dtype) for g, p in zip(grads, params)]
         return (None, None, None, g_cond.view(cond_shape), None if g_code is None else g_code.view(code_shape), *grads)
 
 
@@ -336,29 +353,14 @@ field = _field.apply
 
 # ------------------------------------------------------------------------------------------------ the torso field
 def _torso_field_workspace(model, M):
-    need = _capi.lib().gfpp_torso_field_workspace_bytes(M)
-    if need == 0:
-        raise _capi.GfppError(f"the torso training field does not support {M} points per call")
-    dev = model.density_bitfield.device
-    ws = model.__dict__.get("_torso_field_ws")
-    if ws is None or ws.numel() < need or ws.device != dev:
-        ws = model.__dict__["_torso_field_ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
-    return ws
+    return _workspace(model, "_torso_field_ws", _capi.lib().gfpp_torso_field_workspace_bytes, M, "the torso training field")
 
 
 def _torso_field_desc(model, keep):
     """The gfpp_model_desc fields section (H) reads -- torso grid, the six torso weights, torso_code_dim, torso_shrink -- with no
     device-to-host copy."""
     d = _capi.ModelDesc()
-    gp = model.torso_embedder
-    lay = gp.layout
-    emb = _cuda_f32(gp.embeddings.detach())
-    off = _host_offsets(gp)
-    keep += [emb, off]
-    g = d.torso_grid
-    g.embeddings, g.offsets_host = emb.data_ptr(), off.ctypes.data
-    g.input_dim, g.num_levels, g.base_resolution = lay.input_dim, lay.num_levels, lay.base_resolution
-    g.log2_per_level_scale, g.gridtype, g.interp, g.align_corners = float(lay.S), lay.gridtype_id, lay.interp_id, int(lay.align_corners)
+    _fill_grid(d.torso_grid, model.torso_embedder, _cuda_f32(model.torso_embedder.embeddings.detach()), keep)
     ws = [_cuda_f32(w.weight.detach()) for w in list(model.torso_deform_net.net) + list(model.torso_canonicial_net.net)]
     keep += ws
     for i in range(3):
@@ -406,25 +408,20 @@ class _torso_field(Function):
         xy, p6, cd, *params = ctx.saved_tensors
         model, code_shape = ctx.model, ctx.code_shape
         M, dev = xy.shape[0], xy.device
-        g_alpha = torch.zeros(M, device=dev) if g_alpha is None else _cuda_f32(g_alpha).reshape(-1)
-        g_color = torch.zeros(M, 3, device=dev) if g_color is None else _cuda_f32(g_color)
-        g_dx = torch.zeros(M, 2, device=dev) if g_dx is None else _cuda_f32(g_dx)
-        alloc = torch.zeros if M == 0 else torch.empty
-        grad_w = [alloc(p.shape, dtype=torch.float32, device=dev) for p in params[:6]]
-        g_tab = torch.zeros(params[6].shape, dtype=torch.float32, device=dev)
-        g_code = alloc(cd.shape, dtype=torch.float32, device=dev) if code_shape is not None else None
+        (g_alpha, g_color, g_dx), grads, g_code = _backward_buffers(M, dev, (g_alpha, g_color, g_dx), ((M,), (M, 3), (M, 2)), params,
+                                                                    None if code_shape is None else cd, tables=(6,))
         keep = []
         d = _torso_field_desc(model, keep)
         ws = _torso_field_workspace(model, M)
-        p_def = (ctypes.c_void_p * 3)(*[g.data_ptr() for g in grad_w[:3]])
-        p_can = (ctypes.c_void_p * 3)(*[g.data_ptr() for g in grad_w[3:]])
+        p_def = (ctypes.c_void_p * 3)(*[g.data_ptr() for g in grads[:3]])
+        p_can = (ctypes.c_void_p * 3)(*[g.data_ptr() for g in grads[3:6]])
         with torch.cuda.device(dev):
             _capi.check(_capi.lib().gfpp_torso_field_backward(ctypes.byref(d), xy.data_ptr(), M, p6.data_ptr(),
                                                               None if code_shape is None else cd.data_ptr(), g_alpha.data_ptr(),
                                                               g_color.data_ptr(), g_dx.data_ptr(), ctypes.byref(p_def), ctypes.byref(p_can),
-                                                              None if g_code is None else g_code.data_ptr(), g_tab.data_ptr(), ws.data_ptr(),
+                                                              None if g_code is None else g_code.data_ptr(), grads[6].data_ptr(), ws.data_ptr(),
                                                               ws.numel(), _capi.stream_ptr(dev)), "gfpp_torso_field_backward")
-        grads = [g.to(p.dtype) for g, p in zip(grad_w + [g_tab], params)]
+        grads = [g.to(p.dtype) for g, p in zip(grads, params)]
         return (None, None, None, None if g_code is None else g_code.view(code_shape), *grads)
 
 
@@ -433,14 +430,7 @@ torso_field = _torso_field.apply
 
 # ------------------------------------------------------------------------------------------------ the torso-SR field
 def _torso_sr_field_workspace(model, M):
-    need = _capi.lib().gfpp_torso_sr_field_workspace_bytes(M)
-    if need == 0:
-        raise _capi.GfppError(f"the torso-SR training field does not support {M} points per call")
-    dev = model.density_bitfield.device
-    ws = model.__dict__.get("_torso_sr_field_ws")
-    if ws is None or ws.numel() < need or ws.device != dev:
-        ws = model.__dict__["_torso_sr_field_ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
-    return ws
+    return _workspace(model, "_torso_sr_field_ws", _capi.lib().gfpp_torso_sr_field_workspace_bytes, M, "the torso-SR training field")
 
 
 def torso_sr_params(model):
@@ -458,15 +448,9 @@ def _torso_sr_field_desc(model, params, keep):
     """The gfpp_torso_sr_desc fields section (I) reads -- torso grid, the six torso weights, torso_code_dim, head_aware and the
     encoder, torso_shrink -- from `params` (torso_sr_params order), with no device-to-host copy."""
     d = _capi.TorsoSrDesc()
-    gp = model.torso_embedder
-    lay = gp.layout
     ws = [_cuda_f32(p.detach()) for p in params]
-    off = _host_offsets(gp)
-    keep += ws + [off]
-    g = d.torso_grid
-    g.embeddings, g.offsets_host = ws[6].data_ptr(), off.ctypes.data
-    g.input_dim, g.num_levels, g.base_resolution = lay.input_dim, lay.num_levels, lay.base_resolution
-    g.log2_per_level_scale, g.gridtype, g.interp, g.align_corners = float(lay.S), lay.gridtype_id, lay.interp_id, int(lay.align_corners)
+    keep += ws
+    _fill_grid(d.torso_grid, model.torso_embedder, ws[6], keep)
     for i in range(3):
         d.torso_deform_w[i], d.torso_canon_w[i] = ws[i].data_ptr(), ws[3 + i].data_ptr()
     d.torso_code_dim = model.torso_individual_embedding_dim
@@ -529,13 +513,8 @@ class _torso_sr_field(Function):
         xy, lm, cd, img, ws_, *params = ctx.saved_tensors
         model, code_shape = ctx.model, ctx.code_shape
         M, dev = xy.shape[0], xy.device
-        g_alpha = torch.zeros(M, device=dev) if g_alpha is None else _cuda_f32(g_alpha).reshape(-1)
-        g_color = torch.zeros(M, 3, device=dev) if g_color is None else _cuda_f32(g_color)
-        g_dx = torch.zeros(M, 2, device=dev) if g_dx is None else _cuda_f32(g_dx)
-        alloc = torch.zeros if M == 0 else torch.empty
-        grads = [alloc(p.shape, dtype=torch.float32, device=dev) for p in params]
-        grads[6] = torch.zeros(params[6].shape, dtype=torch.float32, device=dev)      # the table gradient is accumulated into
-        g_code = alloc(cd.shape, dtype=torch.float32, device=dev) if code_shape is not None else None
+        (g_alpha, g_color, g_dx), grads, g_code = _backward_buffers(M, dev, (g_alpha, g_color, g_dx), ((M,), (M, 3), (M, 2)), params,
+                                                                    None if code_shape is None else cd, tables=(6,))
         keep = []
         d = _torso_sr_field_desc(model, params, keep)
         ws = _torso_sr_field_workspace(model, M)

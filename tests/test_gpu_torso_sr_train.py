@@ -1,5 +1,5 @@
 """The trainable torso-SR field on the GPU (gfpp.h section I: RADNeRFTorsowithSR.forward_torso in training mode, fused fp32 forward
-and backward, csrc/torso_sr_train_kernel.cu):
+and backward, csrc/torso_train_kernel.cu):
   * the training forward is bit-identical to the render epilogue's (gfpp_torso_sr_composite) alpha and deform at its masked pixels;
   * gradients against the float64 autograd oracle (oracle/torso_sr_train.py) for several M and configurations (head-aware with and
     without an image, no head-aware encoder and no code), no further from float64 than the fp32 arithmetic of the reference;
