@@ -247,10 +247,12 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         ph_last = now_;                                                                    \
     }
 
-        // refill dead lanes of `sl` from the warp's feed (all lanes of the warp, converged)
+        // refill dead lanes of `sl` from the warp's feed (all lanes of the warp, converged).  Pass 1 fills every dead lane within
+        // two tries (each hit record is a live ray); in pass 2 a survivor already at its cap is finalised on adoption, so a warp
+        // may go through many rounds before it holds a live ray, and every round given up is an empty batch
         auto refill = [&]() {
 #pragma unroll 1
-            for (int tries = 0; tries < 4; ++tries) {
+            for (int tries = 0; tries < 64; ++tries) {
                 const unsigned need = __ballot_sync(0xffffffffu, !sl.active);
                 if (!need) break;
                 if (wf.next >= wf.end) {
@@ -344,10 +346,11 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
 
         for (;;) {
             const bool valid = cu.valid;
-            {   // batch accounting: this warp's "live rows" flag, then the split-phase batch barrier
+            {   // batch accounting: this warp's "live rows" flag, then the split-phase batch barrier.  A warp whose feed is not dry
+                // keeps the CTA going without live rows: the rays its next refill adopts must still get a batch
                 const unsigned any = __ballot_sync(0xffffffffu, valid);
                 if (lane == 0) {
-                    ms.flag[bpar][warp] = any ? 1 : 0;
+                    ms.flag[bpar][warp] = (any || !wf.dry) ? 1 : 0;
                     mbar_arrive(&ms.batch_bar);
                 }
             }
