@@ -34,6 +34,7 @@ cudaError_t launch_pack_octs(const GridMeta &, const float *, void *, uint32_t, 
 cudaError_t launch_pack_octs_i16(const GridMeta &, const float *, void *, uint32_t, uint32_t *, float *, cudaStream_t);
 // tc_pack.cu
 cudaError_t launch_pack_tc_tile(const float *, int, int, int, int, int, int, int, int, unsigned char *, unsigned char *, cudaStream_t);
+cudaError_t launch_pack_fold_tile(const float *, int, int, const float *, unsigned char *, int, cudaStream_t);
 cudaError_t launch_tc_selftest(const float *, int, const unsigned char *, const unsigned char *, int, int, int, int, float *, cudaStream_t);
 // train_kernels.cu
 size_t march_train_scratch_bytes(uint32_t N);
@@ -498,18 +499,19 @@ int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes,
         // v2 weight images: streamed tiles in the kernel's schedule order (head_kernel.cuh), then the resident block
         unsigned char *vs = (unsigned char *)(base + L.v2_stream), *vr = (unsigned char *)(base + L.v2_res);
         struct T { const float *w; int ld, row0, col0, kc; bool split; };
-        const T tiles[11] = {{d->ambient_w[0], 96, 0, 0, 64, true},  {d->ambient_w[0], 96, 0, 64, 32, true},
-                             {d->ambient_w[1], 128, 0, 0, 64, true}, {d->ambient_w[1], 128, 0, 64, 64, true},
-                             {d->sigma_w[0], 64, 0, 0, 64, false},   {d->sigma_w[1], 128, 0, 0, 64, false},  {d->sigma_w[1], 128, 0, 64, 64, false},
-                             {d->sigma_w[2], 128, 1, 0, 64, false},  {d->sigma_w[2], 128, 1, 64, 64, false},
-                             {d->color_w[0], col0_in, 0, 16, 64, false}, {d->color_w[0], col0_in, 0, 80, 64, false}};
+        const T tiles[7] = {{d->ambient_w[0], 96, 0, 0, 64, true},  {d->ambient_w[0], 96, 0, 64, 32, true},
+                            {d->ambient_w[1], 128, 0, 0, 64, true}, {d->ambient_w[1], 128, 0, 64, 64, true},
+                            {d->sigma_w[0], 64, 0, 0, 64, false},   {d->sigma_w[1], 128, 0, 0, 64, false},  {d->sigma_w[1], 128, 0, 64, 64, false}};
         int ti = 0;
-        for (int c = 0; c < 11; ++c) {
+        for (int c = 0; c < 7; ++c) {
             const bool sp = robust && tiles[c].split;
             unsigned char *hi = vs + (size_t)ti * V2_TILE_BYTES, *lo = sp ? hi + V2_TILE_BYTES : nullptr;
             CK(launch_pack_tc_tile(tiles[c].w, tiles[c].ld, tiles[c].row0, tiles[c].col0, 128, tiles[c].kc, 0, 0, 0, hi, lo, st));
             ti += sp ? 2 : 1;
         }
+        // the last two: sigma L2's geo rows folded into color L0's geo columns (one fp16 image in both modes, DESIGN §6)
+        CK(launch_pack_fold_tile(d->color_w[0], col0_in, 16, d->sigma_w[2], vs + (size_t)ti * V2_TILE_BYTES, V2_TILE_BYTES, st));
+        static_assert(V2_NTILE_X1 == 7 + 2 && V2_NTILE_ROBUST == 7 + 4 + 2, "v2 tile table");
         for (int kt = 0; kt < 2; ++kt) {
             CK(launch_pack_tc_tile(d->ambient_w[2], 128, 0, kt * 64, amb_dim, 64, 0, 0, 0, vr + V2_RES_AMBN_HI + kt * 2048,
                                    robust ? vr + V2_RES_AMBN_LO + kt * 2048 : nullptr, st));

@@ -80,8 +80,9 @@ size_t head_tc_smem_bytes(bool split);
 // ---- v2 (head_v2_kernel.cu): one CTA per SM, 2-3 row-owner slots of 128 samples sharing one weight stream ----
 constexpr int V2_TILE_BYTES = 16384;            // one streamed weight tile: 128 rows x 64 k x 2 B (SW128)
 // Streamed tiles of one super-batch, in order.  fp16: amb0 a (k 0-63: position features + conditioning 0-31), b (k 64-95: conditioning
-// 32-63) | amb1 a,b | sig0 | sig1 a,b | sig2 a,b (geo rows) | col0 a,b (geo columns); robust: every ambient tile is followed by its lo image.
-constexpr int V2_NTILE_X1 = 11, V2_NTILE_ROBUST = 15;
+// 32-63) | amb1 a,b | sig0 | sig1 a,b | fold a,b (W_fold = color L0 geo columns x sigma L2 geo rows, K = 128 over sigma L1's output);
+// robust: every ambient tile is followed by its lo image.  Sigma L2 has no streamed tile: its sigma row is resident (V2_RES_SIGROW).
+constexpr int V2_NTILE_X1 = 9, V2_NTILE_ROBUST = 13;
 // Resident small tiles (loaded once per CTA): 16-row N tiles of the narrow layers, 2 KB per 64-wide K tile, and the K16 SH tile
 constexpr int V2_RES_AMBN_HI = 0, V2_RES_AMBN_LO = 4096, V2_RES_SIGROW = 8192, V2_RES_COLSH = 12288, V2_RES_COLN = 16384, V2_RES_BYTES = 20480;
 struct HeadV2Args {

@@ -70,8 +70,9 @@ struct Misc {
     volatile int flag[2][16];            // per batch parity, per owner warp: "I have live rows"
 };
 
-// the sigma logits of a slot's rows, from sigma L2 to the row owners (TM floats per slot): the robust mode keeps them at the
-// head of the slot's residual tile l (idle from ambient out to the next batch's operand rows), fp16 behind Misc
+// the sigma logits of a slot's rows, from the sigma row's MMA (issued with color L0) to the row owners (TM floats per slot): the
+// robust mode keeps them at the head of the slot's residual tile l (idle from ambient out to the next batch's operand rows), fp16
+// behind Misc
 template <bool ROBUST>
 constexpr size_t slogit_bytes() { return ROBUST ? 0 : (size_t)Cfg<ROBUST>::NSLOT * TM * sizeof(float); }
 template <bool ROBUST>
@@ -492,9 +493,15 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                 wgmma_sw<128, false>(d, h_u + o, w0, 4, 0u);
                 wgmma_sw<128, false>(d, h_u + V2_TILE_BYTES + o, w1, 4, 1u);
             }, [&](const float (&d)[64], int hf) { epilogue_half<true, false, false>(d, h, h, hf, lane, wwarp, nullptr); });
-            ARRIVE_A();   // -> sigma L2
+            ARRIVE_A();   // -> color L0 + sigma row
             PH(11)  // MMA + epilogue: sigma L1
-            {   // sigma L2: 128 geo rows (streamed) + the sigma row (resident N = 16 tile)
+
+            // ---------------- sigma L2 + color net (16 SH + 128 geo [+ folded individual code]) -> 128 -> 3 (radnerf.py:127-141) ----------------
+            // The 128 geo rows of sigma L2 have no activation and only feed color L0, which is linear in them: the pack folds them into
+            // color L0's geo columns (W_fold = W_c0[:, 16:144] * W_s2[1:129, :], k_pack_fold_tile), so color L0 reads sigma L1's output
+            // h_s1 directly.  One commit group per M-half: W_fold over K = 128 (streamed), SH K = 16 (resident no-swizzle tile against
+            // the slot's SH operand tile), and the sigma row of sigma L2 (resident N = 16 tile) on the same h_s1 operand rows.
+            {
                 const uint32_t w0 = tile(0), w1 = tile(1);
 #pragma unroll 1
                 for (int hf = 0; hf < 2; ++hf) {
@@ -503,6 +510,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                     wg_fence();
                     wgmma_sw<128, false>(d, h_u + o, w0, 4, 0u);
                     wgmma_sw<128, false>(d, h_u + V2_TILE_BYTES + o, w1, 4, 1u);
+                    wgmma<128, false>(d, desc_k16(sh_u + (o ? K16_HALF : 0u)), desc_k16(res_u + V2_RES_COLSH), 1u);
                     mma16(d16, h_u + o, res_u + V2_RES_SIGROW, 0u);
                     wg_commit();
                     wg_wait<0>();
@@ -512,22 +520,12 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                         slogit[64 * hf + frag_row(0, lane, wwarp)] = d16[0];
                         slogit[64 * hf + frag_row(2, lane, wwarp)] = d16[2];
                     }
-                    epilogue_half<false, false, false>(d, h, h, hf, lane, wwarp, nullptr);   // geo features (no activation) -> color-net input
+                    epilogue_half<true, true, false>(d, h, h, hf, lane, wwarp, ms.cbias);
                 }
                 release(2);
             }
-            ARRIVE_A();   // -> color L0 (geo K = 128 + SH K = 16)
-            PH(12)  // MMA + epilogue: sigma L2 (sigma + geo)
-
-            // ---------------- color net (16 SH + 128 geo [+ folded individual code]) -> 128 -> 3 (radnerf.py:137-141) ----------------
-            // color L0: geo K = 128 (streamed) + SH K = 16 (resident no-swizzle tile against the slot's SH operand tile)
-            layer128(2, [&](float (&d)[64], uint32_t o, uint32_t w0, uint32_t w1) {
-                wgmma_sw<128, false>(d, h_u + o, w0, 4, 0u);
-                wgmma_sw<128, false>(d, h_u + V2_TILE_BYTES + o, w1, 4, 1u);
-                wgmma<128, false>(d, desc_k16(sh_u + (o ? K16_HALF : 0u)), desc_k16(res_u + V2_RES_COLSH), 1u);
-            }, [&](const float (&d)[64], int hf) { epilogue_half<true, true, false>(d, h, h, hf, lane, wwarp, ms.cbias); });
             ARRIVE_A();   // -> color out (N = 16)
-            PH(13)  // MMA + epilogue: color L0
+            PH(13)  // MMA + epilogue: sigma row + color L0
 #pragma unroll
             for (int hf = 0; hf < 2; ++hf) {   // color out: N = 16 group -> the hand-over buffer
                 const uint32_t o = (uint32_t)hf * SW128_HALF;

@@ -34,6 +34,26 @@ cudaError_t launch_pack_tc_tile(const float *W, int ld, int row0, int col0, int 
     return cudaGetLastError();
 }
 
+// The geo part of sigma L2 folded into color L0 (k_head_v2): W_fold[n][k] = sum_j Wc[n][c0 + j] * Ws[1 + j][k], n, j, k < 128
+// (Wc: color L0 [.][ldc], its geo columns from c0; Ws: sigma L2 [129][128], row 0 = the sigma row).  Accumulated in double in
+// ascending j, rounded to fp32 and then to fp16, and written as the two K = 64 SW128 tiles k_pack_tc_tile would make of it
+// (tile k / 64 at tiles + (k / 64) * tile_bytes).
+__global__ void k_pack_fold_tile(const float *__restrict__ Wc, int ldc, int c0, const float *__restrict__ Ws,
+                                 unsigned char *__restrict__ tiles, int tile_bytes) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 128 * 128) return;
+    const int n = i >> 7, k = i & 127;
+    double acc = 0.0;
+    for (int j = 0; j < 128; ++j) acc += (double)Wc[(size_t)n * ldc + c0 + j] * (double)Ws[(size_t)(1 + j) * 128 + k];
+    const uint32_t off = (uint32_t)(k >> 6) * (uint32_t)tile_bytes + sw128_off(n, (k & 63) >> 3) + (uint32_t)(k & 7) * 2u;
+    *reinterpret_cast<__half *>(tiles + off) = __float2half_rn((float)acc);
+}
+
+cudaError_t launch_pack_fold_tile(const float *Wc, int ldc, int c0, const float *Ws, unsigned char *tiles, int tile_bytes, cudaStream_t st) {
+    k_pack_fold_tile<<<128 * 128 / 256, 256, 0, st>>>(Wc, ldc, c0, Ws, tiles, tile_bytes);
+    return cudaGetLastError();
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Self-test: out[128][N] = A[128][K] * W[N][K]^T through exactly the tile layouts, descriptors, wgmma issue and accumulator
 // fragment layout the fused kernels use (warpgroup g computes rows 64g..64g+63).  K = 64*nt64 (+16 when k16_tail); the weight
