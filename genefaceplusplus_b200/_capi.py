@@ -93,7 +93,7 @@ EXPORTS = [
     "gfpp_composite_rays", "gfpp_grid_encode_forward", "gfpp_sh_encode_forward", "gfpp_freq_encode_forward",
     "gfpp_model_packed_bytes", "gfpp_model_pack", "gfpp_render_workspace_bytes", "gfpp_render_frames",
     "gfpp_last_launch_count", "gfpp_profile_enable", "gfpp_profile_read", "gfpp_profile_phases", "gfpp_tc_selftest", "gfpp_debug_generate_rays",
-    "gfpp_sr_packed_bytes", "gfpp_sr_pack", "gfpp_sr_workspace_bytes", "gfpp_sr_forward",
+    "gfpp_sr_packed_bytes", "gfpp_sr_pack", "gfpp_sr_workspace_bytes", "gfpp_sr_forward", "gfpp_sr_forward_video",
     "gfpp_torso_sr_packed_bytes", "gfpp_torso_sr_pack", "gfpp_torso_sr_workspace_bytes", "gfpp_torso_sr_composite",
     "gfpp_march_rays_train_scratch_bytes", "gfpp_march_rays_train", "gfpp_march_rays_train_backward", "gfpp_composite_rays_train_forward",
     "gfpp_composite_rays_train_backward", "gfpp_grid_encode_forward_dydx", "gfpp_grid_encode_backward", "gfpp_grad_total_variation",
@@ -142,6 +142,8 @@ def lib():
         L.gfpp_sr_workspace_bytes.argtypes = [c_u32, c_u32]
         L.gfpp_sr_forward.argtypes = [ctypes.POINTER(SrModel), c_u32, c_u32, c_void_p, ctypes.POINTER(c_void_p * 4), c_u32, c_void_p,
                                       c_int, c_void_p, c_size_t, c_void_p]
+        L.gfpp_sr_forward_video.argtypes = [ctypes.POINTER(SrModel), c_u32, c_u32, c_void_p, ctypes.POINTER(c_void_p * 4), c_u32,
+                                            c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
         L.gfpp_torso_sr_packed_bytes.restype = c_size_t
         L.gfpp_torso_sr_packed_bytes.argtypes = []
         L.gfpp_torso_sr_pack.argtypes = [ctypes.POINTER(TorsoSrDesc), c_void_p, c_size_t, ctypes.POINTER(TorsoSrModel), c_void_p]

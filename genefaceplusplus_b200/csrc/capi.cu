@@ -817,16 +817,21 @@ int gfpp_sr_pack(const gfpp_sr_desc *d, void *packed, size_t packed_bytes, gfpp_
 
 size_t gfpp_sr_workspace_bytes(uint32_t n_frames, uint32_t in_res) { return sr_work_layout(n_frames, in_res).total; }
 
-int gfpp_sr_forward(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in, const float *const noise[4],
-                    uint32_t noise_per_frame, float *out, int clamp01, void *workspace, size_t workspace_bytes, void *stream) {
-    if (!model || !rgb_in || !out || !workspace) return fail(GFPP_ERR_INVALID, "sr_forward: null pointer%s");
+}  // extern "C"
+
+// gfpp_sr_forward (out, clamp01) and gfpp_sr_forward_video (out and/or out_u8, always clamped): `who` names the entry point in errors
+static int sr_forward_impl(const char *who, const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in,
+                           const float *const noise[4], uint32_t noise_per_frame, float *out, uint8_t *out_u8, int clamp01, void *workspace,
+                           size_t workspace_bytes, void *stream) {
+    if (!model || !rgb_in || (!out && !out_u8) || !workspace) return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
+    if (((uintptr_t)out_u8 & 3u) != 0) return fail(GFPP_ERR_INVALID, "%s: out_u8 must be 4-byte aligned", who);
     SrHost m;
     memcpy(&m, model, sizeof(m));
-    if (m.magic != kSrMagic) return fail(GFPP_ERR_INVALID, "sr_forward: model handle not initialised by gfpp_sr_pack%s");
-    if (n_frames == 0 || in_res == 0 || in_res % 128 != 0 || in_res > 1024) return fail(GFPP_ERR_UNSUPPORTED, "sr_forward: in_res must be a multiple of 128 (256 in the reference)%s");
-    if ((uint64_t)n_frames * in_res * in_res * 4 >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "sr_forward: too many frames per call%s");
+    if (m.magic != kSrMagic) return fail(GFPP_ERR_INVALID, "%s: model handle not initialised by gfpp_sr_pack", who);
+    if (n_frames == 0 || in_res == 0 || in_res % 128 != 0 || in_res > 1024) return fail(GFPP_ERR_UNSUPPORTED, "%s: in_res must be a multiple of 128 (256 in the reference)", who);
+    if ((uint64_t)n_frames * in_res * in_res * 4 >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: too many frames per call", who);
     const SrWork W = sr_work_layout(n_frames, in_res);
-    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "sr_forward: workspace too small%s");
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "%s: workspace too small", who);
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     const int F = (int)n_frames, R = (int)in_res;
@@ -851,8 +856,24 @@ int gfpp_sr_forward(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_r
     a.in = (const __half *)(ws + W.x1a); a.F = F; a.H = 2 * R; a.W = 2 * R; a.wt = m.tiles[2]; a.bias = m.bias[3];
     a.noise = noise ? noise[3] : nullptr; a.noise_fstride = hi;
     a.rgb_w = m.rgb_w[1]; a.rgb_b = m.rgb_b[1]; a.img_in = (const float *)(ws + W.img0); a.img_out = out; a.clamp01 = clamp01;
+    a.img_u8 = out_u8;
     CK(launch_sr_conv(2, a, st));
     return GFPP_OK;
+}
+
+extern "C" {
+
+int gfpp_sr_forward(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in, const float *const noise[4],
+                    uint32_t noise_per_frame, float *out, int clamp01, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!out) return fail(GFPP_ERR_INVALID, "sr_forward: null pointer%s");
+    return sr_forward_impl("sr_forward", model, n_frames, in_res, rgb_in, noise, noise_per_frame, out, nullptr, clamp01, workspace,
+                           workspace_bytes, stream);
+}
+
+int gfpp_sr_forward_video(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in, const float *const noise[4],
+                          uint32_t noise_per_frame, float *out, uint8_t *out_u8, void *workspace, size_t workspace_bytes, void *stream) {
+    return sr_forward_impl("sr_forward_video", model, n_frames, in_res, rgb_in, noise, noise_per_frame, out, out_u8, 1, workspace,
+                           workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -14,6 +14,8 @@
 //                                                         intermediate, no separate filter pass
 //   k_sr_conv<2>   block1.conv1   64 -> 64, 3x3 at 512^2  implicit GEMM; epilogue: activation, fused toRGB, + the 2x FIR
 //                                                         up-sampled img0 (closed form: 4 taps), optional clamp -> [F,3,512,512]
+//                                                         and/or the uint8 video frames [F,512,512,3] (interleaved, as imageio
+//                                                         takes them), each store optional
 //
 // Implicit GEMM: a tile is 128 consecutive pixels of one image row (the 128 rows of the MMA); K runs over the 9 taps x
 // C_in in chunks of 64 channels.  For every chunk the CTA's threads copy the shifted 128 x 64 fp16 window of the NHWC
@@ -228,14 +230,27 @@ __global__ void __launch_bounds__(NT, LAYER == 1 ? 1 : 2) k_sr_conv(const __grid
                         a.img_out[pix * 3 + o] = __ldg(a.img_in + pix * 3 + o) + r;
                     }
                 } else {
-                    float sk[3];
+                    float sk[3], rc[3];
                     upsampled_skip(a.img_in + (size_t)f * (a.H / 2) * (a.W / 2) * 3, a.H / 2, a.W / 2, y, x, sk);
 #pragma unroll
                     for (int o = 0; o < 3; ++o) {
                         float r = s.part[o * TM + tid] + __ldg(a.rgb_b + o);
                         r = sk[o] + fminf(fmaxf(r, -256.f), 256.f);
-                        if (a.clamp01) r = fminf(fmaxf(r, 0.f), 1.f);
-                        a.img_out[(((size_t)f * 3 + o) * a.H + y) * a.W + x] = r;
+                        rc[o] = fminf(fmaxf(r, 0.f), 1.f);
+                        if (a.img_out) a.img_out[(((size_t)f * 3 + o) * a.H + y) * a.W + x] = a.clamp01 ? rc[o] : r;
+                    }
+                    if (a.img_u8) {
+                        // video frame (rgb * 255).int() of the clamped colour, the rule of k_epilogue and dist.to_uint8.  A pixel is 3
+                        // bytes: the tile's 128 pixels are staged in `part` (once this warpgroup has read it) and leave as 96 words
+                        wg_sync(1);
+                        unsigned char *stage = reinterpret_cast<unsigned char *>(s.part);
+#pragma unroll
+                        for (int o = 0; o < 3; ++o) stage[3 * tid + o] = (unsigned char)(int)__fmul_rn(rc[o], 255.0f);
+                        wg_sync(1);
+                        if (tid < 3 * TM / 4) {
+                            uint32_t *dst = reinterpret_cast<uint32_t *>(a.img_u8 + (((size_t)f * a.H + y) * a.W + x0) * 3);
+                            dst[tid] = reinterpret_cast<const uint32_t *>(stage)[tid];
+                        }
                     }
                 }
             }

@@ -21,8 +21,9 @@ struct SrConvArgs {
     const float *rgb_w;        // [3][COUT] effective toRGB weights (layers 0 and 2)
     const float *rgb_b;        // [3]
     const float *img_in;       // LAYER 0: the NeRF image [F,H,W,3]; LAYER 2: img0 [F,H/2,W/2,3]
-    float *img_out;            // LAYER 0: img0 [F,H,W,3]; LAYER 2: the final image [F,3,H,W] (planar)
+    float *img_out;            // LAYER 0: img0 [F,H,W,3]; LAYER 2: the final image [F,3,H,W] (planar), or nullptr with img_u8
     int clamp01;               // LAYER 2: clamp the final image to [0,1] (what every caller of the SR head does next)
+    unsigned char *img_u8;     // LAYER 2: optional video frames [F,H,W,3] (interleaved) = (int)(clamp01(rgb) * 255); else nullptr
 };
 
 // block0.conv0: 3 -> 128, 3x3, fp32 on CUDA cores (K = 27 is no tensor-core shape), fp16 NHWC out

@@ -10,7 +10,14 @@ change in forward_secc2video is
     out_imgs = video_uint8(pred_rgbs).cpu().numpy()                                                           # what imageio gets (:505)
 
 For drivers that can hand over c2w poses instead of materialised rays (1.5 GB for 250 frames), `model.render_clip` generates
-the rays in-kernel; this shim is for the unmodified batch layout.  Non-SR head / head+torso models (SR models render per frame).
+the rays in-kernel; this shim is for the unmodified batch layout.  All four model classes: for the `with_sr` checkpoints
+(RADNeRFwithSR / RADNeRFTorsowithSR) the frames are the 512x512 `sr_rgb_map` the driver takes (:464-465, 480-481), and the
+change is
+
+    out_imgs = render_driver_batch(self.secc2video_model, batch, T_thresh=inp['raymarching_end_threshold'], as_uint8=True).cpu().numpy()
+
+For the `low_memory_usage` mode (:449-470), `iter_video_frames` yields the frames as host uint8 chunks for `writer.append_data`,
+with only two chunks of frames alive at any time.
 """
 import torch
 
@@ -36,27 +43,135 @@ def cond_feat_from_windows(model, cond_wins, eye_area_percent=None):
     return feat
 
 
-@torch.no_grad()
-def render_driver_batch(model, batch, T_thresh=1e-2, frames_per_call=32, dt_gamma=None, max_steps=None):
-    """-> [T,3,H,W] fp32 in [0,1] on the model's device (H = W = sqrt(N))."""
+SR_FRAMES_PER_CALL = 8   # frames per SR-head call: its workspace is 68 MB per frame (as RADNeRF*withSR.render_clip)
+
+
+def _is_sr(model):
+    return hasattr(model, "sr_net")
+
+
+def _frame_hw(model, batch):
+    """(H, W) of the frames the driver writes: the NeRF image (H = W = sqrt(N)), or the SR head's 2x output."""
+    if _is_sr(model):
+        R = 2 * model.sr_input_resolution
+        return R, R
+    N = batch["rays_o"][0].numel() // 3
+    H = int(round(N ** 0.5))
+    return H, N // H
+
+
+def _render_kw(model, T_thresh, dt_gamma, max_steps):
     hp = model.hparams
+    return {"dt_gamma": hp["dt_gamma"] if dt_gamma is None else dt_gamma, "max_steps": hp["max_steps"] if max_steps is None else max_steps,
+            "T_thresh": T_thresh}
+
+
+def _render_chunk(model, batch, feat, s, e, kw, out=None, out_u8=None, sr_noise_mode="random"):
+    """Frames [s, e) of the batch in one libgfpp call per stage.  Non-SR models: returns render_frames' result (`rgb_map` [n,N,3];
+    with out_u8 [n,N,3] the uint8 frames go there instead).  SR models: the clamped 512x512 frames go into out [n,3,512,512]
+    and/or out_u8 [n,512,512,3] -- what render()'s `sr_rgb_map` gives frame by frame: the head field with the frame's rays
+    (torso-SR: on a zero background, then the torso field + composite with its `lm68` row over `bg_img`), then the SR head."""
+    N = batch["rays_o"][0].numel() // 3
+    rays_o = torch.stack([batch["rays_o"][i].reshape(N, 3) for i in range(s, e)])
+    rays_d = torch.stack([batch["rays_d"][i].reshape(N, 3) for i in range(s, e)])
+    if not _is_sr(model):
+        pose6 = torch.stack([batch["poses"][i].reshape(6) for i in range(s, e)]) if model.has_torso else None
+        return model.render_frames(feat[s:e], rays_o=rays_o, rays_d=rays_d, pose6=pose6,
+                                   bg_coords=batch["bg_coords"] if model.has_torso else None, bg_color=batch.get("bg_img"),
+                                   **kw, want_torso_maps=False, **({} if out_u8 is None else {"u8_out": out_u8}))
+    dev = model.density_bitfield.device
+    with torch.autocast(dev.type, enabled=False):
+        if hasattr(model, "torso_composite_native"):
+            lm68 = torch.as_tensor(batch["lm68"]).reshape(-1, 136)[s:e]
+            hd = model.render_frames(feat[s:e], rays_o=rays_o, rays_d=rays_d, bg_color=torch.zeros(N, 3, device=dev), **kw)
+            img = model.torso_composite_native(hd["rgb_map"], hd["weights_sum"], lm68, batch["bg_coords"], batch.get("bg_img"),
+                                               want_maps=False)["rgb_map"]
+        else:
+            img = model.render_frames(feat[s:e], rays_o=rays_o, rays_d=rays_d, bg_color=batch.get("bg_img"), **kw, want_aux=False)["rgb_map"]
+        model.sr_net.forward_native(img, noise_mode=sr_noise_mode, clamp=True, out=out, u8_out=out_u8, frames_per_call=e - s)
+
+
+@torch.no_grad()
+def render_driver_batch(model, batch, T_thresh=1e-2, frames_per_call=32, dt_gamma=None, max_steps=None, as_uint8=False,
+                        sr_noise_mode="random"):
+    """-> [T,3,H,W] fp32 in [0,1] on the model's device (H = W = sqrt(N); SR models: the 512x512 `sr_rgb_map` frames), or with
+    as_uint8 the video frames uint8 [T,H,W,3] `(rgb*255).int()`, written by the last kernel itself.  SR models take the batch's
+    `lm68` [T,136] (torso-SR) and render at most SR_FRAMES_PER_CALL frames per call; sr_noise_mode as render()'s."""
     T = len(batch["poses"])
     dev = model.density_bitfield.device
     feat = cond_feat_from_windows(model, batch["cond_wins"], batch.get("eye_area_percent"))
-    N = batch["rays_o"][0].numel() // 3
-    H = int(round(N ** 0.5))
-    out = torch.empty(T, N, 3, device=dev, dtype=torch.float32)
+    H, W = _frame_hw(model, batch)
+    kw = _render_kw(model, T_thresh, dt_gamma, max_steps)
+    if _is_sr(model):
+        fpc = min(frames_per_call, SR_FRAMES_PER_CALL)
+        out = torch.empty((T, H, W, 3) if as_uint8 else (T, 3, H, W), device=dev, dtype=torch.uint8 if as_uint8 else torch.float32)
+        for s in range(0, T, fpc):
+            e = min(T, s + fpc)
+            _render_chunk(model, batch, feat, s, e, kw, out=None if as_uint8 else out[s:e], out_u8=out[s:e] if as_uint8 else None,
+                          sr_noise_mode=sr_noise_mode)
+        return out
+    N = H * W
+    out = torch.empty(T, N, 3, device=dev, dtype=torch.uint8 if as_uint8 else torch.float32)
     for s in range(0, T, frames_per_call):
         e = min(T, s + frames_per_call)
-        rays_o = torch.stack([batch["rays_o"][i].reshape(N, 3) for i in range(s, e)])
-        rays_d = torch.stack([batch["rays_d"][i].reshape(N, 3) for i in range(s, e)])
-        pose6 = torch.stack([batch["poses"][i].reshape(6) for i in range(s, e)]) if model.has_torso else None
-        res = model.render_frames(feat[s:e], rays_o=rays_o, rays_d=rays_d, pose6=pose6,
-                                  bg_coords=batch["bg_coords"] if model.has_torso else None, bg_color=batch.get("bg_img"),
-                                  dt_gamma=hp["dt_gamma"] if dt_gamma is None else dt_gamma,
-                                  max_steps=hp["max_steps"] if max_steps is None else max_steps, T_thresh=T_thresh, want_torso_maps=False)
-        out[s:e] = res["rgb_map"]
-    return out.view(T, H, N // H, 3).permute(0, 3, 1, 2)
+        if as_uint8:
+            _render_chunk(model, batch, feat, s, e, kw, out_u8=out[s:e])
+        else:
+            out[s:e] = _render_chunk(model, batch, feat, s, e, kw)["rgb_map"]
+    return out.view(T, H, W, 3) if as_uint8 else out.view(T, H, W, 3).permute(0, 3, 1, 2)
+
+
+def _pinned(shape):
+    return torch.empty(shape, dtype=torch.uint8, pin_memory=True)
+
+
+@torch.no_grad()
+def iter_video_frames(model, batch, frames_per_call=8, T_thresh=1e-2, dt_gamma=None, max_steps=None, sr_noise_mode="random"):
+    """The `low_memory_usage` loop of forward_secc2video (genefacepp_infer.py:449-470) for all four model classes: yields the
+    clip's video frames -- what render_driver_batch(..., as_uint8=True) returns -- as host uint8 [n,H,W,3] chunks in frame order
+    (n <= frames_per_call; SR models: <= SR_FRAMES_PER_CALL), e.g. `for c in iter_video_frames(...): for f in c.numpy(): writer.append_data(f)`.
+
+    Two device and two pinned host buffers: chunk k+1 renders on the current stream while chunk k is copied to the host on a
+    side stream and handed to the caller.  A yielded chunk stays valid until the generator is advanced.  When the generator
+    ends, fails or is closed early, it waits for both streams: no queued work is left behind."""
+    T = len(batch["poses"])
+    dev = model.density_bitfield.device
+    feat = cond_feat_from_windows(model, batch["cond_wins"], batch.get("eye_area_percent"))
+    H, W = _frame_hw(model, batch)
+    kw = _render_kw(model, T_thresh, dt_gamma, max_steps)
+    fpc = min(frames_per_call, SR_FRAMES_PER_CALL) if _is_sr(model) else frames_per_call
+    starts = list(range(0, T, fpc))
+    compute = torch.cuda.current_stream(dev)
+    side = torch.cuda.Stream(dev)
+    rows = min(fpc, T)
+    dbuf = [torch.empty(rows, H, W, 3, device=dev, dtype=torch.uint8) for _ in range(2)]
+    hbuf = [_pinned((rows, H, W, 3)) for _ in range(2)]
+    rendered = [torch.cuda.Event() for _ in range(2)]
+    copied = [torch.cuda.Event() for _ in range(2)]
+
+    def launch(k):
+        """Queue chunk k: render into device buffer k % 2, copy it to host buffer k % 2 on the side stream."""
+        s, b = starts[k], k % 2
+        e = min(T, s + fpc)
+        compute.wait_event(copied[b])           # chunk k-2 has left device buffer b
+        _render_chunk(model, batch, feat, s, e, kw, out_u8=dbuf[b][:e - s], sr_noise_mode=sr_noise_mode)
+        rendered[b].record(compute)
+        side.wait_event(rendered[b])
+        with torch.cuda.stream(side):
+            hbuf[b][:e - s].copy_(dbuf[b][:e - s], non_blocking=True)
+        copied[b].record(side)
+        return e - s
+
+    try:
+        n = launch(0) if starts else 0
+        for k in range(len(starts)):
+            n_next = launch(k + 1) if k + 1 < len(starts) else 0   # host buffer (k+1) % 2 was handed out as chunk k-1: released
+            copied[k % 2].synchronize()
+            yield hbuf[k % 2][:n]
+            n = n_next
+    finally:
+        side.synchronize()
+        compute.synchronize()
 
 
 def video_uint8(pred_rgbs):

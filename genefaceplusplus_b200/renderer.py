@@ -759,25 +759,38 @@ class RADNeRFwithSR(RADNeRF):
         return results
 
     @torch.no_grad()
-    def render_clip(self, poses_c2w, intrinsics, H=256, W=256, *args, sr_noise_mode="random", sr_frames_per_call=8, **kwargs):
+    def render_clip(self, poses_c2w, intrinsics, H=256, W=256, *args, sr_noise_mode="random", sr_frames_per_call=8, as_uint8=False, **kwargs):
         """Clip API: NeRF at 256x256 for all frames (libgfpp), then the SR head over chunks of frames.
-        Returns the clamped 512x512 frames [T,3,512,512]; `intrinsics` are those of the 256x256 camera."""
+        Returns the clamped 512x512 frames [T,3,512,512]; `intrinsics` are those of the 256x256 camera.
+        as_uint8: returns the video frames uint8 [T,512,512,3] (HWC) `(rgb*255).int()` instead, written by the SR head's last
+        kernel chunk by chunk into `out` (optional preallocated buffer of that shape); the NeRF stage still renders fp32, the
+        SR head's input.  Without as_uint8, `out` is the NeRF clip's buffer ([T,256*256,3] fp32), as in RADNeRF.render_clip."""
+        from .dist import to_uint8
         R = self.sr_input_resolution
         if (H, W) != (R, R):
             raise ValueError(f"SR models render the NeRF at {R}x{R} (radnerf_sr.py:205)")
         want_stats = kwargs.get("want_stats", False)
+        u8 = kwargs.pop("out", None) if as_uint8 else None
         res = super().render_clip(poses_c2w, intrinsics, H, W, *args, **kwargs)
         rgb, stats = res if want_stats else (res, None)
         T = rgb.shape[0]
-        out = torch.empty(T, 3, 2 * R, 2 * R, device=rgb.device, dtype=torch.float32)
+        if as_uint8:
+            u8 = u8 if u8 is not None else torch.empty(T, 2 * R, 2 * R, 3, device=rgb.device, dtype=torch.uint8)
+            if u8.shape != (T, 2 * R, 2 * R, 3) or u8.dtype != torch.uint8 or not u8.is_contiguous():
+                raise ValueError(f"out must be a contiguous uint8 [{T},{2 * R},{2 * R},3] tensor")
+        native = rgb.is_cuda and self.sr_net.backend == "native"
+        out = None if as_uint8 and native else torch.empty(T, 3, 2 * R, 2 * R, device=rgb.device, dtype=torch.float32)
         with torch.autocast(rgb.device.type, enabled=False):
-            if rgb.is_cuda and self.sr_net.backend == "native":
+            if native:
                 # libgfpp's SR kernels read the renderer's [T,N,3] frames as they are and clamp in their last epilogue
-                self.sr_net.forward_native(rgb, noise_mode=sr_noise_mode, clamp=True, out=out, frames_per_call=sr_frames_per_call)
+                self.sr_net.forward_native(rgb, noise_mode=sr_noise_mode, clamp=True, out=out, frames_per_call=sr_frames_per_call, u8_out=u8)
             else:
                 for s in range(0, T, sr_frames_per_call):
                     e = min(T, s + sr_frames_per_call)
                     out[s:e] = self.sr_net(rgb[s:e].view(e - s, R, R, 3).permute(0, 3, 1, 2), noise_mode=sr_noise_mode).clamp(0, 1)
+                    if as_uint8:
+                        u8[s:e] = to_uint8(out[s:e].permute(0, 2, 3, 1))
+        out = u8 if as_uint8 else out
         return (out, stats) if want_stats else out
 
 
@@ -1188,11 +1201,15 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
 
     @torch.no_grad()
     def render_clip(self, poses_c2w, intrinsics, H=256, W=256, cond_seq=None, bg_color=None, bg_coords=None, lm68_seq=None,
-                    eye_area_percent=None, dt_gamma=None, max_steps=None, T_thresh=1e-2, sr_noise_mode="random", cond_feat=None, **unused):
+                    eye_area_percent=None, dt_gamma=None, max_steps=None, T_thresh=1e-2, sr_noise_mode="random", cond_feat=None,
+                    as_uint8=False, **unused):
         """Clip API of the torso-SR model -> the clamped 512x512 frames [T,3,512,512].  With the native backends (the default) every
         stage runs in libgfpp chunk by chunk -- head field with rays generated in-kernel, torso-SR field + composite, SR head -- with
         no per-frame host work; with a "torch" backend it falls back to frame-by-frame `render()`.  poses_c2w [T,4,4] (c2w,
-        dataset.poses), cond_seq [T,1,C] (or cond_feat [T,64] precomputed), lm68_seq [T,136], eye_area_percent [T] or None."""
+        dataset.poses), cond_seq [T,1,C] (or cond_feat [T,64] precomputed), lm68_seq [T,136], eye_area_percent [T] or None.
+        as_uint8: returns the video frames uint8 [T,512,512,3] (HWC) `(rgb*255).int()` instead, written by the SR head's last kernel
+        chunk by chunk into `out` (optional preallocated buffer of that shape); no fp32 512x512 frame is written then."""
+        from .dist import to_uint8
         from .scene import cond_window, convert_poses, get_rays
         R = self.sr_input_resolution
         if (H, W) != (R, R):
@@ -1200,8 +1217,15 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
         hp = self.hparams
         T = poses_c2w.shape[0]
         dev = self.density_bitfield.device
-        out = torch.empty(T, 3, 2 * R, 2 * R, device=dev, dtype=torch.float32)
-        if self.torso_backend == "native" and self.sr_net.backend == "native":
+        native = self.torso_backend == "native" and self.sr_net.backend == "native"
+        u8 = None
+        if as_uint8:
+            u8 = unused.get("out")
+            u8 = u8 if u8 is not None else torch.empty(T, 2 * R, 2 * R, 3, device=dev, dtype=torch.uint8)
+            if u8.shape != (T, 2 * R, 2 * R, 3) or u8.dtype != torch.uint8 or not u8.is_contiguous():
+                raise ValueError(f"out must be a contiguous uint8 [{T},{2 * R},{2 * R},3] tensor")
+        out = None if as_uint8 and native else torch.empty(T, 3, 2 * R, 2 * R, device=dev, dtype=torch.float32)
+        if native:
             # everything in libgfpp, chunk by chunk: head field (rays generated in-kernel, background 0 => premultiplied colour),
             # torso-SR field + composite, SR head; no per-frame host work
             fpc = min(8, int(unused.get("frames_per_call", 8)))     # the SR workspace is 68 MB per frame
@@ -1217,8 +1241,9 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
                                             max_steps=hp["max_steps"] if max_steps is None else max_steps, T_thresh=T_thresh)
                     tr = self.torso_composite_native(hd["rgb_map"], hd["weights_sum"], lm68_seq[s:e].reshape(e - s, 136), bg_coords, bg_color,
                                                      want_maps=False)
-                    self.sr_net.forward_native(tr["rgb_map"], noise_mode=sr_noise_mode, clamp=True, out=out[s:e], frames_per_call=fpc)
-            return out
+                    self.sr_net.forward_native(tr["rgb_map"], noise_mode=sr_noise_mode, clamp=True, out=None if out is None else out[s:e],
+                                               frames_per_call=fpc, u8_out=None if u8 is None else u8[s:e])
+            return u8 if as_uint8 else out
         if cond_seq is None:
             raise ValueError("the frame-by-frame host path of the torso-SR clip needs cond_seq (cond_feat is only taken by the all-native path)")
         for t in range(T):
@@ -1230,7 +1255,9 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
                               eye_area_percent=None if eye_area_percent is None else eye_area_percent[t].reshape(1, 1),
                               sr_noise_mode=sr_noise_mode)
             out[t] = res["sr_rgb_map"][0]
-        return out
+            if as_uint8:
+                u8[t] = to_uint8(out[t].permute(1, 2, 0))
+        return u8 if as_uint8 else out
 
 
 # ------------------------------------------------------------------------------------------------ torso model

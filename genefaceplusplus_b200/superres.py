@@ -261,11 +261,14 @@ class Superresolution(nn.Module):
         return st
 
     @torch.no_grad()
-    def forward_native(self, rgb_flat, noise_mode="random", clamp=False, out=None, frames_per_call=8, noise_planes=None):
+    def forward_native(self, rgb_flat, noise_mode="random", clamp=False, out=None, frames_per_call=8, noise_planes=None, u8_out=None):
         """rgb_flat [F, R*R, 3] fp32 CUDA in [0,1] (the layout the renderer writes `rgb_map` in), R = 256 -> [F,3,2R,2R]
         through libgfpp's sm_90a kernels (4 launches per chunk of frames).  `noise_planes`: optional list of four tensors
         ([res,res] shared by all frames or [F,res,res]; None entries = no noise), already multiplied by the layers'
-        noise_strength, instead of drawing them here (tests; callers that want reproducible 'random' noise)."""
+        noise_strength, instead of drawing them here (tests; callers that want reproducible 'random' noise).
+        u8_out: optional contiguous uint8 [F,2R,2R,3] CUDA tensor that receives the video frames `(clamped rgb * 255).int()`
+        straight from the last kernel (gfpp_sr_forward_video).  The result is then clamped (clamp=False is refused); `out` may be
+        omitted, and without it no fp32 frame is written at all.  Returns u8_out then, else the fp32 frames."""
         from . import _capi
         R = self.input_resolution
         if not rgb_flat.is_cuda:
@@ -277,8 +280,13 @@ class Superresolution(nn.Module):
         F_ = x.shape[0]
         st = self._native_state()
         L = _capi.lib()
-        res = out if out is not None else torch.empty(F_, 3, 2 * R, 2 * R, device=dev, dtype=torch.float32)
-        if res.shape != (F_, 3, 2 * R, 2 * R) or res.dtype != torch.float32 or not res.is_contiguous():
+        if u8_out is not None:
+            if not clamp:
+                raise ValueError("the video frames are made from the clamped image: u8_out needs clamp=True")
+            if u8_out.shape != (F_, 2 * R, 2 * R, 3) or u8_out.dtype != torch.uint8 or not u8_out.is_contiguous() or u8_out.device != dev:
+                raise ValueError(f"u8_out must be a contiguous uint8 [{F_},{2 * R},{2 * R},3] tensor on {dev}")
+        res = out if out is not None or u8_out is not None else torch.empty(F_, 3, 2 * R, 2 * R, device=dev, dtype=torch.float32)
+        if res is not None and (res.shape != (F_, 3, 2 * R, 2 * R) or res.dtype != torch.float32 or not res.is_contiguous()):
             raise ValueError(f"out must be a contiguous float32 [{F_},3,{2 * R},{2 * R}] tensor")
         if noise_mode not in ("random", "const", "none"):
             raise ValueError(f"noise_mode must be random / const / none, not {noise_mode!r}")
@@ -309,11 +317,18 @@ class Superresolution(nn.Module):
             if st["ws"] is None or st["ws"].numel() < need or st["ws"].device != dev:
                 st["ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
             with torch.cuda.device(dev):
-                _capi.check(L.gfpp_sr_forward(ctypes.byref(st["model"]), n, R, _capi.ptr(x[s0:s0 + n], torch.float32), ctypes.byref(arr),
-                                              1 if per_frame else 0, _capi.ptr(res[s0:s0 + n], torch.float32),
-                                              1 if clamp else 0, _capi.ptr(st["ws"]), st["ws"].numel(), _capi.stream_ptr(dev)),
-                            "gfpp_sr_forward")
-        return res
+                if u8_out is None:
+                    _capi.check(L.gfpp_sr_forward(ctypes.byref(st["model"]), n, R, _capi.ptr(x[s0:s0 + n], torch.float32), ctypes.byref(arr),
+                                                  1 if per_frame else 0, _capi.ptr(res[s0:s0 + n], torch.float32),
+                                                  1 if clamp else 0, _capi.ptr(st["ws"]), st["ws"].numel(), _capi.stream_ptr(dev)),
+                                "gfpp_sr_forward")
+                else:
+                    _capi.check(L.gfpp_sr_forward_video(ctypes.byref(st["model"]), n, R, _capi.ptr(x[s0:s0 + n], torch.float32),
+                                                        ctypes.byref(arr), 1 if per_frame else 0,
+                                                        None if res is None else _capi.ptr(res[s0:s0 + n], torch.float32),
+                                                        _capi.ptr(u8_out[s0:s0 + n], torch.uint8), _capi.ptr(st["ws"]), st["ws"].numel(),
+                                                        _capi.stream_ptr(dev)), "gfpp_sr_forward_video")
+        return res if u8_out is None else u8_out
 
     def forward(self, rgb, noise_mode="random"):
         if rgb.is_cuda and self.backend == "native" and rgb.shape[-2:] == (self.input_resolution, self.input_resolution):

@@ -270,6 +270,15 @@ GFPP_API size_t gfpp_sr_workspace_bytes(uint32_t n_frames, uint32_t in_res);
 GFPP_API int gfpp_sr_forward(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in,
                              const float *const noise[4], uint32_t noise_per_frame, float *out, int clamp01, void *workspace,
                              size_t workspace_bytes, void *stream);
+/* gfpp_sr_forward for the video writer: the same four launches and workspace, the result always clamped to [0,1], and the
+ * last epilogue writes either or both of
+ *   out     [F, 3, 2*in_res, 2*in_res] fp32 planar (bit-identical to gfpp_sr_forward with clamp01 = 1), NULL: not written;
+ *   out_u8  [F, 2*in_res, 2*in_res, 3] uint8 interleaved (HWC, what video writers take), 4-byte aligned, NULL: not written;
+ *           value (int)(x * 255) of the clamped fp32 x -- the driver's `(rgb * 255).int()` (genefacepp_infer.py:469, 505).
+ * At least one of them must be given.  A uint8-only call writes a quarter of the bytes of the fp32 frames. */
+GFPP_API int gfpp_sr_forward_video(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in,
+                                   const float *const noise[4], uint32_t noise_per_frame, float *out, uint8_t *out_u8,
+                                   void *workspace, size_t workspace_bytes, void *stream);
 
 /* ------------------------------------------------------------------ (C) torso field of the torso-SR checkpoints
  *
