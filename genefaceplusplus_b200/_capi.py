@@ -102,6 +102,7 @@ EXPORTS = [
     "gfpp_torso_grid_workspace_bytes", "gfpp_torso_query_workspace_bytes", "gfpp_torso_query", "gfpp_torso_grid_update", "gfpp_torso_sr_grid_update",
     "gfpp_model_set_torso_threshold", "gfpp_torso_sr_set_threshold",
     "gfpp_field_backward_workspace_bytes", "gfpp_field_forward", "gfpp_field_backward",
+    "gfpp_field_tc_workspace_bytes", "gfpp_field_tc_forward", "gfpp_field_tc_backward",
     "gfpp_torso_field_workspace_bytes", "gfpp_torso_field_forward", "gfpp_torso_field_backward",
     "gfpp_torso_sr_field_workspace_bytes", "gfpp_torso_sr_field_forward", "gfpp_torso_sr_field_backward",
 ]
@@ -185,6 +186,10 @@ def lib():
         L.gfpp_field_backward_workspace_bytes.argtypes = [c_u32]
         L.gfpp_field_forward.argtypes = [ctypes.POINTER(ModelDesc), P, P, c_u32, P, P, P, P, P, c_size_t, P]
         L.gfpp_field_backward.argtypes = [ctypes.POINTER(ModelDesc), P, P, c_u32, P, P, P, P, ctypes.POINTER(P * 8), P, P, P, P, P, c_size_t, P]
+        L.gfpp_field_tc_workspace_bytes.restype = c_size_t
+        L.gfpp_field_tc_workspace_bytes.argtypes = [c_u32]
+        L.gfpp_field_tc_forward.argtypes = L.gfpp_field_forward.argtypes
+        L.gfpp_field_tc_backward.argtypes = L.gfpp_field_backward.argtypes
         L.gfpp_torso_field_workspace_bytes.restype = c_size_t
         L.gfpp_torso_field_workspace_bytes.argtypes = [c_u32]
         L.gfpp_torso_field_forward.argtypes = [ctypes.POINTER(ModelDesc), P, c_u32, P, P, P, P, P, P, c_size_t, P]

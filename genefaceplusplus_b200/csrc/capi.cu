@@ -9,6 +9,7 @@
 #include "../../include/gfpp.h"
 #include "common.cuh"
 #include "field_train_kernel.cuh"
+#include "field_train_tc_kernel.cuh"
 #include "head_kernel.cuh"
 #include "launch.cuh"
 #include "sr_kernel.cuh"
@@ -1768,6 +1769,75 @@ int gfpp_torso_sr_field_backward(const gfpp_torso_sr_desc *desc, const float *xy
         }
     return torso_field_backward<true>("torso_sr_field_backward", a, xy, M, grad_alpha, grad_color, grad_deform, grad_deform_w, grad_canon_w,
                                       grad_code, grad_torso_table, workspace, workspace_bytes, stream);
+}
+
+// ---------------------------------------------------------------- (J) trainable head field on tensor cores
+static uint32_t field_tc_ctas(uint32_t M) {
+    const uint32_t tiles = (M + FIELD_TC_TP - 1) / FIELD_TC_TP;
+    return tiles < (uint32_t)FIELD_CTAS ? tiles : (uint32_t)FIELD_CTAS;
+}
+
+size_t gfpp_field_tc_workspace_bytes(uint32_t M) {
+    if (M >= (1u << 30)) return 0;
+    return (size_t)FieldTcImg::total + (size_t)field_tc_ctas(M) * FieldPart::total * 4;
+}
+
+int gfpp_field_tc_forward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat, float *sigma,
+                          float *color, float *ambient_pos, void *workspace, size_t workspace_bytes, void *stream) {
+    FieldTcArgs t;
+    FieldArgs &a = t.f;
+    const int rc = field_setup("field_tc_forward", desc, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xyzs || !dirs || !cond_feat || !sigma || !color || !ambient_pos || !workspace) return fail(GFPP_ERR_INVALID, "field_tc_forward: null pointer%s");
+    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "field_tc_forward: M must be < 2^30%s");
+    if (workspace_bytes < FieldTcImg::total) return fail(GFPP_ERR_WORKSPACE, "field_tc_forward: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "field_tc_forward: workspace must be 256-byte aligned%s");
+    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    t.img = (unsigned char *)workspace;
+    a.wt = (float *)(t.img + FieldTcImg::bias);
+    a.sigma = sigma; a.color = color; a.ambient = ambient_pos;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_field_tc_relayout(t, st));
+    CK(launch_field_tc_fwd(t, st));
+    return GFPP_OK;
+}
+
+int gfpp_field_tc_backward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat,
+                           const float *grad_sigma, const float *grad_color, const float *grad_ambient_pos, float *const grad_w[8], float *grad_cond,
+                           float *grad_code, float *grad_position_table, float *grad_ambient_table, void *workspace, size_t workspace_bytes,
+                           void *stream) {
+    FieldTcArgs t;
+    FieldArgs &a = t.f;
+    const int rc = field_setup("field_tc_backward", desc, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xyzs || !dirs || !cond_feat || !grad_sigma || !grad_color || !grad_ambient_pos || !grad_w || !grad_cond || !grad_position_table ||
+        !grad_ambient_table || !workspace || (a.ind_dim > 0 && !grad_code))
+        return fail(GFPP_ERR_INVALID, "field_tc_backward: null pointer%s");
+    for (int i = 0; i < 8; ++i)
+        if (!grad_w[i]) return fail(GFPP_ERR_INVALID, "field_tc_backward: null weight gradient%s");
+    if (((uintptr_t)grad_position_table & 7u) || ((uintptr_t)grad_ambient_table & 7u))
+        return fail(GFPP_ERR_INVALID, "field_tc_backward: table gradients must be 8-byte aligned%s");
+    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "field_tc_backward: M must be < 2^30%s");
+    if (workspace_bytes < gfpp_field_tc_workspace_bytes(M)) return fail(GFPP_ERR_WORKSPACE, "field_tc_backward: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "field_tc_backward: workspace must be 256-byte aligned%s");
+    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    t.img = (unsigned char *)workspace;
+    a.wt = (float *)(t.img + FieldTcImg::bias);
+    a.part = (float *)(t.img + FieldTcImg::total);
+    a.n_cta = field_tc_ctas(M);
+    a.g_sigma = grad_sigma; a.g_color = grad_color; a.g_ambient = grad_ambient_pos;
+    a.g_pos_tab = (float2 *)grad_position_table; a.g_amb_tab = (float2 *)grad_ambient_table;
+    for (int i = 0; i < 8; ++i) a.g_w[i] = grad_w[i];
+    a.g_cond = grad_cond; a.g_code = grad_code;
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(launch_field_tc_relayout(t, st));
+    CK(launch_field_tc_bwd(t, st));
+    CK(launch_field_reduce(a, st));
+    return GFPP_OK;
 }
 
 }  // extern "C"

@@ -186,5 +186,25 @@ __device__ __forceinline__ void store_pair(unsigned char *hi_tile, unsigned char
     if (SPLIT) *reinterpret_cast<uint32_t *>(lo_tile + off) = pack2<BF16>(a - round16<BF16>(a), b - round16<BF16>(b));
 }
 
+// ---- transposed (MN-major) operands: D[64 x N] (+)= A^T * B with A [K x 64] and B [K x N] both row-major over K ----
+// A [rows x 64 elements] SW128 tile read along its rows is the canonical MN-major SW128 layout as it stands: one 128-byte row per
+// k, 8-row groups 1024 B apart (SBO), 64-element blocks of the M / N extent `lbo` bytes apart (LBO; unused when the extent is 64).
+// A k-step of 16 is 16 rows: 2048 B.  This is the weight-gradient product dW = dY^T X with both operands point-major.
+__device__ __forceinline__ uint64_t desc_sw128_mn(uint32_t saddr, uint32_t lbo) {
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+template <int N>
+__device__ __forceinline__ void wgmma_tn(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc);
+#define GFPP_ACC8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+template <> __device__ __forceinline__ void wgmma_tn<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 1, 1;\n\t}"
+                 : GFPP_ACC8(0), GFPP_ACC8(8), GFPP_ACC8(16), GFPP_ACC8(24) : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_tn<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 1, 1;\n\t}"
+                 : GFPP_ACC8(0), GFPP_ACC8(8), GFPP_ACC8(16), GFPP_ACC8(24), GFPP_ACC8(32), GFPP_ACC8(40), GFPP_ACC8(48), GFPP_ACC8(56) : "l"(da), "l"(db), "r"(acc));
+}
+#undef GFPP_ACC8
+
 }  // namespace tc
 }  // namespace gfpp

@@ -193,6 +193,10 @@ class RADNeRF(nn.Module):
         # reference runs under autocast), "bf16x3" (wgmma hi/lo split, ~fp32 accuracy), "bf16" (wgmma), "robust" (wgmma fp16
         # with the hi/lo split on the ambient net only + a 16-bit fixed-point position table: holds 1e-3 on well-conditioned scenes)
         self.mlp_precision = hparams.get("gfpp_mlp_precision", "fp32")
+        # arithmetic of the training field (forward() and the training branch of render()): "fp32" (CUDA-core FFMA, gfpp.h section
+        # G) or "fp16" (fp16 wgmma operands, fp32 accumulation, fp32 parameters and gradients, section J: what the reference's
+        # amp: true trains with, here without rounding the tables or the inputs of tanh and exp)
+        self.train_precision = hparams.get("gfpp_train_precision", "fp32")
         self._packed = None  # (key, packed_dev, Model, keepalive)
         self._workspace = None
 
@@ -590,11 +594,14 @@ class RADNeRF(nn.Module):
     def forward(self, position, direction, cond_feat, individual_code, cond_mask=None):
         """radnerf.py:108-141: (sigma [N] raw, color [N,3], ambient_pos [N,A]) at positions [N,3] in [-bound, bound] and directions
         [N,3], for one conditioning vector [1,64] and one individual code [ind_dim] (or None).  Differentiable w.r.t. the eight MLP
-        weights, both grid tables, cond_feat and individual_code, through libgfpp's fused fp32 kernels (gfpp.h section G).  cond_mask
-        is accepted and ignored, as in the reference.  The field always runs in fp32 and returns fp32, also under torch.autocast (the
-        reference's amp: false arithmetic; its autocast field would round the MLP operands and tables to fp16)."""
+        weights, both grid tables, cond_feat and individual_code, through libgfpp's fused kernels: fp32 FFMA (gfpp.h section G) or,
+        with train_precision = "fp16", fp16 tensor-core products with fp32 accumulation (section J).  cond_mask is accepted and
+        ignored, as in the reference.  Parameters, outputs and gradients are fp32 in both, also under torch.autocast, which does not
+        reach into the field (with train_precision = "fp32" that is the reference's amp: false arithmetic)."""
         if self.mlp_precision != "fp32":
             raise NotImplementedError(f"the training field runs in fp32 only (mlp_precision is {self.mlp_precision!r})")
+        if self.train_precision not in ("fp32", "fp16"):
+            raise ValueError(f'train_precision must be "fp32" or "fp16", got {self.train_precision!r}')
         if position.requires_grad or direction.requires_grad:
             raise NotImplementedError("gradients w.r.t. positions or directions (camera-pose optimisation) are not implemented")
         if self.density_bitfield.device.type != "cuda":

@@ -7,7 +7,8 @@ meaning and autograd behaviour -- over csrc/train_kernels.cu through the C-ABI (
                                                             perturb, 128, force_all_rays, dt_gamma, max_steps)
     weights_sum, ambient_sum, depth, image = raymarching.composite_rays_train(sigmas, rgbs, ambient, deltas, rays, T_thresh)
 
-`field` is RADNeRF.forward with its gradient (include/gfpp.h section G, csrc/field_train_kernel.cu); RADNeRF.forward calls it.
+`field` is RADNeRF.forward with its gradient (include/gfpp.h section G, csrc/field_train_kernel.cu, or with the model's
+train_precision = "fp16" section J, csrc/field_train_tc_kernel.cu); RADNeRF.forward calls it.
 `torso_field` is RADNeRFTorso.forward_torso with its gradient (section H); forward_torso calls it in training mode.
 `torso_sr_field` is the same for RADNeRFTorsowithSR.forward_torso (section I).  Both run csrc/torso_train_kernel.cu, one source
 instantiated for each field.
@@ -275,8 +276,13 @@ def _backward_buffers(M, dev, upstream, shapes, targets, code, tables):
 
 
 # ------------------------------------------------------------------------------------------------ the head field
-def _field_workspace(model, M):
-    return _workspace(model, "_field_ws", _capi.lib().gfpp_field_backward_workspace_bytes, M, "the training field")
+# model.train_precision -> (workspace attribute, workspace-size, forward and backward entry points); the two sets take the same arguments
+_FIELD_ENTRY = {"fp32": ("_field_ws", "gfpp_field_backward_workspace_bytes", "gfpp_field_forward", "gfpp_field_backward"),
+                "fp16": ("_field_tc_ws", "gfpp_field_tc_workspace_bytes", "gfpp_field_tc_forward", "gfpp_field_tc_backward")}
+
+
+def _field_workspace(model, entry, M):
+    return _workspace(model, entry[0], getattr(_capi.lib(), entry[1]), M, "the training field")
 
 
 def _field_desc(model, code, keep):
@@ -300,10 +306,14 @@ class _field(Function):
     """RADNeRF.forward (radnerf.py:108-141) over gfpp_field_forward / gfpp_field_backward: (xyzs [M,3], dirs [M,3], cond_feat [64] or
     [1,64], code [ind_dim] or None) -> (sigma [M], color [M,3], ambient_pos [M,A]).  `params` are the eight MLP weights and the two grid
     tables of `model`, passed so that autograd routes their gradients; the kernels read them in place.  No gradient reaches xyzs or
-    dirs (the caller rejects inputs that require one)."""
+    dirs (the caller rejects inputs that require one).  model.train_precision picks the entry points (_FIELD_ENTRY) at the forward;
+    the backward uses the same ones."""
 
     @staticmethod
     def forward(ctx, model, xyzs, dirs, cond_feat, code, *params):
+        if model.train_precision not in _FIELD_ENTRY:
+            raise ValueError(f'train_precision must be "fp32" or "fp16", got {model.train_precision!r}')
+        entry = ctx.entry = _FIELD_ENTRY[model.train_precision]
         x, dr = _cuda_f32(xyzs).view(-1, 3), _cuda_f32(dirs).view(-1, 3)
         if cond_feat.numel() != model.cond_out_dim:
             raise ValueError(f"cond_feat must hold one conditioning vector of {model.cond_out_dim} values, got shape {tuple(cond_feat.shape)}")
@@ -317,10 +327,10 @@ class _field(Function):
         amb = torch.empty(M, A, dtype=torch.float32, device=dev)
         keep = []
         d = _field_desc(model, cd, keep)
-        ws = _field_workspace(model, 0)
+        ws = _field_workspace(model, entry, 0)
         with torch.cuda.device(dev):
-            _capi.check(_capi.lib().gfpp_field_forward(ctypes.byref(d), x.data_ptr(), dr.data_ptr(), M, c.data_ptr(), sigma.data_ptr(), color.data_ptr(),
-                                                       amb.data_ptr(), ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_field_forward")
+            _capi.check(getattr(_capi.lib(), entry[2])(ctypes.byref(d), x.data_ptr(), dr.data_ptr(), M, c.data_ptr(), sigma.data_ptr(), color.data_ptr(),
+                                                       amb.data_ptr(), ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), entry[2])
         ctx.model = model
         ctx.shapes = (cond_feat.shape, None if code is None else code.shape)
         ctx.save_for_backward(x, dr, c, cd if cd is not None else torch.empty(0, device=dev), *params)
@@ -337,13 +347,13 @@ class _field(Function):
         grad_w, g_pos, g_tab, g_cond = grads[:8], grads[8], grads[9], grads[10]
         keep = []
         d = _field_desc(model, cd if code_shape is not None else None, keep)
-        ws = _field_workspace(model, M)
+        ws = _field_workspace(model, ctx.entry, M)
         ptrs = (ctypes.c_void_p * 8)(*[g.data_ptr() for g in grad_w])
         with torch.cuda.device(dev):
-            _capi.check(_capi.lib().gfpp_field_backward(ctypes.byref(d), x.data_ptr(), dr.data_ptr(), M, c.data_ptr(), g_sigma.data_ptr(),
-                                                        g_color.data_ptr(), g_amb.data_ptr(), ctypes.byref(ptrs), g_cond.data_ptr(),
-                                                        None if g_code is None else g_code.data_ptr(), g_pos.data_ptr(), g_tab.data_ptr(),
-                                                        ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_field_backward")
+            _capi.check(getattr(_capi.lib(), ctx.entry[3])(ctypes.byref(d), x.data_ptr(), dr.data_ptr(), M, c.data_ptr(), g_sigma.data_ptr(),
+                                                           g_color.data_ptr(), g_amb.data_ptr(), ctypes.byref(ptrs), g_cond.data_ptr(),
+                                                           None if g_code is None else g_code.data_ptr(), g_pos.data_ptr(), g_tab.data_ptr(),
+                                                           ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), ctx.entry[3])
         grads = [g.to(p.dtype) for g, p in zip(grads, params)]
         return (None, None, None, g_cond.view(cond_shape), None if g_code is None else g_code.view(code_shape), *grads)
 

@@ -39,6 +39,8 @@
  *  (H) the trainable torso field: RADNeRFTorso.forward_torso and its backward at explicit points, fp32.
  *
  *  (I) the trainable torso-SR field: RADNeRFTorsowithSR.forward_torso and its backward at explicit points, fp32.
+ *
+ *  (J) the trainable head field of (G) on tensor cores: fp16 operands, fp32 accumulation, fp32 parameters and gradients.
  */
 #ifndef GFPP_H_
 #define GFPP_H_
@@ -557,6 +559,31 @@ GFPP_API int gfpp_torso_sr_field_backward(const gfpp_torso_sr_desc *desc, const 
                                           const float *grad_deform, float *const grad_deform_w[3], float *const grad_canon_w[3],
                                           float *const grad_ha_w[3], float *const grad_ha_b[3], float *grad_code, float *grad_torso_table,
                                           void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------ (J) trainable head field on tensor cores
+ *
+ * The functions of (G) in a second arithmetic: the six 128-wide layers run as fp16 wgmma products with fp32 accumulation, forward
+ * and backward (input gradients against transposed fp16 weight images, weight gradients as dY^T X over 128-point tiles).  The
+ * parameters are read in place as fp32 and are not rounded in memory; all gradients come out in fp32.  Rounded to fp16: the
+ * operands of those products only (grid features, SH, hidden activations, weights, output gradients).  The grid gathers and
+ * scatters, biases, activation functions and their derivatives and the three narrow layers (ambient logits, the sigma row, colour
+ * logits) are fp32, the narrow layers on the fp32 accumulators -- the inputs of tanh and exp are never rounded to 16 bits.
+ * Every block of output gradients is scaled by a power of two taken from its largest magnitude before it is rounded and the product
+ * is scaled back in fp32, so upstream gradients multiplied by 2^k (loss scaling) give the same gradients times 2^k, and tiny
+ * upstream gradients are not flushed to zero.
+ *
+ * Arguments, desc fields read, validation, status codes, M == 0, gradient targets (grad_w overwritten, table gradients accumulated)
+ * and determinism are those of gfpp_field_forward / gfpp_field_backward; mlp_precision must be 0 here too (it names the inference
+ * arithmetic).  Results differ from (G) by the fp16 rounding: about 1e-3 absolute on colour and ambient_pos.
+ * Workspace (256-byte aligned): gfpp_field_tc_workspace_bytes(M) for the backward (0 = unsupported M); the forward needs
+ * gfpp_field_tc_workspace_bytes(0) bytes (the per-call fp16 weight images, ~340 KB). */
+GFPP_API size_t gfpp_field_tc_workspace_bytes(uint32_t M);
+GFPP_API int gfpp_field_tc_forward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat,
+                                   float *sigma, float *color, float *ambient_pos, void *workspace, size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_field_tc_backward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat,
+                                    const float *grad_sigma, const float *grad_color, const float *grad_ambient_pos, float *const grad_w[8],
+                                    float *grad_cond, float *grad_code, float *grad_position_table, float *grad_ambient_table,
+                                    void *workspace, size_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }
