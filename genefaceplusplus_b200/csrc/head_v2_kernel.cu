@@ -14,7 +14,9 @@
 //   * the 3-wide outputs and the sigma logit are N=16 MMAs against small RESIDENT tiles, handed to the row owners through a
 //     small buffer at the head of the slot's second operand tile (the sigma logit through a per-row buffer of its own);
 //   * the CTA is whole warpgroups: NSLOT owner warpgroups and one producer warpgroup, whose registers (setmaxnreg) go to
-//     the owners.
+//     the owners;
+//   * fp16: the position-grid features of a row's NEXT sample are looked up by the slot's GATHER WARP (producer warp 1 + s) while
+//     the slot runs its layers, and handed over through a per-row staging slot, so the owners never wait on those loads.
 //
 // Precision modes: FP16_X1 (the reference's autocast arithmetic) with 3 slots, and FP16_ROBUST with 2 slots: fp16 hi/lo
 // split (3 MMAs per k-step, ~22 mantissa bits) on the ambient net and a 16-bit fixed-point position table (gather8.cuh) --
@@ -37,6 +39,14 @@ using namespace headc;
 namespace {
 
 constexpr int TM = HEAD_TM;          // rows per slot
+// fp16: the first position level the gather warps look up; the owners look up levels [0, GATHER_L0) themselves, into the same
+// staging row.  0: the gather warps take all 16 levels; 8: the owners keep levels 0-7.  On an H100 80GB HBM3 (700 W) with the
+// bench's tables one warp per slot does not finish 16 levels in the shadow of the slot's layers (the "wait for staged position
+// features" stamp: 11 k cycles per batch at 0, 1.3 k at 8)
+constexpr int GATHER_L0 = 8;
+constexpr int GATHER_N = 2;          // levels per lookup call of a gather warp: 2 x 32-byte loads in flight per lane (56 registers, no spills)
+static_assert(GATHER_L0 == 0 || GATHER_L0 == 8, "the owners gather whole 8-level halves");
+static_assert(GATHER_N % 2 == 0 && 8 % GATHER_N == 0, "a lookup call of a gather warp stores whole 8-byte pairs of levels");
 
 template <bool ROBUST>
 struct Cfg {
@@ -45,9 +55,13 @@ struct Cfg {
     static constexpr int NTILE = ROBUST ? V2_NTILE_ROBUST : V2_NTILE_X1;
     static constexpr int NWORK = 4 * NSLOT;                 // row-owner warps
     static constexpr int NT = 128 * (NSLOT + 1);            // + one producer warpgroup: its warp 0 is the loader
+    // fp16: producer warps 1..NSLOT are the slots' gather warps and the owners read the position features from the staging rows;
+    // the robust mode has no shared memory left for staging and gathers in the owners
+    static constexpr bool STAGED = !ROBUST;
+    static constexpr int OWN_LV = STAGED ? GATHER_L0 : 16;  // position levels the owners look up themselves
     // register split (setmaxnreg): the owner warpgroups grow to OWNER_REGS, the producer warpgroup shrinks to PRODUCER_REGS.
     // The launch allocates 65536 / NT per thread (128 | 168); the owners' increase is served by the producer's decrease.
-    static constexpr int OWNER_REGS = ROBUST ? 232 : 160, PRODUCER_REGS = ROBUST ? 40 : 24;
+    static constexpr int OWNER_REGS = ROBUST ? 232 : 152, PRODUCER_REGS = ROBUST ? 40 : 56;
     static constexpr int LAUNCH_REGS = (65536 / NT) & ~7;
     static_assert(NSLOT * 128 * OWNER_REGS + 128 * PRODUCER_REGS <= 65536, "register split exceeds the register file");
     static_assert(NSLOT * 128 * (OWNER_REGS - LAUNCH_REGS) <= 128 * (LAUNCH_REGS - PRODUCER_REGS), "owners grow by more than the producer frees");
@@ -66,6 +80,10 @@ struct Misc {
     float occ_lo[3], occ_hi[3];
     bool have_box;
     unsigned long long w_full[4], w_free[4], res_full, batch_bar;
+    // fp16, per slot, one phase per batch: the owners have posted their rows' next coordinates (TM arrivals) | the gather warp
+    // has staged their features (32 arrivals); `pos_quit`: the owners' last request, the gather warp leaves
+    unsigned long long pos_req[3], pos_done[3];
+    volatile int pos_quit[3];
     volatile int stop;
     volatile int flag[2][16];            // per batch parity, per owner warp: "I have live rows"
 };
@@ -75,8 +93,12 @@ struct Misc {
 // behind Misc
 template <bool ROBUST>
 constexpr size_t slogit_bytes() { return ROBUST ? 0 : (size_t)Cfg<ROBUST>::NSLOT * TM * sizeof(float); }
+// fp16: the gather warps' staging rows behind the sigma logits, [NSLOT][TM] x 64 bytes: 16 levels as packed fp16 pairs (level j
+// in 32-bit word j) or, from the owner's post to the gather warp's reply, the row's next grid coordinates in chunk 0
 template <bool ROBUST>
-constexpr size_t smem_bytes() { return (size_t)Cfg<ROBUST>::OFF_MISC + sizeof(Misc) + slogit_bytes<ROBUST>() + 1024; }
+constexpr size_t stage_bytes() { return Cfg<ROBUST>::STAGED ? (size_t)Cfg<ROBUST>::NSLOT * TM * 64 : 0; }
+template <bool ROBUST>
+constexpr size_t smem_bytes() { return (size_t)Cfg<ROBUST>::OFF_MISC + sizeof(Misc) + slogit_bytes<ROBUST>() + stage_bytes<ROBUST>() + 1024; }
 static_assert(smem_bytes<false>() <= 227 * 1024 && smem_bytes<true>() <= 227 * 1024, "v2 shared memory budget");
 
 // Epilogue of one M = 64 half (rows 64*half ..) of a 128-wide layer from the accumulator fragment: (+bias) -> (ReLU) ->
@@ -101,6 +123,10 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 __device__ __forceinline__ float2 unpack_h2(uint32_t h) { return __half22float2(*reinterpret_cast<const __half2 *>(&h)); }
+
+// 16-byte chunk c of staging row `row`: chunks rotate with row / 2, so that eight consecutive rows' 16-byte accesses (the owners'
+// and the gather warp's) fall on distinct banks
+__device__ __forceinline__ uint32_t stage_off(int row, int c) { return (uint32_t)row * 64u + (uint32_t)((c ^ (row >> 1)) & 3) * 16u; }
 
 // N = 16 group over K = 128: operand tiles a | a + one tile against the two 2 KB halves of a resident tile at w
 __device__ __forceinline__ void mma16(float (&d)[8], uint32_t a, uint32_t w, uint32_t acc_first) {
@@ -142,6 +168,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
     unsigned char *sm = smem_raw_ + ((1024u - (smem_u32(smem_raw_) & 1023u)) & 1023u);
     Misc &ms = *reinterpret_cast<Misc *>(sm + C::OFF_MISC);
     unsigned char *wring = sm + C::OFF_W, *res = sm + C::OFF_RES;
+    unsigned char *stage = sm + C::OFF_MISC + sizeof(Misc) + slogit_bytes<ROBUST>();
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
     // ---------------- one-time setup ----------------
@@ -157,6 +184,8 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         for (int i = 0; i < 4; ++i) { mbar_init(&ms.w_full[i], 1); mbar_init(&ms.w_free[i], NWORK); }
         mbar_init(&ms.res_full, 1);
         mbar_init(&ms.batch_bar, NWORK);
+        if (C::STAGED)
+            for (int i = 0; i < C::NSLOT; ++i) { mbar_init(&ms.pos_req[i], TM); mbar_init(&ms.pos_done[i], 32); ms.pos_quit[i] = 0; }
         mbar_fence_init();
         ms.stop = 0;
     }
@@ -202,7 +231,9 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         struct { bool valid; int fate, D, gid, frame, nsamp; float dt, t_post, ws, depth, r, g, b, near, far; } cu;
         cu.valid = false; cu.fate = 0; cu.D = 0; cu.gid = 0; cu.frame = 0; cu.nsamp = 0;
         cu.dt = cu.t_post = cu.ws = cu.depth = cu.r = cu.g = cu.b = cu.near = cu.far = 0.f;
-        uint32_t feat[16];        // position features of the current sample (packed fp16 pairs), prefetched during the previous batch
+        // robust: position features of the current sample (packed fp16 pairs), looked up during the previous batch
+        uint32_t feat[C::STAGED ? 1 : 16];
+        unsigned char *stg = stage + s * TM * 64;   // fp16: this slot's staging rows
         uint32_t featl[ROBUST ? 16 : 1];
 
         // operand rows written by this warpgroup -> visible to its MMAs
@@ -320,15 +351,41 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
 #pragma unroll
                 for (int i = 0; i < 16; ++i) f[i] = 0.f;
             }
+            if constexpr (C::STAGED) {   // the staging row's chunks of these levels: the gather warp only touches chunks [GATHER_L0 / 4, 4)
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const uint32_t hi = pack2<false>(f[2 * i], f[2 * i + 1]);
-                feat[half * 8 + i] = hi;
-                if (ROBUST) {
-                    const float2 b = unpack_h2(hi);
-                    featl[half * 8 + i] = pack2<false>(f[2 * i] - b.x, f[2 * i + 1] - b.y);
+                for (int k = 0; k < 2; ++k)
+                    *reinterpret_cast<uint4 *>(stg + stage_off(row, 2 * half + k)) =
+                        make_uint4(pack2<false>(f[8 * k], f[8 * k + 1]), pack2<false>(f[8 * k + 2], f[8 * k + 3]),
+                                   pack2<false>(f[8 * k + 4], f[8 * k + 5]), pack2<false>(f[8 * k + 6], f[8 * k + 7]));
+            } else {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const uint32_t hi = pack2<false>(f[2 * i], f[2 * i + 1]);
+                    feat[half * 8 + i] = hi;
+                    if (ROBUST) {
+                        const float2 b = unpack_h2(hi);
+                        featl[half * 8 + i] = pack2<false>(f[2 * i] - b.x, f[2 * i + 1] - b.y);
+                    }
                 }
             }
+        };
+        // 16-byte chunk c (levels 4c .. 4c+3) of the current sample's position features
+        auto pos_chunk = [&](int c) -> uint4 {
+            if constexpr (C::STAGED) return *reinterpret_cast<const uint4 *>(stg + stage_off(row, c));
+            else return make_uint4(feat[4 * c], feat[4 * c + 1], feat[4 * c + 2], feat[4 * c + 3]);
+        };
+        // fp16: the NEXT sample's grid coordinates -> the row's staging slot, a request to the slot's gather warp.  An inactive row
+        // posts a point outside the grid, whose features are zeros
+        auto post_pos = [&]() {
+            float u = -1.f, vv = -1.f, w = -1.f;
+            if (sl.active) {
+                const float inv2b = 2.0f * mc.bound;
+                u = __fdiv_rn(__fadd_rn(sl.px, mc.bound), inv2b);
+                vv = __fdiv_rn(__fadd_rn(sl.py, mc.bound), inv2b);
+                w = __fdiv_rn(__fadd_rn(sl.pz, mc.bound), inv2b);
+            }
+            *reinterpret_cast<float4 *>(stg + stage_off(row, GATHER_L0 / 4)) = make_float4(u, vv, w, 0.f);
+            mbar_arrive(&ms.pos_req[s]);
         };
         // make `cu` the sample `sl` points at
         auto rotate = [&]() {
@@ -340,8 +397,9 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
 
         // ---------------- prologue: first rays, first samples, their position features ----------------
         refill();
-        prefetch_pos(0);
-        prefetch_pos(1);
+        if (C::OWN_LV > 0) prefetch_pos(0);
+        if (C::OWN_LV > 8) prefetch_pos(1);
+        if (C::STAGED) post_pos();
         rotate();
         mbar_wait(&ms.res_full, 0);   // the resident N = 16 / SH weight tiles
 
@@ -355,6 +413,10 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                     mbar_arrive(&ms.batch_bar);
                 }
             }
+            if (C::STAGED) {   // the gather warp's reply to the request posted during the previous batch (or the prologue)
+                mbar_wait(&ms.pos_done[s], bpar);
+                PH(6)   // wait for staged position features
+            }
             // ---------------- ambient-net input: h0 k[0,32) <- position features, k[32,64) | h1 k[0,32) <- conditioning ----------------
             if (newray && valid) {   // SH(dir) is constant along the ray: its K16 operand row is written once per ray (shencoder.cu:43-68)
                 float shv[16];
@@ -365,7 +427,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
             }
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
-                *reinterpret_cast<uint4 *>(h + sw128_off(row, c)) = make_uint4(feat[4 * c], feat[4 * c + 1], feat[4 * c + 2], feat[4 * c + 3]);
+                *reinterpret_cast<uint4 *>(h + sw128_off(row, c)) = pos_chunk(c);
                 if (ROBUST) *reinterpret_cast<uint4 *>(l + sw128_off(row, c)) = make_uint4(featl[4 * c], featl[4 * c + 1], featl[4 * c + 2], featl[4 * c + 3]);
             }
             {   // the frame's conditioning vector as pre-rounded fp16 images (k_cond_images): 8 x 16 bytes straight into the operand tiles
@@ -452,7 +514,7 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
             PH(4)   // MMA: ambient out
             const float amb0 = tanhf(outc[row]), amb1 = tanhf(outc[TM + row]), amb2 = tanhf(outc[2 * TM + row]);
             PH(5)   // tanh
-            // ---------------- sigma-net input: h0 k[0,32) <- position features (registers), k[32,64) <- ambient grid ----------------
+            // ---------------- sigma-net input: h0 k[0,32) <- position features, k[32,64) <- ambient grid ----------------
             {
                 float u = 0.f, vv = 0.f, w = 0.f;
                 if (valid) {   // GridEncoder.forward with bound = 1: (x + 1) / 2
@@ -461,8 +523,10 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                     w = __fdiv_rn(__fadd_rn(amb2, 1.0f), 2.0f);
                 }
 #pragma unroll
-                for (int c = 0; c < 4; ++c)
-                    *reinterpret_cast<uint4 *>(h + sw128_off(row, c)) = make_uint4(feat[4 * c], feat[4 * c + 1], feat[4 * c + 2], feat[4 * c + 3]);
+                for (int c = 0; c < 4; ++c) *reinterpret_cast<uint4 *>(h + sw128_off(row, c)) = pos_chunk(c);
+                // that was the last read of the staging row: it takes the next request now, so the gather warp's lookups run in the
+                // shadow of the ambient gather and this slot's sigma and colour nets
+                if (C::STAGED) post_pos();
 #pragma unroll 1
                 for (int half = 0; half < 2; ++half) {
                     float f[16];
@@ -477,9 +541,11 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                 }
             }
             PH(7)   // ambient gather
-            // the NEXT sample's position features (the current ones are in the operand tile now)
-            prefetch_pos(0);
-            PH(8)   // prefetch: position levels 0-7 of the next sample
+            // the NEXT sample's position features the owner looks up itself (the current ones are in the operand tile now)
+            if (C::OWN_LV > 0) {
+                prefetch_pos(0);
+                PH(8)   // prefetch: position levels 0-7 of the next sample
+            }
             ARRIVE_A();   // -> sigma L0
 
             // ---------------- sigma net 64 -> 128 -> 128 -> (128 geo + sigma) (radnerf.py:127-130) ----------------
@@ -487,8 +553,10 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
                      [&](const float (&d)[64], int hf) { epilogue_half<true, false, false>(d, h, h, hf, lane, wwarp, nullptr); });
             ARRIVE_A();   // -> sigma L1
             PH(9)   // MMA + epilogue: sigma L0
-            prefetch_pos(1);
-            PH(10)  // prefetch: position levels 8-15 of the next sample
+            if (C::OWN_LV > 8) {
+                prefetch_pos(1);
+                PH(10)  // prefetch: position levels 8-15 of the next sample
+            }
             layer128(2, [&](float (&d)[64], uint32_t o, uint32_t w0, uint32_t w1) {   // sigma L1: K = 128
                 wgmma_sw<128, false>(d, h_u + o, w0, 4, 0u);
                 wgmma_sw<128, false>(d, h_u + V2_TILE_BYTES + o, w1, 4, 1u);
@@ -595,6 +663,11 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         }
 #undef PH
 #undef ARRIVE_A
+        if (C::STAGED) {   // once the gather warp has served the last batch's request, a final one with the quit flag releases it
+            mbar_wait(&ms.pos_done[s], bpar);
+            if (row == 0) ms.pos_quit[s] = 1;
+            mbar_arrive(&ms.pos_req[s]);
+        }
         // stop the loader: the NSTAGE tiles it has prefetched for a batch that never comes must land before the CTA may exit.
         // `stop` is raised only once all of them have landed: the other slots may still be releasing their last tiles, and a
         // loader that saw `stop` before issuing these would leave the waits below hanging.
@@ -608,10 +681,56 @@ __global__ void __launch_bounds__(Cfg<ROBUST>::NT, 1) k_head_v2(const __grid_con
         __syncwarp();
     } else {
         // =====================================================================================================
-        // PRODUCER WARPGROUP: hands its registers to the owners; warp 0 is the LOADER, the other three leave.  No barrier
-        // counts them: `w_free` and `batch_bar` count owner warps, the named barriers the 128 threads of one slot.
+        // PRODUCER WARPGROUP: hands its registers to the owners; warp 0 is the LOADER, warp 1 + s (fp16) the GATHER WARP of
+        // slot s, any other leaves.  `w_free` and `batch_bar` count owner warps, the named barriers the 128 threads of one slot;
+        // only `pos_done` counts a gather warp, and its owners stop waiting on it before they release it.
         // =====================================================================================================
         setmaxnreg_dec<C::PRODUCER_REGS>();
+        if (C::STAGED && warp > NWORK && warp <= NWORK + C::NSLOT) {
+            // GATHER WARP: per request of its slot, the 16 - GATHER_L0 position levels [GATHER_L0, 16) of every row's posted point
+            // into the row's staging slot; lane l serves rows l, l + 32, .., GATHER_N levels per lookup call
+            const int gs = warp - NWORK - 1;
+            unsigned char *sg = stage + gs * TM * 64;
+            const bool smooth = a.pos_gm.interp == 1;
+#pragma unroll 1
+            for (uint32_t par = 0;; par ^= 1u) {
+                mbar_wait(&ms.pos_req[gs], par);
+                if (ms.pos_quit[gs]) break;
+                // outside the grid the lookup gives zeros (gather8.cuh): its loads are skipped
+                auto inside = [](const float4 &p) { return !(p.x < 0.f || p.x > 1.f || p.y < 0.f || p.y > 1.f || p.z < 0.f || p.z > 1.f); };
+                // a row's octs go towards L2 one row ahead of its loads: GATHER_N loads in flight per lane are too few to cover
+                // DRAM latency on their own
+                auto prefetch_row = [&](int r) {
+                    const float4 p = *reinterpret_cast<const float4 *>(sg + stage_off(r, GATHER_L0 / 4));
+                    if (inside(p)) prefetch_levels_l2<16 - GATHER_L0>(&ms.lvl[0][2 * GATHER_L0], a.pos_gm.align_off, a.pos_octs, p.x, p.y, p.z);
+                };
+                prefetch_row(lane);
+#pragma unroll 1
+                for (int r = lane; r < TM; r += 32) {
+                    const float4 p = *reinterpret_cast<const float4 *>(sg + stage_off(r, GATHER_L0 / 4));
+                    const bool in = inside(p);
+                    if (r + 32 < TM) prefetch_row(r + 32);
+#pragma unroll 1
+                    for (int lv = GATHER_L0; lv < 16; lv += GATHER_N) {
+                        float f[2 * GATHER_N];
+                        if (in) {
+                            lookup_levels<OCT_F16, GATHER_N>(&ms.lvl[0][2 * lv], a.pos_gm.align_off, smooth, a.pos_octs, p.x, p.y, p.z, f);
+                        } else {
+#pragma unroll
+                            for (int i = 0; i < 2 * GATHER_N; ++i) f[i] = 0.f;
+                        }
+                        uint32_t q[GATHER_N];
+#pragma unroll
+                        for (int i = 0; i < GATHER_N; ++i) q[i] = pack2<false>(f[2 * i], f[2 * i + 1]);
+#pragma unroll
+                        for (int i = 0; i < GATHER_N; i += 2)   // level lv + i in word (lv + i) % 4 of chunk (lv + i) / 4
+                            *reinterpret_cast<uint2 *>(sg + stage_off(r, (lv + i) / 4) + 4 * ((lv + i) % 4)) = make_uint2(q[i], q[i + 1]);
+                    }
+                }
+                mbar_arrive(&ms.pos_done[gs]);
+            }
+            return;
+        }
         if (warp != NWORK) return;
         // LOADER: resident tiles once, then the weight stream, NSTAGE tiles ahead of the issue warp
         if (elect_one()) {
