@@ -1,9 +1,11 @@
 """Shared helpers of the GPU parity tests."""
 import math
 
+import numpy as np
 import torch
 
 from genefaceplusplus_b200 import scene as scn
+from genefaceplusplus_b200.config import GridLayout
 from genefaceplusplus_b200.renderer import RADNeRF, RADNeRFTorso
 
 
@@ -25,6 +27,47 @@ def build_model(sc: scn.Scene, state=None, device="cuda", precision="fp32"):
     m.load_state_dict(state if state is not None else sc.state, strict=True)
     m.density_scale = sc.density_scale
     return m.to(device).eval()
+
+
+def relu_ties(trace, flip_band):
+    """Points within flip_band (relative to the layer's largest pre-activation) of a ReLU tie in any of the five ReLU layers of an
+    oracle forward's trace: a last-bit difference between two implementations can flip such a ReLU."""
+    tie = torch.zeros(trace["relu_pre"][0].shape[0], dtype=torch.bool)
+    for pre in trace["relu_pre"]:
+        tie |= (pre.abs() < flip_band * pre.abs().max()).any(1)
+    return tie
+
+
+def _ambient_levels(amb, hp):
+    """(scale, pos = u * scale + 0.5) per level of the ambient grid for ambient coordinates amb [N,A] in [-1,1], u = (amb + 1) / 2,
+    in float64."""
+    lay = GridLayout(amb.shape[1], log2_hashmap_size=hp["log2_hashmap_size"], desired_resolution=hp["desired_resolution"])
+    u = (amb.detach().double() + 1) / 2
+    for lv in range(lay.num_levels):
+        scale = float(np.exp2(np.float32(lv) * lay.S) * np.float32(lay.base_resolution) - np.float32(1.0))
+        yield scale, u * scale + 0.5
+
+
+def ties(trace, amb, hp, flip_band, cell_band):
+    """(points at a ReLU tie (relu_ties), points whose ambient coordinate lies within cell_band of a cell face of any level of the
+    ambient grid), from an oracle forward's trace and ambient output."""
+    face = torch.zeros(amb.shape[0], dtype=torch.bool)
+    for scale, pos in _ambient_levels(amb, hp):
+        face |= ((pos - pos.round()).abs() < cell_band * scale).any(1)
+    return relu_ties(trace, flip_band), face
+
+
+def cell_flips(amb_a, amb_b, hp):
+    """Points whose two ambient coordinates [N,A] fall into different cells of some level of the ambient grid, where the grid's
+    input gradient (a per-cell slope) jumps.  The cell is floor(u * scale + 0.5) with u = (amb + 1) / 2, in the fp32 arithmetic of
+    the grid kernels and of the C checker."""
+    lay = GridLayout(amb_a.shape[1], log2_hashmap_size=hp["log2_hashmap_size"], desired_resolution=hp["desired_resolution"])
+    ua, ub = (amb_a.detach().float() + 1) / 2, (amb_b.detach().float() + 1) / 2
+    flip = torch.zeros(amb_a.shape[0], dtype=torch.bool)
+    for lv in range(lay.num_levels):
+        scale = torch.tensor(np.exp2(np.float32(lv) * np.float32(lay.S)) * np.float32(lay.base_resolution) - np.float32(1.0), dtype=torch.float32)
+        flip |= (torch.floor(ua * scale + 0.5) != torch.floor(ub * scale + 0.5)).any(1)
+    return flip
 
 
 def psnr(a, b):

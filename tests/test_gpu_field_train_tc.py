@@ -225,6 +225,31 @@ def test_grad_scaler_step(setup):
     assert (m.sigma_net.net[1].weight.detach() - before).abs().max().item() > 0
 
 
+@pytest.mark.parametrize("value", [float("inf"), float("nan")], ids=["inf", "nan"])
+@pytest.mark.parametrize("which", ["gc", "gs"], ids=["grad_color", "grad_sigma"])
+def test_non_finite_upstream_skips_the_step(setup, which, value):
+    """One inf or NaN in the upstream gradient: a weight gradient comes out non-finite and a GradScaler step is skipped (loss scaling
+    relies on it; block_scale's fmaxf leaves a NaN out of the block's largest magnitude, so it must travel through the products)."""
+    s = setup
+    bad = dict(s)
+    bad[which] = s[which].clone()
+    bad[which].view(-1)[1234] = value
+    m = _model(s["sc"], s["hp"], s["state"], "fp16")
+    before = {k: p.detach().clone() for k, p in m.named_parameters() if k in ft.TRAINABLE}
+    opt = torch.optim.Adam([p for k, p in m.named_parameters() if k in ft.TRAINABLE], lr=1e-3)
+    scaler = torch.amp.GradScaler("cuda", init_scale=2.0 ** 16)
+    code = s["code"].cuda() if s["code"] is not None else None
+    out = m.forward(s["xyzs"].cuda(), s["dirs"].cuda(), s["cond"].cuda(), code)
+    scaler.scale(_loss(out, bad, s["xyzs"].shape[0])).backward()
+    finite = {k: bool(torch.isfinite(p.grad).all()) for k, p in m.named_parameters() if k in ft.TRAINABLE}
+    scaler.step(opt)
+    scaler.update()
+    print(f"{which}[1234] = {value}: non-finite gradients {[k for k, v in finite.items() if not v]}; scale {scaler.get_scale():.0f}")
+    assert not all(finite[k] for k in ft.TRAINABLE[:8]), finite
+    assert scaler.get_scale() < 2.0 ** 16, "the step was not skipped"
+    assert all(torch.equal(p.detach(), before[k]) for k, p in m.named_parameters() if k in ft.TRAINABLE)
+
+
 def test_backward_is_deterministic(setup):
     s = setup
     out1, g1 = _gpu_field(s)

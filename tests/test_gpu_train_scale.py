@@ -24,6 +24,7 @@ from genefaceplusplus_b200 import scene as scn
 from genefaceplusplus_b200 import train_ops
 from genefaceplusplus_b200.config import GridLayout, may_hparams
 from genefaceplusplus_b200.renderer import RADNeRF
+from helpers import ties
 from oracle import field_train as ft
 from oracle import ops
 
@@ -65,21 +66,6 @@ def _rm():
 
 
 # ------------------------------------------------------------------------------------------------ 1. head field across CTA tiles
-def _ties(trace, amb, hp):
-    """Points at a ReLU tie of any of the five ReLU layers (FLIP_BAND) and points whose ambient coordinate lies within CELL_BAND of a
-    cell face of any level of the ambient grid, from an oracle forward's trace and ambient output."""
-    tie = torch.zeros(amb.shape[0], dtype=torch.bool)
-    for pre in trace["relu_pre"]:
-        tie |= (pre.abs() < FLIP_BAND * pre.abs().max()).any(1)
-    lay = GridLayout(amb.shape[1], log2_hashmap_size=hp["log2_hashmap_size"], desired_resolution=hp["desired_resolution"])
-    u = (amb.detach().double() + 1) / 2
-    face = torch.zeros_like(tie)
-    for lv in range(lay.num_levels):
-        scale = float(np.exp2(np.float32(lv) * lay.S) * np.float32(lay.base_resolution) - np.float32(1.0))
-        pos = u * scale + 0.5
-        face |= ((pos - pos.round()).abs() < CELL_BAND * scale).any(1)
-    return tie, face
-
 
 @pytest.fixture(scope="module", params=SHAPES, ids=lambda v: f"amb{v[0]}_ind{v[1]}")
 def field_case(request):
@@ -106,7 +92,7 @@ def field_case(request):
     gs, gc, ga = torch.randn(M, generator=g), torch.randn(M, 3, generator=g), torch.randn(M, amb_dim, generator=g)
     trace = {}
     _, _, amb = ft.field_forward(ft.field_params(state), hp, xyzs, dirs, cond_feat.cpu(), code, trace=trace)
-    tie, face = _ties(trace, amb, hp)
+    tie, face = ties(trace, amb, hp, FLIP_BAND, CELL_BAND)
     gs[tie | face], gc[tie | face], ga[tie | face] = 0, 0, 0
     print(f"[amb {amb_dim}, ind {ind_dim}] {int(tie.sum())} of {M} points at a ReLU tie, {int((face & ~tie).sum())} more at an ambient cell face")
     return dict(hp=hp, state=state, model=model, xyzs=xyzs, dirs=dirs, cond=cond_feat.cpu(), code=code, gs=gs, gc=gc, ga=ga)
@@ -618,7 +604,7 @@ def test_steady_state_training_step(monkeypatch):
         if "mask" not in keep:
             tr = {}
             out = field_forward(p, hp, xyzs, dirs, cf, code, trace=tr)
-            tie, face = _ties(tr, out[2], hp)
+            tie, face = ties(tr, out[2], hp, FLIP_BAND, CELL_BAND)
             keep["mask"] = ~(tie | face)
             keep["counts"] = (int(tie.sum()), int((face & ~tie).sum()))
         else:
