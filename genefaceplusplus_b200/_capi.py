@@ -105,6 +105,7 @@ EXPORTS = [
     "gfpp_field_tc_workspace_bytes", "gfpp_field_tc_forward", "gfpp_field_tc_backward",
     "gfpp_torso_field_workspace_bytes", "gfpp_torso_field_forward", "gfpp_torso_field_backward",
     "gfpp_torso_sr_field_workspace_bytes", "gfpp_torso_sr_field_forward", "gfpp_torso_sr_field_backward",
+    "gfpp_frozen_head_workspace_bytes", "gfpp_frozen_head",
 ]
 
 
@@ -190,6 +191,10 @@ def lib():
         L.gfpp_field_tc_workspace_bytes.argtypes = [c_u32]
         L.gfpp_field_tc_forward.argtypes = L.gfpp_field_forward.argtypes
         L.gfpp_field_tc_backward.argtypes = L.gfpp_field_backward.argtypes
+        L.gfpp_frozen_head_workspace_bytes.restype = c_size_t
+        L.gfpp_frozen_head_workspace_bytes.argtypes = [c_u32, c_u32]
+        L.gfpp_frozen_head.argtypes = [ctypes.POINTER(Model), P, P, c_u32, ctypes.POINTER(c_f), P, P, P, c_f,
+                                       c_u32, c_f, P, P, P, c_size_t, P]
         L.gfpp_torso_field_workspace_bytes.restype = c_size_t
         L.gfpp_torso_field_workspace_bytes.argtypes = [c_u32]
         L.gfpp_torso_field_forward.argtypes = [ctypes.POINTER(ModelDesc), P, c_u32, P, P, P, P, P, P, c_size_t, P]

@@ -165,6 +165,8 @@ struct ModelHost {
     const unsigned char *v2_stream, *v2_res;
     const float *v2_pos_step;       // robust mode: per-level step of the 16-bit position table
     const float *amb0_src;          // ambient_net.net.0.weight [128,96] (its conditioning columns are folded per frame)
+    const float *color0_src;        // color_net.net.0.weight [128, 144 + ind_dim] (gfpp_frozen_head folds a per-call code into a copy of `narrow`)
+    int ind_dim;
 };
 static_assert(sizeof(ModelHost) <= sizeof(gfpp_model), "gfpp_model opaque storage too small");
 constexpr uint32_t kMagic = 0x67667070u;  // "gfpp"
@@ -496,6 +498,8 @@ int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes,
     const bool robust = d->mlp_precision == 4;
     if (d->mlp_precision != 0) CKN(cudaMemsetAsync(base + L.tc_hi, 0, L.pos_quads - L.tc_hi, st));
     m.amb0_src = d->ambient_w[0];
+    m.color0_src = d->color_w[0];
+    m.ind_dim = (int)d->ind_dim;
     if (d->mlp_precision == 1 || robust) {
         // v2 weight images: streamed tiles in the kernel's schedule order (head_kernel.cuh), then the resident block
         unsigned char *vs = (unsigned char *)(base + L.v2_stream), *vr = (unsigned char *)(base + L.v2_res);
@@ -1837,6 +1841,116 @@ int gfpp_field_tc_backward(const gfpp_model_desc *desc, const float *xyzs, const
     CK(launch_field_tc_relayout(t, st));
     CK(launch_field_tc_bwd(t, st));
     CK(launch_field_reduce(a, st));
+    return GFPP_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------- (K) frozen head of the torso training steps
+namespace {
+struct FrozenWork { size_t narrow, depth, rays_t, survivors, hits, zero_begin, hist, counters, zero_end, cond, total; };
+FrozenWork frozen_work_layout(uint32_t N, uint32_t max_steps) {
+    FrozenWork W;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
+    W.narrow = take(8 * 128 * 4);          // the packed narrow rows with this call's individual code folded into row 7
+    W.depth = take((size_t)N * 4);
+    W.rays_t = take((size_t)N * 4);
+    W.survivors = take((size_t)N * 4);
+    W.hits = take((size_t)N * 64);         // HitRecord (head_common.cuh)
+    W.zero_begin = o;
+    W.hist = take((size_t)(max_steps + 2) * 4);
+    W.counters = take(16 * 4);
+    W.zero_end = o;
+    W.cond = take(64 * 2 * 2);             // fp16 hi + lo images of cond_feat (v2 head kernel)
+    W.total = o;
+    return W;
+}
+}  // namespace
+
+extern "C" {
+
+size_t gfpp_frozen_head_workspace_bytes(uint32_t N, uint32_t max_steps) {
+    if (N == 0 || N >= (1u << 31) || max_steps < 1 || max_steps > 4096) return 0;
+    return frozen_work_layout(N, max_steps).total;
+}
+
+int gfpp_frozen_head(const gfpp_model *model, const float *rays_o, const float *rays_d, uint32_t N, const float aabb[6], const float *cond_feat,
+                     const float *code, const float *noises, float dt_gamma, uint32_t max_steps, float T_thresh, float *weights_sum, float *image,
+                     void *workspace, size_t workspace_bytes, void *stream) {
+    if (!model || !rays_o || !rays_d || !aabb || !cond_feat || !weights_sum || !image || !workspace)
+        return fail(GFPP_ERR_INVALID, "frozen_head: null pointer%s");
+    ModelHost m;
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "frozen_head: model handle not initialised by gfpp_model_pack%s");
+    if (N == 0) return fail(GFPP_ERR_INVALID, "frozen_head: no rays%s");
+    if (N >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "frozen_head: N must be < 2^31%s");
+    if (max_steps < 1 || max_steps > 4096) return fail(GFPP_ERR_UNSUPPORTED, "frozen_head: max_steps must be in 1..4096%s");
+    if ((m.ind_dim > 0) != (code != nullptr)) return fail(GFPP_ERR_INVALID, "frozen_head: code must be given iff the model has individual codes%s");
+    for (int k = 0; k < 3; ++k)
+        if (!(aabb[k] <= aabb[3 + k])) return fail(GFPP_ERR_INVALID, "frozen_head: aabb must be (xmin, ymin, zmin, xmax, ymax, zmax)%s");
+    const bool use_v2 = m.v2_ok && (m.mlp_precision == 4 || (m.mlp_precision == 1 && getenv("GFPP_HEAD_V1") == nullptr));
+    if (m.mlp_precision == 4 && !use_v2) return fail(GFPP_ERR_UNSUPPORTED, "frozen_head: robust mode unavailable for this model%s");
+    const FrozenWork W = frozen_work_layout(N, max_steps);
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "frozen_head: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "frozen_head: workspace must be 256-byte aligned%s");
+    cudaStream_t st = (cudaStream_t)stream;
+    char *ws = (char *)workspace;
+    g_launches = 0;
+    CKN(cudaMemsetAsync(ws + W.zero_begin, 0, W.zero_end - W.zero_begin, st));
+    // this call's individual code: a copy of the packed narrow rows with `code` folded into the colour-L0 bias (row 7) exactly as
+    // gfpp_model_pack folds row 0; the packed model is never written, so render() keeps using row 0
+    float *narrow = (float *)(ws + W.narrow);
+    CKN(cudaMemcpyAsync(narrow, m.narrow, (code ? 7 : 8) * 128 * 4, cudaMemcpyDeviceToDevice, st));
+    if (code) CK(launch_fold_bias(m.color0_src, 16 + 128 + m.ind_dim, 144, m.ind_dim, code, 128, narrow + 7 * 128, st));
+
+    HeadArgs a;
+    memset(&a, 0, sizeof(a));
+    a.pos_gm = m.pos_gm; a.amb_gm = m.amb_gm;
+    a.pos_tab = m.pos_tab; a.amb_tab = m.amb_tab;
+    a.pos_quads = m.pos_quads; a.amb_quads = m.amb_quads;
+    a.pos_octs = m.pos_octs; a.amb_octs = m.amb_octs;
+    a.wide = m.wide; a.narrow = narrow;
+    for (int c = 0; c < HEAD_NCHUNK; ++c) { a.chunk_off[c] = m.chunk_off[c]; a.chunk_k[c] = kChunkK[c]; }
+    march_const_init(a.mc, m.bound, dt_gamma, max_steps, m.cascade, m.grid_size, m.bitfield);
+    a.occ_bounds = m.occ_bounds;
+    a.coarse_bits = m.coarse_bits;
+    a.coarse_words = m.coarse_words;
+    memcpy(a.aabb, aabb, sizeof(a.aabb));
+    a.min_near = m.min_near; a.density_scale = m.density_scale;
+    // the occupied-box shortcut assumes no sample position is clamped to the cube: it holds for this call's aabb only if it lies inside
+    const float cube = m.bound;
+    a.use_occ_box = (m.cascade == 1 && aabb[0] >= -cube && aabb[1] >= -cube && aabb[2] >= -cube && aabb[3] <= cube && aabb[4] <= cube &&
+                     aabb[5] <= cube) ? 1 : 0;
+    a.n_frames = 1; a.n_rays = (int)N;
+    a.rays_o = rays_o; a.rays_d = rays_d;
+    a.cond_feat = cond_feat;
+    a.max_steps = (int)max_steps; a.T_thresh = T_thresh;
+    a.noises = noises;
+    a.image = image;
+    a.wsum = weights_sum;
+    a.depth = (float *)(ws + W.depth);
+    a.rays_t = (float *)(ws + W.rays_t);
+    a.hist = (int *)(ws + W.hist);
+    a.survivors = (int *)(ws + W.survivors);
+    int *counters = (int *)(ws + W.counters);
+    a.n_survivors = counters + 2;
+    a.hits = (uint4 *)(ws + W.hits);
+    a.n_hits = counters + 3;
+    a.pass = 1;
+    a.cursor = counters + 0;
+    // pass 1 only: a ray that reaches max_steps samples is final (march_rays_train gives it no more), so there is no schedule,
+    // no pass 2 and no epilogue
+    CK(launch_ray_setup(a, st));
+    if (m.mlp_precision == 0) CK(launch_head(a, -1, st, true));
+    else if (use_v2) {
+        HeadV2Args v2;
+        v2.w_stream = m.v2_stream; v2.w_res = m.v2_res; v2.pos_step = m.v2_pos_step;
+        v2.cond_hi = (const unsigned char *)(ws + W.cond);
+        v2.cond_lo = v2.cond_hi + 128;
+        CK(launch_cond_images(cond_feat, 1, ws + W.cond, ws + W.cond + 128, st));
+        CK(launch_head_v2(a, v2, m.mlp_precision, st, true));
+    } else CK(launch_head_tc(a, m.tc, m.mlp_precision, -1, st, true));
     return GFPP_OK;
 }
 

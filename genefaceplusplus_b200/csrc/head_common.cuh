@@ -22,6 +22,7 @@ __device__ __forceinline__ void warp_agg_add(int *base, int key, int val) {
 struct Slot {
     RayGeom g;
     float t, near, far, ws, depth, r, gch, b;
+    float T;       // transmittance as composite_rays_train carries it (training termination only; see composite_and_advance)
     float far_m;   // marching bound: min(far, exit of the padded occupied box) -- nothing is occupied beyond it
     float px, py, pz, dt;  // pending sample
     int gid, frame, nsamp, cap;
@@ -160,7 +161,7 @@ __device__ __forceinline__ int refill_and_publish(const HeadArgs &a, SmemT &s, S
                     ray_geom_init(sl.g, hr.ox, hr.oy, hr.oz, hr.dx, hr.dy, hr.dz);
                     sl.near = hr.near; sl.far = hr.far; sl.far_m = hr.far_m;
                     sl.t = hr.t; sl.px = hr.px; sl.py = hr.py; sl.pz = hr.pz; sl.dt = hr.dt;
-                    sl.ws = 0.f; sl.depth = 0.f; sl.r = sl.gch = sl.b = 0.f;
+                    sl.ws = 0.f; sl.depth = 0.f; sl.r = sl.gch = sl.b = 0.f; sl.T = 1.f;
                     sl.nsamp = 0; sl.cap = a.max_steps;
                     live = true;
                 } else {
@@ -195,14 +196,18 @@ __device__ __forceinline__ int refill_and_publish(const HeadArgs &a, SmemT &s, S
 
 // Front-to-back compositing of the batch's sample in the owner thread (raymarching.cu:978-1006), termination test,
 // then march to the ray's next sample (or retire the ray).
-template <class SmemT>
+// TRAIN: the termination of composite_rays_train (raymarching.cu:647-667) instead, for the frozen head of the torso training
+// step (gfpp_frozen_head, pass 1 only): T is the running product of (1 - alpha) and the ray stops after the sample that takes
+// it below T_thresh.  Inference uses T = 1 - weights_sum before the sample and stops one sample later.
+template <bool TRAIN = false, class SmemT>
 __device__ __forceinline__ void composite_and_advance(const HeadArgs &a, SmemT &s, Slot &sl, const MarchConst &mc, int tid) {
     constexpr int TM = HEAD_TM;
     if (tid < TM && sl.active) {
         const float sigma = s.sig[tid];
         const float alpha = 1.0f - expf(-sigma * sl.dt);
-        const float T = 1.0f - sl.ws;
+        const float T = TRAIN ? sl.T : 1.0f - sl.ws;
         const float w = alpha * T;
+        if (TRAIN) sl.T = T * (1.0f - alpha);
         sl.ws += w;
         sl.depth += w * sl.t;  // sl.t is already the post-sample t (deltas[1])
         sl.r += w * s.rgb[tid];
@@ -212,7 +217,7 @@ __device__ __forceinline__ void composite_and_advance(const HeadArgs &a, SmemT &
         if (a.valid_samples) warp_agg_add(a.valid_samples, sl.frame, 1);
         int D = 0;  // death index (1-based sample position), 0 = still alive
         bool suspend = false;
-        if (T < a.T_thresh) D = sl.nsamp;
+        if ((TRAIN ? sl.T : T) < a.T_thresh) D = sl.nsamp;
         else if (sl.nsamp >= sl.cap) suspend = true;
         else if (!march_next(mc, sl.g, sl.far_m, sl.t, sl.px, sl.py, sl.pz, sl.dt)) D = sl.nsamp + 1;
         if (D) {

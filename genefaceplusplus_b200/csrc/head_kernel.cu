@@ -201,6 +201,8 @@ using namespace headc;
 
 }  // namespace
 
+// TRAIN: composite_rays_train's termination (composite_and_advance), pass 1 only (gfpp_frozen_head)
+template <bool TRAIN>
 __global__ void __launch_bounds__(HEAD_NT, 1) k_head(const __grid_constant__ HeadArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Smem &s = *reinterpret_cast<Smem *>(smem_raw);
@@ -365,7 +367,7 @@ __global__ void __launch_bounds__(HEAD_NT, 1) k_head(const __grid_constant__ Hea
         __syncthreads();
 
         // ================= composite + advance (head_common.cuh) =================
-        composite_and_advance(a, s, sl, mc, tid);
+        composite_and_advance<TRAIN>(a, s, sl, mc, tid);
         // no barrier needed here: the refill starts with one before shared memory is touched again
     }
 
@@ -613,16 +615,17 @@ cudaError_t launch_dump_rays(const HeadArgs &a, float *rays_o, float *rays_d, cu
 
 size_t head_smem_bytes() { return sizeof(Smem); }
 
-cudaError_t launch_head(const HeadArgs &a, int total_hint, cudaStream_t st) {
+cudaError_t launch_head(const HeadArgs &a, int total_hint, cudaStream_t st, bool train) {
+    auto kern = train ? k_head<true> : k_head<false>;
     // function attributes are per device: set on every launch, never cached process-wide
-    cudaError_t e = cudaFuncSetAttribute(k_head, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem));
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem));
     if (e != cudaSuccess) return e;
     int blocks = sm_count();
     if (total_hint >= 0) {
         const int need = (total_hint + TM - 1) / TM;
         if (need < blocks) blocks = need > 0 ? need : 1;
     }
-    k_head<<<blocks, NT, sizeof(Smem), st>>>(a);
+    kern<<<blocks, NT, sizeof(Smem), st>>>(a);
     return cudaGetLastError();
 }
 

@@ -74,7 +74,7 @@ constexpr int head_tc_chunk_ksteps(int c) { return kHeadTcChunks[c].k16 ? 1 : kH
 struct HeadTcArgs {
     const unsigned char *w_hi, *w_lo;       // the 12 streamed tiles back to back (head_tc_chunk_off), hi and lo images with identical layout
 };
-cudaError_t launch_head_tc(const HeadArgs &a, const HeadTcArgs &t, int precision, int total_hint, cudaStream_t st);
+cudaError_t launch_head_tc(const HeadArgs &a, const HeadTcArgs &t, int precision, int total_hint, cudaStream_t st, bool train = false);
 size_t head_tc_smem_bytes(bool split);
 
 // ---- v2 (head_v2_kernel.cu): one CTA per SM, 2-3 row-owner slots of 128 samples sharing one weight stream ----
@@ -92,7 +92,7 @@ struct HeadV2Args {
     const unsigned char *cond_lo;    // [F,64] fp16 residuals (robust mode)
     const float *pos_step;           // [16] per-level step of the 16-bit fixed-point position table (robust mode) or nullptr
 };
-cudaError_t launch_head_v2(const HeadArgs &a, const HeadV2Args &t, int precision, cudaStream_t st);
+cudaError_t launch_head_v2(const HeadArgs &a, const HeadV2Args &t, int precision, cudaStream_t st, bool train = false);
 cudaError_t launch_cond_images(const float *cond_feat, int n_frames, void *cond_hi, void *cond_lo, cudaStream_t st);
 size_t head_v2_smem_bytes(bool robust);
 
@@ -138,7 +138,8 @@ cudaError_t launch_density(const HeadArgs &a, const DensityArgs &d, cudaStream_t
 cudaError_t launch_density_tc(const HeadArgs &a, const HeadTcArgs &t, const DensityArgs &d, cudaStream_t st);
 
 size_t head_smem_bytes();
-cudaError_t launch_head(const HeadArgs &a, int total_hint, cudaStream_t st);
+// train: pass 1 with composite_rays_train's termination (k_head<true>, k_head_tc<.., .., true>, k_head_v2_train; gfpp_frozen_head)
+cudaError_t launch_head(const HeadArgs &a, int total_hint, cudaStream_t st, bool train = false);
 cudaError_t launch_ray_setup(const HeadArgs &a, cudaStream_t st);
 cudaError_t launch_dump_rays(const HeadArgs &a, float *rays_o, float *rays_d, cudaStream_t st);
 cudaError_t launch_schedule(const int *hist, int n_frames, int n_rays, int max_steps, int *B_total, cudaStream_t st);

@@ -188,7 +188,8 @@ __device__ __noinline__ void lookup4(const GridMeta &gm, const float2 *__restric
 
 }  // namespace
 
-template <bool BF16, bool SPLIT>
+// TRAIN: composite_rays_train's termination (composite_and_advance), pass 1 only (gfpp_frozen_head)
+template <bool BF16, bool SPLIT, bool TRAIN>
 __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid_constant__ HeadArgs a, const __grid_constant__ HeadTcArgs t) {
     extern __shared__ __align__(1024) unsigned char smem_raw_[];
     unsigned char *smem_raw = smem_raw_ + ((1024u - (smem_u32(smem_raw_) & 1023u)) & 1023u);
@@ -411,7 +412,7 @@ __global__ void __launch_bounds__(HEAD_NT, SPLIT ? 1 : 2) k_head_tc(const __grid
 
         PH(9)   // color net: 2 MMA layers + epilogue + sigmoid
         // ================= composite + advance (head_common.cuh) =================
-        composite_and_advance(a, s, sl, mc, tid);
+        composite_and_advance<TRAIN>(a, s, sl, mc, tid);
         PH(10)  // composite + march to next sample
         if (a.phase_cycles && tid == 0) atomicAdd(a.phase_cycles + 31, 1ull);   // batches
         // no barrier needed here: the refill starts with one before shared memory is touched again
@@ -425,7 +426,7 @@ static_assert(sizeof(SmemTC<false>) + 1024 <= 113 * 1024, "single-pass kernel mu
 static_assert(sizeof(SmemTC<true>) + 1024 <= 227 * 1024, "split kernel exceeds the per-CTA shared memory limit");
 size_t head_tc_smem_bytes(bool split) { return (split ? sizeof(SmemTC<true>) : sizeof(SmemTC<false>)) + 1024; }
 
-cudaError_t launch_head_tc(const HeadArgs &a, const HeadTcArgs &t, int precision, int total_hint, cudaStream_t st) {
+cudaError_t launch_head_tc(const HeadArgs &a, const HeadTcArgs &t, int precision, int total_hint, cudaStream_t st, bool train) {
     const bool split = precision == BF16_X3;
     int blocks = sm_count() * (split ? 1 : 2);   // single-pass kernels: two resident CTAs per SM
     if (getenv("GFPP_ONE_CTA")) blocks = sm_count();   // diagnostics: phase timings without the co-resident CTA
@@ -435,20 +436,20 @@ cudaError_t launch_head_tc(const HeadArgs &a, const HeadTcArgs &t, int precision
     }
     const size_t smem = head_tc_smem_bytes(split);
     cudaError_t e;
-#define GO(BF, SP)                                                                                             \
-    e = cudaFuncSetAttribute(k_head_tc<BF, SP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);       \
+#define GO(BF, SP, TR)                                                                                         \
+    e = cudaFuncSetAttribute(k_head_tc<BF, SP, TR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   \
     if (e != cudaSuccess) return e;                                                                            \
-    e = cudaFuncSetAttribute(k_head_tc<BF, SP>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared); \
+    e = cudaFuncSetAttribute(k_head_tc<BF, SP, TR>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared); \
     if (e != cudaSuccess) return e;                                                                            \
     if (getenv("GFPP_DEBUG")) {                                                                                \
         int occ = 0;                                                                                           \
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_head_tc<BF, SP>, NT, smem);                      \
-        fprintf(stderr, "[gfpp] k_head_tc<%d,%d>: %zu B smem, %d CTA/SM, grid %d\n", (int)BF, (int)SP, smem, occ, blocks); \
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_head_tc<BF, SP, TR>, NT, smem);                  \
+        fprintf(stderr, "[gfpp] k_head_tc<%d,%d,%d>: %zu B smem, %d CTA/SM, grid %d\n", (int)BF, (int)SP, (int)TR, smem, occ, blocks); \
     }                                                                                                          \
-    k_head_tc<BF, SP><<<blocks, NT, smem, st>>>(a, t);
-    if (precision == FP16_X1) { GO(false, false) }
-    else if (precision == BF16_X1) { GO(true, false) }
-    else if (precision == BF16_X3) { GO(true, true) }
+    k_head_tc<BF, SP, TR><<<blocks, NT, smem, st>>>(a, t);
+    if (precision == FP16_X1) { if (train) { GO(false, false, true) } else { GO(false, false, false) } }
+    else if (precision == BF16_X1) { if (train) { GO(true, false, true) } else { GO(true, false, false) } }
+    else if (precision == BF16_X3) { if (train) { GO(true, true, true) } else { GO(true, true, false) } }
     else return cudaErrorInvalidValue;
 #undef GO
     return cudaGetLastError();

@@ -643,6 +643,70 @@ class RADNeRF(nn.Module):
         results["depth_map"] = (torch.clamp(depth - nears, min=0) / (fars - nears)).view(*prefix)
         return results
 
+    # ------------------------------------------------------------------ the frozen head of the torso training steps
+    def _aabb_train_host(self):
+        """aabb_train as six host floats, copied from the device once per buffer version (the slab test takes them by value)."""
+        key = (self.aabb_train.data_ptr(), self.aabb_train._version)
+        cached = self.__dict__.get("_aabb_train_cache")
+        if cached is None or cached[0] != key:
+            vals = (ctypes.c_float * 6)(*[float(v) for v in self.aabb_train.detach().cpu().tolist()])
+            cached = self.__dict__["_aabb_train_cache"] = (key, vals)
+        return cached[1]
+
+    def frozen_head(self, rays_o, rays_d, cond_feat, ind_code, perturb=False, dt_gamma=0, max_steps=1024, T_thresh=1e-4, force_all_rays=False):
+        """The no-grad head block of the torso training step (radnerf_torso.py:92-150, radnerf_torso_sr.py:150) in one fused pass over
+        the packed head model (gfpp.h section K): (weights_sum [N], image [N,3]) fp32, the first and fourth outputs of
+        near_far_from_aabb(aabb_train) + march_rays_train + forward + composite_rays_train, without ambient_sum and depth.
+
+        rays_o / rays_d: [..., 3] with N rays.  cond_feat: one conditioning vector ([64] or [1,64]).  ind_code: the training row
+        individual_embeddings[index] (a device tensor, read on the device), or None iff the model has no individual codes.  The
+        head runs in the model's mlp_precision (fp32, or the arithmetic of the torso configs' amp: true with "fp16"), in train or
+        eval mode, and never records autograd.  perturb=True draws one torch.rand(N) on the model's device before anything else
+        random, as march_rays_train does, so a seeded call jitters each ray as the composed path does.  step_counter / local_step
+        are neither read nor written; with mean_count > 0 march_rays_train would truncate rays to its sample budget, which this
+        call does not model, so it raises unless force_all_rays."""
+        dev = self.density_bitfield.device
+        if dev.type != "cuda":
+            raise _capi.GfppNoCpuPath("model is not on a CUDA device: libgfpp has no CPU path (call .cuda())")
+        if not force_all_rays and self.mean_count > 0:
+            raise ValueError(f"frozen_head: mean_count is {self.mean_count}: march_rays_train would cut rays to that sample budget "
+                             "(pass force_all_rays=True to give every ray max_steps samples)")
+        f32 = torch.float32
+        if not torch.is_tensor(rays_o) or not torch.is_tensor(rays_d) or rays_o.shape[-1] != 3 or rays_o.shape != rays_d.shape or rays_o.numel() == 0:
+            raise ValueError(f"rays_o and rays_d must both be [...,3] with the same shape, got {tuple(getattr(rays_o, 'shape', ()))} and "
+                             f"{tuple(getattr(rays_d, 'shape', ()))}")
+        if not torch.is_tensor(cond_feat) or cond_feat.numel() != self.cond_out_dim:
+            raise ValueError(f"cond_feat must hold one conditioning vector of {self.cond_out_dim} values")
+        dim = self.individual_embedding_dim
+        if (ind_code is None) != (dim == 0) or (ind_code is not None and (not torch.is_tensor(ind_code) or ind_code.numel() != dim)):
+            raise ValueError(f"ind_code must hold {dim} values (None iff the model has no individual codes)")
+        if not 1 <= int(max_steps) <= 4096:
+            raise ValueError(f"max_steps must be in 1..4096, got {max_steps}")
+        N = rays_o.numel() // 3
+        with torch.no_grad():
+            noise = torch.rand(N, dtype=f32, device=dev) if perturb else None
+            _, _, model, _ = self._ensure_packed()
+            L = _capi.lib()
+            ro = rays_o.detach().to(dev, f32).reshape(N, 3).contiguous()
+            rd = rays_d.detach().to(dev, f32).reshape(N, 3).contiguous()
+            c = cond_feat.detach().to(dev, f32).reshape(-1).contiguous()
+            code = ind_code.detach().to(dev, f32).reshape(-1).contiguous() if ind_code is not None else None
+            weights_sum = torch.empty(N, dtype=f32, device=dev)
+            image = torch.empty(N, 3, dtype=f32, device=dev)
+            need = L.gfpp_frozen_head_workspace_bytes(N, int(max_steps))
+            if need == 0:
+                raise _capi.GfppError(f"frozen_head does not support {N} rays")
+            ws = self.__dict__.get("_frozen_ws")
+            if ws is None or ws.numel() < need or ws.device != dev:
+                ws = self.__dict__["_frozen_ws"] = torch.empty(need, dtype=torch.uint8, device=dev)
+            with torch.cuda.device(dev):
+                _capi.check(L.gfpp_frozen_head(ctypes.byref(model), ro.data_ptr(), rd.data_ptr(), N, self._aabb_train_host(), c.data_ptr(),
+                                               None if code is None else code.data_ptr(), None if noise is None else noise.data_ptr(),
+                                               float(dt_gamma), int(max_steps), float(T_thresh), weights_sum.data_ptr(), image.data_ptr(),
+                                               ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_frozen_head")
+            self.last_launch_count = int(L.gfpp_last_launch_count())
+        return weights_sum, image
+
     # ------------------------------------------------------------------ the reference's render()
     trains_field = True   # render() has a training branch; the SR and torso subclasses do not
 

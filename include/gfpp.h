@@ -585,6 +585,30 @@ GFPP_API int gfpp_field_tc_backward(const gfpp_model_desc *desc, const float *xy
                                     float *grad_cond, float *grad_code, float *grad_position_table, float *grad_ambient_table,
                                     void *workspace, size_t workspace_bytes, void *stream);
 
+/* ------------------------------------------------------------------ (K) frozen head of the torso training steps
+ *
+ * The no-grad head block of the torso training step (radnerf_torso.py:92-150 and radnerf_torso_sr.py:150 under torch.no_grad):
+ * near_far_from_aabb + march_rays_train + RADNeRF.forward + composite_rays_train in one pass over the packed head model of
+ * gfpp_model_pack, for one frame of N rays.  It runs k_ray_setup and pass 1 of the head kernel of the model's mlp_precision, with
+ * composite_rays_train's termination: T is the running product of (1 - alpha), a ray stops after the sample that takes T below
+ * T_thresh, after max_steps samples, or when it leaves the volume.  Nothing is written to HBM per sample and the host is never
+ * synchronised.  Rays are slab-tested against the per-call `aabb` (host, xmin ymin zmin xmax ymax zmax; the torso steps pass
+ * aabb_train) with the model's min_near.  cond_feat: device [64].  code: device [ind_dim], the training row of
+ * individual_embeddings, folded into a copy of the colour-L0 bias in the workspace (the packed model is not written), or NULL;
+ * it must be given iff the model was packed with ind_dim > 0.  noises: device [N] in [0,1), march_rays_train's jittered starts
+ * (near + clamp(near * dt_gamma, dt_min, dt_max) * noise), or NULL for none.  Outputs: weights_sum [N] and the premultiplied head
+ * image [N,3] (before any background) -- composite_rays_train's first and fourth outputs; rays that miss the volume get zeros.
+ * There is no ambient_sum and no depth.  The sample budget of march_rays_train with mean_count > 0 is not modelled: every ray
+ * gets up to max_steps samples (force_all_rays).
+ * Validation (before any CUDA call): NULL pointers, a model handle not filled by gfpp_model_pack, N == 0, max_steps outside
+ * 1..4096, code given iff ind_dim > 0, aabb with min > max, a workspace below gfpp_frozen_head_workspace_bytes(N, max_steps)
+ * or not 256-byte aligned.  Stream-ordered, no host sync, deterministic.
+ * gfpp_frozen_head_workspace_bytes returns 0 for N == 0, N >= 2^31 or max_steps outside 1..4096. */
+GFPP_API size_t gfpp_frozen_head_workspace_bytes(uint32_t N, uint32_t max_steps);
+GFPP_API int gfpp_frozen_head(const gfpp_model *model, const float *rays_o, const float *rays_d, uint32_t N, const float aabb[6],
+                              const float *cond_feat, const float *code, const float *noises, float dt_gamma, uint32_t max_steps,
+                              float T_thresh, float *weights_sum, float *image, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,7 +7,9 @@ CUDA events around each leg, median over --iters after --warmup, on the syntheti
   * the same in eager PyTorch, fp32 (F.linear over train_ops.grid_encode with input gradients; TF32 off) and under fp16 autocast;
   * the same eager field over the reference's own grid kernels (oracle/_ref), when they were built;
   * the whole torso training step (oracle/torso_train.gfpp_train_step, the README recipe) at 65 536 rays, split into the head part
-    (marching, head field under no_grad, compositing) and the torso part (mask, forward_torso, composite, loss, backward).
+    (marching, head field under no_grad, compositing) and the torso part (mask, forward_torso, composite, loss, backward);
+  * that step and its head part with the head as one RADNeRF.frozen_head call against the composed head, in fp32 and fp16,
+    the legs alternating in one process (--rounds).
 The card's name and power limit are read in the same run.
 """
 import argparse
@@ -52,6 +54,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--rounds", type=int, default=3, help="alternating rounds of the frozen_head / composed legs")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -113,8 +116,61 @@ def main():
     out["step.head_part_ms@65536"] = timed(head_part, args.iters, args.warmup)
     out["step.torso_part_ms@65536"] = round(out["step_ms@65536"] - out["step.head_part_ms@65536"], 4)
     out["step.torso_pixels"] = holder["pixels"]
+
+    # the same step with its no-grad head block as one RADNeRF.frozen_head call (gfpp.h section K), against the composed head, in
+    # fp32 and fp16 (composed: the training field with train_precision "fp16"; frozen_head: mlp_precision "fp16").  The legs
+    # alternate, --rounds times, in this process; each number is the median over the rounds of the per-round medians.
+    def with_precision(prec, frozen, fn):
+        def run():
+            m.mlp_precision, m.train_precision = (prec, "fp32") if frozen else ("fp32", prec)
+            fn(frozen)
+        return run
+
+    def head_only(frozen):
+        f = frozen_train_step if frozen else tt.gfpp_train_step
+        holder["res"] = f(m, ro, rd, cond, bgc, pose6, idx, bgcol, 16, torso_field=_no_torso)
+
+    def full_step(frozen):
+        m.zero_grad(set_to_none=True)
+        res = (frozen_train_step if frozen else tt.gfpp_train_step)(m, ro, rd, cond, bgc, pose6, idx, bgcol, 16)
+        tt.task_loss(res, gt, tt.LAMBDA_WEIGHTS_ENTROPY).backward()
+
+    legs = {}
+    for prec in ("fp32", "fp16"):
+        for frozen in (False, True):
+            name = f"{'frozen_head' if frozen else 'composed'}.{prec}"
+            legs[f"{name}.step_ms@65536"] = with_precision(prec, frozen, full_step)
+            legs[f"{name}.head_part_ms@65536"] = with_precision(prec, frozen, head_only)
+    rounds = {k: [] for k in legs}
+    for _ in range(args.rounds):
+        for k, f in legs.items():
+            rounds[k].append(timed(f, args.iters, args.warmup))
+    m.mlp_precision, m.train_precision = "fp32", "fp32"
+    for k, v in rounds.items():
+        out[k] = sorted(v)[len(v) // 2]
+    for prec in ("fp32", "fp16"):
+        c, f = out[f"composed.{prec}.head_part_ms@65536"], out[f"frozen_head.{prec}.head_part_ms@65536"]
+        out[f"frozen_head.{prec}.head_part_speedup"] = round(c / f, 3)
     name, power = card()
     print(json.dumps({"tool": "torso_train_bench", "gpu": name, "power_limit": power, "iters": args.iters, "warmup": args.warmup, **out}))
+
+
+def frozen_train_step(model, rays_o, rays_d, cond, bg_coords, poses, index, bg_color, max_steps, torso_field=None):
+    """oracle/torso_train.gfpp_train_step with its no-grad head block replaced by one RADNeRF.frozen_head call."""
+    rays_o, rays_d, bg_coords = rays_o.reshape(-1, 3), rays_d.reshape(-1, 3), bg_coords.reshape(-1, 2)
+    with torch.no_grad():
+        cond_feat = model.cal_cond_feat(cond)
+    weights_sum, image = model.frozen_head(rays_o, rays_d, cond_feat, model.individual_embeddings[index], max_steps=max_steps)
+    mask = model.torso_mask(bg_coords)
+    N = rays_o.shape[0]
+    torso_alpha = torch.zeros(N, 1, device=rays_o.device)
+    torso_color = torch.zeros(N, 3, device=rays_o.device)
+    alpha, color, deform = (torso_field or model.forward_torso)(bg_coords[mask], poses, model.torso_individual_codes[index])
+    torso_alpha[mask] = alpha
+    torso_color[mask] = color
+    bg = torso_color * torso_alpha + bg_color.reshape(-1, 3) * (1 - torso_alpha)
+    rgb = (image + (1 - weights_sum).unsqueeze(-1) * bg).clamp(0, 1)
+    return {"torso_alpha_map": torso_alpha, "torso_rgb_map": bg, "rgb_map": rgb, "weights_sum": weights_sum, "deform": deform}
 
 
 def _autocast(f, x, p, c):
