@@ -320,15 +320,33 @@ class RADNeRF(nn.Module):
         d.has_torso = 0
         d.mlp_precision = MLP_PRECISIONS[self.mlp_precision]
 
-    def _ensure_packed(self):
+    def _head_pack_sources(self):
+        """Every tensor of the head field that _fill_desc reads.  The pack holds transposed, rounded or folded copies of them (the
+        colour-L0 bias folds individual_embeddings[0], the sigma-L2 geo rows fold into colour L0), so an in-place edit of any one
+        must rebuild it."""
+        ts = [self.density_bitfield, self.aabb_infer, self.position_embedder.embeddings, self.ambient_embedder.embeddings]
+        ts += [l.weight for net in (self.ambient_net, self.sigma_net, self.color_net) for l in net.net]
+        if self.individual_embedding_dim > 0:
+            ts.append(self.individual_embeddings)
+        return ts
+
+    def _torso_pack_sources(self):
+        """The tensors of the torso part of the pack (none for a head-only pack)."""
+        return []
+
+    def _ensure_packed(self, head_only=False):
+        """The packed model, rebuilt when anything it was packed from has changed.  head_only: the caller reads only the head
+        field (frozen_head), so a pack whose torso part is out of date still serves it; the torso training steps update the torso
+        weights in place every step and would otherwise repack the head with each one."""
         dev = self.density_bitfield.device
         if dev.type != "cuda":
             raise _capi.GfppError("model is not on a CUDA device: libgfpp has no CPU path (call .cuda())")
-        # in-place edits of the occupancy / tables / weights bump tensor._version: the packed copies are then rebuilt
-        vers = tuple(int(t._version) for t in (self.density_bitfield, self.position_embedder.embeddings, self.ambient_embedder.embeddings,
-                                               self.ambient_net.net[0].weight, self.sigma_net.net[0].weight, self.color_net.net[0].weight))
-        key = (float(self.density_scale), getattr(self, "mean_density_torso", None), dev.index, self.mlp_precision, vers)
-        if self._packed is not None and self._packed[0] == key:
+        # in-place edits bump tensor._version, and a replaced tensor has a new data_ptr: either rebuilds the packed copies
+        def vers(ts):
+            return tuple((t.data_ptr(), int(t._version)) for t in ts)
+        key = ((float(self.density_scale), dev.index, self.mlp_precision, vers(self._head_pack_sources())),
+               (getattr(self, "mean_density_torso", None), vers(self._torso_pack_sources())))
+        if self._packed is not None and (self._packed[0] == key or (head_only and self._packed[0][0] == key[0])):
             return self._packed
         L = _capi.lib()
         with torch.cuda.device(dev):
@@ -685,7 +703,7 @@ class RADNeRF(nn.Module):
         N = rays_o.numel() // 3
         with torch.no_grad():
             noise = torch.rand(N, dtype=f32, device=dev) if perturb else None
-            _, _, model, _ = self._ensure_packed()
+            _, _, model, _ = self._ensure_packed(head_only=True)
             L = _capi.lib()
             ro = rays_o.detach().to(dev, f32).reshape(N, 3).contiguous()
             rd = rays_d.detach().to(dev, f32).reshape(N, 3).contiguous()
@@ -989,12 +1007,12 @@ class _TorsoGrid:
         mean = self.refresh_torso_grid(cond, code, noise, decay)
         self.mean_density_torso = mean.item()
         self._set_torso_threshold(float(min(self.density_thresh_torso, self.mean_density_torso)))
-        # the head pack's cache key (RADNeRF._ensure_packed: density_scale, mean_density_torso, device, mlp_precision, versions)
-        # follows the new mean without a repack: RADNeRFTorso's handle has just been given the new threshold, and RADNeRFTorsowithSR
-        # packs the head field only (has_torso = 0), which the torso mean does not touch
+        # the head pack's cache key (RADNeRF._ensure_packed: head part, then (mean_density_torso, torso versions)) follows the new
+        # mean without a repack: RADNeRFTorso's handle has just been given the new threshold, and RADNeRFTorsowithSR packs the head
+        # field only (has_torso = 0), which the torso mean does not touch
         if self._packed is not None:
-            key, packed, model, keep = self._packed
-            self._packed = ((key[0], self.mean_density_torso) + key[2:], packed, model, keep)
+            (head_key, torso_key), packed, model, keep = self._packed
+            self._packed = ((head_key, (self.mean_density_torso,) + torso_key[1:]), packed, model, keep)
 
 
 class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
@@ -1372,6 +1390,13 @@ class RADNeRFTorso(_TorsoGrid, RADNeRF):
         # mean_density_torso is a plain attribute that is NOT in the checkpoint (=> 0 after load, radnerf_torso.py:22,167)
         d.density_thresh_torso = float(min(self.density_thresh_torso, self.mean_density_torso))
         d.torso_shrink = float(self.torso_shrink)
+
+    def _torso_pack_sources(self):
+        # density_grid_torso is read in place through its pointer (the refresh writes it there): not a packed copy
+        ts = [self.torso_embedder.embeddings] + [l.weight for l in self.torso_deform_net.net] + [l.weight for l in self.torso_canonicial_net.net]
+        if self.torso_individual_embedding_dim > 0:
+            ts.append(self.torso_individual_codes)
+        return ts
 
     def forward_torso(self, x, poses, c=None):
         """radnerf_torso.py:51-84 in libgfpp (fp32): x [n,2] in [-1,1], poses [1,6] (convert_poses of the head pose), c
