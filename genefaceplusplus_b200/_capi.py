@@ -106,6 +106,7 @@ EXPORTS = [
     "gfpp_torso_field_workspace_bytes", "gfpp_torso_field_forward", "gfpp_torso_field_backward",
     "gfpp_torso_sr_field_workspace_bytes", "gfpp_torso_sr_field_forward", "gfpp_torso_sr_field_backward",
     "gfpp_frozen_head_workspace_bytes", "gfpp_frozen_head",
+    "gfpp_grid_encode_forward_half", "gfpp_grid_encode_backward_half",
 ]
 
 
@@ -162,6 +163,8 @@ def lib():
         L.gfpp_composite_rays_train_backward.argtypes = [P, P, P, P, P, P, P, P, P, P, P, c_u32, c_u32, c_f, P, P, P, P]
         L.gfpp_grid_encode_forward_dydx.argtypes = [P, P, P, P, c_u32, c_u32, c_u32, c_u32, c_f, c_u32, P, c_u32, c_int, c_u32, P]
         L.gfpp_grid_encode_backward.argtypes = [P, P, P, P, P, c_u32, c_u32, c_u32, c_u32, c_f, c_u32, P, P, c_u32, c_int, c_u32, P]
+        L.gfpp_grid_encode_forward_half.argtypes = [P, P, P, P, c_u32, c_u32, c_u32, c_u32, c_f, c_u32, P, c_u32, c_int, c_u32, P]
+        L.gfpp_grid_encode_backward_half.argtypes = L.gfpp_grid_encode_backward.argtypes
         L.gfpp_grad_total_variation.argtypes = [P, P, P, P, c_f, c_u32, c_u32, c_u32, c_u32, c_f, c_u32, c_u32, c_int, P]
         L.gfpp_packbits.argtypes = [P, c_u32, c_f, P, P]
         L.gfpp_morton3D.argtypes = [P, c_u32, P, P]

@@ -6,8 +6,11 @@ wrappers run on libgfpp's per-op kernels.  Call `install()` before `import modul
 Inference exports: near_far_from_aabb, march_rays, composite_rays, grid_encode_forward, sh_encode_forward, freq_encode_forward.
 Training-side exports (SURVEY.md 8(f) rank 4; csrc/train_kernels.cu): march_rays_train(+_backward), composite_rays_train_forward /
 _backward, grid_encode_forward with dy_dx, grid_encode_backward, grad_total_variation, packbits, morton3D(+_invert, _dilation),
-sph_from_ray -- fp32 (run them with autocast disabled).  The input-gradient ops of the SH / frequency encoders (only needed when
-optimising camera poses through the view direction) still raise.
+sph_from_ray -- fp32.  Under autocast the reference hands the grid encoder half tables (grid.py:41-44, C = 2): grid_encode_forward
+and grid_encode_backward dispatch on the table's dtype like its AT_DISPATCH_FLOATING_TYPES_AND_HALF, fp32 to the fp32 ops of gfpp.h
+sections (A) / (D), half to the half ops of section (L); a half table with fp32 outputs (or any other mix) raises RuntimeError, as the
+reference's data_ptr<scalar_t>() does.  Every other op stays fp32 under autocast (custom_fwd(cast_inputs=torch.float32)).  The
+input-gradient ops of the SH / frequency encoders (only needed when optimising camera poses through the view direction) still raise.
 """
 import ctypes
 import sys
@@ -28,7 +31,7 @@ def _P(t, dtype=None):
         raise RuntimeError("libgfpp: expected a contiguous tensor")
     want = dtype if dtype is not None else _DTYPES.get(t.dtype)
     if want is None or t.dtype != want:
-        raise RuntimeError(f"libgfpp: unsupported dtype {t.dtype} (fp32 / int32 / uint8 buffers only; run the encoders with autocast disabled)")
+        raise RuntimeError(f"libgfpp: unsupported dtype {t.dtype} here (expected {want or 'fp32 / int32 / uint8'}; fp16 only for the grid encoder's half buffers)")
     return ctypes.c_void_p(t.data_ptr())
 
 
@@ -47,6 +50,14 @@ def _offsets_host(offsets):
             _OFFSETS_HOST.clear()
         hit = _OFFSETS_HOST[key] = (offsets, np.ascontiguousarray(offsets.detach().cpu().numpy().astype(np.int32)))
     return hit[1]
+
+
+def _all_half(what, **bufs):
+    """The half instantiation reads every 16-bit buffer as at::Half (gridencoder.cu:468, 497): one of another dtype is refused
+    before anything is launched, as the reference's data_ptr<scalar_t>() refuses it."""
+    for name, t in bufs.items():
+        if t is not None and (not torch.is_tensor(t) or t.dtype != torch.float16):
+            raise RuntimeError(f"{what}: {name} must be float16 with a float16 table (got {getattr(t, 'dtype', type(t))})")
 
 
 def _ck(rc, what):
@@ -105,8 +116,16 @@ def make_modules():
     ge = types.ModuleType("_gridencoder")
 
     def grid_encode_forward(inputs, emb, offsets, outputs, B, D, C, Lv, S_, H, dy_dx, gridtype, align_corners, interp):
+        if emb.dtype == torch.float16:   # autocast (grid.py:41-44): the reference's at::Half instantiation
+            _all_half("grid_encode_forward", outputs=outputs, dy_dx=dy_dx)
+            off = _offsets_host(offsets)
+            _ck(L.gfpp_grid_encode_forward_half(_P(inputs, torch.float32), _P(emb, torch.float16), off.ctypes.data_as(ctypes.c_void_p),
+                                                _P(outputs, torch.float16), B, D, C, Lv, cf(S_), H,
+                                                None if dy_dx is None else _P(dy_dx, torch.float16), gridtype, int(align_corners), interp, S()),
+                "grid_encode_forward")
+            return
         if emb.dtype != torch.float32:
-            raise RuntimeError("libgfpp grid tables are fp32 (run the encoder with autocast disabled)")
+            raise RuntimeError(f"libgfpp grid tables are fp32 or fp16, not {emb.dtype}")
         off = _offsets_host(offsets)
         if dy_dx is not None:   # calc_grad_inputs (grid.py:49-52): the ambient grid's input comes out of the ambient net
             _ck(L.gfpp_grid_encode_forward_dydx(_P(inputs, torch.float32), _P(emb), off.ctypes.data_as(ctypes.c_void_p), _P(outputs, torch.float32),
@@ -119,6 +138,15 @@ def make_modules():
     ge.grid_encode_forward = grid_encode_forward
 
     def grid_encode_backward(grad, inputs, emb, offsets, grad_emb, B, D, C, Lv, S_, H, dy_dx, grad_inputs, gridtype, align_corners, interp):
+        if grad.dtype == torch.float16 or emb.dtype == torch.float16:   # the half instantiation: every 16-bit buffer must be half
+            _all_half("grid_encode_backward", grad=grad, embeddings=emb, grad_embeddings=grad_emb, dy_dx=dy_dx, grad_inputs=grad_inputs)
+            off = _offsets_host(offsets)
+            _ck(L.gfpp_grid_encode_backward_half(_P(grad, torch.float16), _P(inputs, torch.float32), _P(emb, torch.float16),
+                                                 off.ctypes.data_as(ctypes.c_void_p), _P(grad_emb, torch.float16), B, D, C, Lv, cf(S_), H,
+                                                 None if dy_dx is None else _P(dy_dx, torch.float16),
+                                                 None if grad_inputs is None else _P(grad_inputs, torch.float16), gridtype, int(align_corners),
+                                                 interp, S()), "grid_encode_backward")
+            return
         off = _offsets_host(offsets)
         _ck(L.gfpp_grid_encode_backward(_P(grad, torch.float32), _P(inputs, torch.float32), _P(emb, torch.float32), off.ctypes.data_as(ctypes.c_void_p),
                                         _P(grad_emb, torch.float32), B, D, C, Lv, cf(S_), H, None if dy_dx is None else _P(dy_dx, torch.float32),

@@ -10,6 +10,7 @@
 #include "common.cuh"
 #include "field_train_kernel.cuh"
 #include "field_train_tc_kernel.cuh"
+#include "grid_half.cuh"
 #include "head_kernel.cuh"
 #include "launch.cuh"
 #include "sr_kernel.cuh"
@@ -1124,6 +1125,67 @@ int gfpp_grad_total_variation(const float *inputs, const float *embeddings, floa
         return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: D must be 2 or 3 and L <= 16%s");
     g_launches = 0;
     CK(launch_grad_tv(gm, inputs, embeddings, grad, weight, B, (cudaStream_t)stream));
+    return GFPP_OK;
+}
+
+// ---------------------------------------------------------------- (L) half-table grid encoder
+namespace {
+
+// the shape checks of the fp32 ops (fill_grid_meta: D, L, non-empty levels), then the raw level layout for the device
+int half_grid_args(HalfGridArgs &g, const int32_t *offsets, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, uint32_t gridtype,
+                   int align_corners, uint32_t interp) {
+    if (C != 2) return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: this build supports C == 2 only%s");
+    GridMeta gm;
+    if (fill_grid_meta(gm, offsets, D, L, S, H, gridtype, align_corners, interp) != 0)
+        return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: D must be 2 or 3 and L <= 16%s");
+    memset(&g, 0, sizeof(g));
+    for (uint32_t l = 0; l <= L; ++l) g.offset[l] = (uint32_t)offsets[l];
+    g.L = L;
+    g.S = S;
+    g.H = H;
+    g.gridtype = gridtype;
+    g.align_corners = align_corners ? 1u : 0u;
+    g.interp = interp;
+    return GFPP_OK;
+}
+
+bool misaligned4(const void *p) { return ((uintptr_t)p & 3u) != 0; }
+
+}  // namespace
+
+int gfpp_grid_encode_forward_half(const float *inputs, const uint16_t *embeddings, const int32_t *offsets_host, uint16_t *outputs,
+                                  uint32_t B, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, uint16_t *dy_dx, uint32_t gridtype,
+                                  int align_corners, uint32_t interp, void *stream) {
+    if (!inputs || !embeddings || !offsets_host || !outputs) return fail(GFPP_ERR_INVALID, "grid_encode_forward_half: null pointer%s");
+    HalfGridArgs g;
+    const int rc = half_grid_args(g, offsets_host, D, C, L, S, H, gridtype, align_corners, interp);
+    if (rc != GFPP_OK) return rc;
+    if (misaligned4(embeddings) || misaligned4(outputs) || misaligned4(dy_dx))
+        return fail(GFPP_ERR_INVALID, "grid_encode_forward_half: half2 buffers must be 4-byte aligned%s");
+    g_launches = 0;
+    if (B == 0) return GFPP_OK;
+    CK(launch_grid_half_forward(g, D, inputs, embeddings, outputs, dy_dx, B, (cudaStream_t)stream));
+    return GFPP_OK;
+}
+
+int gfpp_grid_encode_backward_half(const uint16_t *grad, const float *inputs, const uint16_t *embeddings, const int32_t *offsets_host,
+                                   uint16_t *grad_embeddings, uint32_t B, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H,
+                                   const uint16_t *dy_dx, uint16_t *grad_inputs, uint32_t gridtype, int align_corners, uint32_t interp,
+                                   void *stream) {
+    (void)embeddings;   // only its dtype matters to the reference (gridencoder.cu:497)
+    if (!grad || !inputs || !offsets_host || !grad_embeddings) return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: null pointer%s");
+    if ((dy_dx == nullptr) != (grad_inputs == nullptr))
+        return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: dy_dx and grad_inputs go together%s");
+    HalfGridArgs g;
+    const int rc = half_grid_args(g, offsets_host, D, C, L, S, H, gridtype, align_corners, interp);
+    if (rc != GFPP_OK) return rc;
+    if (misaligned4(grad) || misaligned4(grad_embeddings) || misaligned4(dy_dx))
+        return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: half2 buffers must be 4-byte aligned%s");
+    g_launches = 0;
+    if (B == 0) return GFPP_OK;
+    int nl = 0;
+    CKN(launch_grid_half_backward(g, D, grad, inputs, grad_embeddings, dy_dx, grad_inputs, B, &nl, (cudaStream_t)stream));
+    g_launches = nl;
     return GFPP_OK;
 }
 

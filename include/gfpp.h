@@ -41,6 +41,10 @@
  *  (I) the trainable torso-SR field: RADNeRFTorsowithSR.forward_torso and its backward at explicit points, fp32.
  *
  *  (J) the trainable head field of (G) on tensor cores: fp16 operands, fp32 accumulation, fp32 parameters and gradients.
+ *
+ *  (K) the frozen head of the torso training steps.
+ *
+ *  (L) the grid encoder ops of (A) and (D) on half tables, as the reference runs them under autocast.
  */
 #ifndef GFPP_H_
 #define GFPP_H_
@@ -608,6 +612,32 @@ GFPP_API size_t gfpp_frozen_head_workspace_bytes(uint32_t N, uint32_t max_steps)
 GFPP_API int gfpp_frozen_head(const gfpp_model *model, const float *rays_o, const float *rays_d, uint32_t N, const float aabb[6],
                               const float *cond_feat, const float *code, const float *noises, float dt_gamma, uint32_t max_steps,
                               float T_thresh, float *weights_sum, float *image, void *workspace, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------ (L) grid encoder on half tables
+ *
+ * The grid encoder's ops of (A) and (D) on IEEE binary16 tables, as the reference runs them under autocast (grid.py:41-44 casts
+ * tables with an even C to half): its scalar_t = at::Half instantiations of gridencoder.cu:87-368, argument for argument.  Every
+ * 16-bit buffer is a uint16_t array of binary16 bit patterns (embeddings, outputs, dy_dx, grad, grad_embeddings, grad_inputs),
+ * 4-byte aligned; inputs stay fp32 [B,D] in [0,1] and offsets_host is a HOST pointer as in (A).  C == 2, D in {2,3}, L <= 16.
+ * The arithmetic is the reference's: fp32 weights, a half running sum per output (each corner's term rounded to half, then the
+ * sum rounded to half, in the reference's corner order), the level constants from the device exp2f (scale = exp2f(level*S)*H - 1,
+ * unlike the host-side scale of the fp32 ops), round-to-nearest-even at every rounding site.
+ *
+ * gfpp_grid_encode_forward_half: outputs [L,B,2]; dy_dx [B,L,D,2] or NULL (calc_grad_inputs).  Inputs outside [0,1] give zeros.
+ * gfpp_grid_encode_backward_half: grad [L,B,2]; grad_embeddings [entries,2] (zero-initialised by the caller, grid.py:76) is
+ *   accumulated into with one f16x2 vector reduction (red.global.add.noftz.f16x2) per corner: each add rounds to half and the
+ *   order of the adds is free, as in the reference.  dy_dx [B,L,D,2] and grad_inputs [B,D]: both or neither; grad_inputs is
+ *   overwritten with the half running sum over (level, channel) of the half products grad * dy_dx.
+ * Validation (before any CUDA call): NULL pointers and dy_dx without grad_inputs -> GFPP_ERR_INVALID; C != 2, D outside {2,3},
+ * L outside 1..16 or an empty level -> GFPP_ERR_UNSUPPORTED; a 16-bit pair buffer not 4-byte aligned -> GFPP_ERR_INVALID.
+ * B == 0 returns GFPP_OK without touching the device. */
+GFPP_API int gfpp_grid_encode_forward_half(const float *inputs, const uint16_t *embeddings, const int32_t *offsets_host, uint16_t *outputs,
+                                           uint32_t B, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, uint16_t *dy_dx,
+                                           uint32_t gridtype, int align_corners, uint32_t interp, void *stream);
+GFPP_API int gfpp_grid_encode_backward_half(const uint16_t *grad, const float *inputs, const uint16_t *embeddings, const int32_t *offsets_host,
+                                            uint16_t *grad_embeddings, uint32_t B, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H,
+                                            const uint16_t *dy_dx, uint16_t *grad_inputs, uint32_t gridtype, int align_corners,
+                                            uint32_t interp, void *stream);
 
 #ifdef __cplusplus
 }
