@@ -168,12 +168,13 @@ struct ModelHost {
     const float *amb0_src;          // ambient_net.net.0.weight [128,96] (its conditioning columns are folded per frame)
     const float *color0_src;        // color_net.net.0.weight [128, 144 + ind_dim] (gfpp_frozen_head folds a per-call code into a copy of `narrow`)
     int ind_dim;
+    const unsigned char *tor_tf32;  // tf32 hi / lo images of the wide torso layers (k_epilogue)
 };
 static_assert(sizeof(ModelHost) <= sizeof(gfpp_model), "gfpp_model opaque storage too small");
 constexpr uint32_t kMagic = 0x67667070u;  // "gfpp"
 
 struct PackedLayout {
-    size_t wide, narrow, wd0, wd1, wd2, wc0, wc1, wc2, occ, coarse, tc_hi, tc_lo, v2_stream, v2_res, v2_step, pos_quads, amb_quads, total;
+    size_t wide, narrow, wd0, wd1, wd2, wc0, wc1, wc2, tor_tf32, occ, coarse, tc_hi, tc_lo, v2_stream, v2_res, v2_step, pos_quads, amb_quads, total;
 };
 
 // tensor-core weight stream: kHeadTcChunks (head_kernel.cuh)
@@ -200,6 +201,7 @@ PackedLayout packed_layout(uint32_t cascade = 8, uint32_t grid_size = 128, size_
     L.wc0 = take(76 * 32);
     L.wc1 = take(32 * 32);
     L.wc2 = take(4 * 32);
+    L.tor_tf32 = take(TORSO_TF32_BYTES / 4);
     L.occ = take(8);
     L.coarse = take(coarse_words_for(cascade, grid_size));
     size_t tcb = 0;
@@ -592,6 +594,9 @@ int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes,
         CK(launch_pack_kmajor(d->torso_canon_w[0], 32 + din, 0, 0, 32, 74, 76, wc0, st));
         CK(launch_pack_kmajor(d->torso_canon_w[1], 32, 0, 0, 32, 32, 32, wc1, st));
         CK(launch_pack_rows(d->torso_canon_w[2], 32, 0, 4, 32, 32, wc2, st));
+        CK(launch_pack_tf32(d->torso_deform_w[0], din, d->torso_deform_w[1], d->torso_canon_w[0], 32 + din, d->torso_canon_w[1],
+                            (unsigned char *)(base + L.tor_tf32), st));
+        m.tor_tf32 = (const unsigned char *)(base + L.tor_tf32);
         m.wd0 = wd0; m.wd1 = wd1; m.wd2 = wd2; m.wc0 = wc0; m.wc1 = wc1; m.wc2 = wc2;
         m.torso_def0_src = d->torso_deform_w[0];
         m.torso_can0_src = d->torso_canon_w[0];
@@ -691,6 +696,7 @@ int gfpp_render_frames(const gfpp_model *model, const gfpp_frames *fr, const gfp
     if (m.has_torso) {
         t.tor_gm = m.tor_gm; t.tor_tab = m.tor_tab;
         t.w_def0 = m.wd0; t.w_def1 = m.wd1; t.w_def2 = m.wd2; t.w_can0 = m.wc0; t.w_can1 = m.wc1; t.w_can2 = m.wc2;
+        t.w_tf32 = m.tor_tf32;
         t.bias_def = (float *)(ws + W.bias_def); t.bias_can = (float *)(ws + W.bias_can);
         t.pose6 = fr->torso_pose6;
         t.density_grid_torso = m.density_grid_torso; t.grid_size = (int)m.grid_size;

@@ -206,5 +206,45 @@ template <> __device__ __forceinline__ void wgmma_tn<128>(float (&d)[64], uint64
 }
 #undef GFPP_ACC8
 
+// ---- tf32 operands: D[64 x N] (+)= A[64 x 8] * W[N x 8]^T, one k-step of 8 (32 bytes of each row) ----
+// W (smem, K-major) as no-swizzle K8 blocks: a k-step of 4-byte elements has the byte geometry of a K16 tile of 2-byte
+// elements (two 16-byte K chunks 128 B apart, 8-row groups 256 B apart), so one block of N rows is N * 32 bytes and element
+// (n, k) sits at k16_off(n, k / 4) + 4 * (k % 4).  Unlike SW128, a K extent of 48 or 80 needs no padding to 32-element rows.
+// A comes from registers (tf32 is the one 4-byte type wgmma accepts there): lane l of warp w holds rows 16w + l/4 (a0, a2)
+// and 16w + l/4 + 8 (a1, a3), K columns l%4 (a0, a1) and l%4 + 4 (a2, a3).  Values are tf32 bit patterns (rna_tf32).
+__device__ __forceinline__ uint64_t desc_tf32_k8(uint32_t saddr) { return desc_k16(saddr); }
+__device__ __forceinline__ uint32_t rna_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r;
+}
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t acc);
+#define GFPP_ACC8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+template <> __device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\twgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+                 : GFPP_ACC8(0), GFPP_ACC8(8) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\twgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+                 : GFPP_ACC8(0), GFPP_ACC8(8), GFPP_ACC8(16), GFPP_ACC8(24) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+}
+#undef GFPP_ACC8
+// split tf32 over K steps: D = A_lo W_hi + A_hi W_lo + A_hi W_hi (the small products first), fp32 accumulation.
+// W_hi / W_lo: K8 blocks of N rows, block j at + j * N * 32 bytes.  `acc_first` = 0 starts a new accumulation.  Issues and
+// commits one group; the caller waits.
+template <int N, int KS>
+__device__ __forceinline__ void wgmma_tf32x3(float (&d)[N / 2], const uint32_t (&ahi)[KS][4], const uint32_t (&alo)[KS][4],
+                                             uint32_t w_hi, uint32_t w_lo, uint32_t acc_first) {
+    wg_fence();
+#pragma unroll
+    for (int j = 0; j < KS; ++j) wgmma_tf32<N>(d, alo[j], desc_tf32_k8(w_hi + (uint32_t)(j * N * 32)), j > 0 ? 1u : acc_first);
+#pragma unroll
+    for (int j = 0; j < KS; ++j) wgmma_tf32<N>(d, ahi[j], desc_tf32_k8(w_lo + (uint32_t)(j * N * 32)), 1u);
+#pragma unroll
+    for (int j = 0; j < KS; ++j) wgmma_tf32<N>(d, ahi[j], desc_tf32_k8(w_hi + (uint32_t)(j * N * 32)), 1u);
+    wg_commit();
+}
+
 }  // namespace tc
 }  // namespace gfpp

@@ -1,6 +1,6 @@
-// torso_common.cuh -- device helpers shared by the torso epilogues (torso_kernel.cu: radnerf_torso.py field;
-// torso_sr_kernel.cu: radnerf_torso_sr.py field): frequency-encoder entries, small FFMA tile GEMMs out of shared memory,
-// grid_sample restated.
+// torso_common.cuh -- device helpers shared by the torso kernels (torso_kernel.cu: radnerf_torso.py field; torso_sr_kernel.cu:
+// radnerf_torso_sr.py field; the grid query and the training fields): frequency-encoder entries, small FFMA tile GEMMs out of
+// shared memory (all of them but k_epilogue, which runs its MLPs on the tensor cores), grid_sample restated.
 #pragma once
 #include "common.cuh"
 

@@ -6,32 +6,109 @@
 // pixel skip the MLPs.  Per-frame constants (freq-encoded pose, torso code) are folded into per-frame
 // bias vectors by k_torso_frame_bias, so the per-pixel GEMMs only see the pixel-dependent columns
 // (deform: 42 of 104, canonical: 74 of 136).
+//
+// The four wide layers (deform 48->64->64, canonical 80->32->32) run on the tensor cores in split tf32 in every precision
+// mode: x = hi + lo with hi = rna_tf32(x), lo = rna_tf32(x - hi) (~21-22 bits at every magnitude: tf32 keeps fp32's
+// exponent), D = A_lo W_hi + A_hi W_lo + A_hi W_hi with fp32 accumulation (tc.cuh, wgmma_tf32x3).  Warpgroup g owns the
+// tile's rows 64g..64g+63 (M = 64); the weights' tf32 hi / lo images (84 KB, torso_kernel.cuh) stay resident in shared
+// memory, filled once by one bulk copy.  The A operand comes from REGISTERS, in the wgmma fragment layout: lane l of warp w
+// holds rows r0 = 16w + l/4 and r1 = r0 + 8, and K positions q = l%4 and q + 4 of every k-step.  So each thread computes
+// its own input features (enc_x entries q, q+4 mod 8 of both rows: ~10 accurate sinf per row; grid levels q, q+4, q+8, q+12
+// of both rows) and a layer's accumulator fragment is the next layer's A operand without leaving the registers: the
+// thread holds columns 8j + 2q, 8j + 2q + 1 of k-step j, so the packed weights take their K rows in that order
+// (k_pack_tf32).  The bias + ReLU epilogues run on the fragments; the narrow outputs (deform 64->2, whose value IS
+// `deform` and moves the canonical lookup; canonical 32->4 into the sigmoids) are fp32 dot products of the fragments,
+// summed over the quad that shares the rows.  enc_x's A values are kept in shared memory (one column per thread) for the
+// canonical net, whose K order [enc_x 42 | 0 x 6 | grid 32] starts with deform L0's.  Every row's arithmetic reads only
+// that row, so a pixel's result does not depend on the other pixels of its tile or on the tile-to-CTA schedule.
+// Budget: 112.5 KB of shared memory and <= 128 registers per thread, two CTAs (16 warps) per SM.
 #include "common.cuh"
 #include "launch.cuh"
+#include "tc.cuh"
 #include "torso_common.cuh"
 #include "torso_kernel.cuh"
 
 namespace gfpp {
 
 using namespace torsoc;
+using namespace tc;
 
 namespace {
 
 constexpr int TP = 128;    // pixels per tile
 constexpr int NT = 256;
-constexpr int LDT = 84;    // A-tile stride (>= 76, 16B aligned, 84 % 32 = 20)
-constexpr int LDE = 44;    // enc_x copy stride
-constexpr int KD0 = 44, KC0 = 76;
+constexpr int NEX = 24;    // enc_x A values of a thread: 6 k-steps x 4
 
 struct Smem {
-    float A[TP * LDT];
-    float E[TP * LDE];
-    float wd0[KD0 * 64], wd1[64 * 64], wc0[KC0 * 32], wc1[32 * 32];
+    unsigned char w[TORSO_TF32_BYTES];   // tf32 hi / lo images of the wide layers (bulk copy; descriptors want 16-byte alignment)
+    float ex[NEX][NT];                   // enc_x A values, one column per thread
     float wd2[2 * 64], wc2[4 * 32];
-    float x2[2 * TP];
     float alpha[TP], col[3 * TP], dxy[2 * TP];
     int mask[TP];
+    unsigned long long bar;
 };
+
+// freq_entry(x, 2, c) with the coordinate picked by a select: c depends on the lane here, and an indexed x would live in
+// local memory.  Same operations, same value.
+__device__ __forceinline__ float enc_x_entry(const float (&x)[2], int c) {
+    const int d = c & 1;
+    const float xd = d ? x[1] : x[0];
+    if (c < 2) return xd;
+    const int col = c / 2 - 1, f = col / 2;
+    return sinf(__fadd_rn(scalbnf(xd, f), (float)(col % 2) * (3.141592653589793f / 2)));
+}
+
+// one k-step of A values -> tf32 hi / lo fragments
+__device__ __forceinline__ void split_tf32(const float (&v)[4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        hi[e] = rna_tf32(v[e]);
+        lo[e] = rna_tf32(v[e] - __uint_as_float(hi[e]));
+    }
+}
+
+// ReLU(acc + bias) of an M = 64, N-wide accumulator fragment -> the next layer's A fragments (K order of k_pack_tf32)
+template <int N>
+__device__ __forceinline__ void relu_to_a(const float (&d)[N / 2], const float *__restrict__ bias, int q, uint32_t (&hi)[N / 8][4],
+                                          uint32_t (&lo)[N / 8][4]) {
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+        const int c = 8 * j + 2 * q;
+        const float b0 = bias ? __ldg(bias + c) : 0.f, b1 = bias ? __ldg(bias + c + 1) : 0.f;
+        const float v[4] = {fmaxf(d[4 * j] + b0, 0.f), fmaxf(d[4 * j + 2] + b0, 0.f), fmaxf(d[4 * j + 1] + b1, 0.f),
+                            fmaxf(d[4 * j + 3] + b1, 0.f)};
+        split_tf32(v, hi[j], lo[j]);
+    }
+}
+
+// O-wide fp32 output layer of ReLU(acc) (no bias): out[r][o] for the thread's rows r0 (r = 0) and r1 (r = 1); every lane of
+// the quad ends with the same sums
+template <int N, int O>
+__device__ __forceinline__ void narrow_out(const float (&d)[N / 2], const float *__restrict__ w /*smem [O][N]*/, int q, float (&out)[2][O]) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int o = 0; o < O; ++o) out[r][o] = 0.f;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int c = 8 * j + 2 * q + e;
+            const float h0 = fmaxf(d[4 * j + e], 0.f), h1 = fmaxf(d[4 * j + 2 + e], 0.f);
+#pragma unroll
+            for (int o = 0; o < O; ++o) {
+                out[0][o] = fmaf(h0, w[o * N + c], out[0][o]);
+                out[1][o] = fmaf(h1, w[o * N + c], out[1][o]);
+            }
+        }
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int o = 0; o < O; ++o) {
+            out[r][o] += __shfl_xor_sync(0xffffffffu, out[r][o], 1);
+            out[r][o] += __shfl_xor_sync(0xffffffffu, out[r][o], 2);
+        }
+}
 
 }  // namespace
 
@@ -65,16 +142,21 @@ __global__ void __launch_bounds__(256, 2) k_epilogue(const __grid_constant__ Tor
     const int tiles_per_frame = (a.n_rays + TP - 1) / TP;
     const int n_tiles = a.n_frames * tiles_per_frame;
     if (a.has_torso) {
-        for (int i = tid; i < KD0 * 64; i += NT) s.wd0[i] = a.w_def0[i];
-        for (int i = tid; i < 64 * 64; i += NT) s.wd1[i] = a.w_def1[i];
-        for (int i = tid; i < KC0 * 32; i += NT) s.wc0[i] = a.w_can0[i];
-        for (int i = tid; i < 32 * 32; i += NT) s.wc1[i] = a.w_can1[i];
+        if (tid == 0) {
+            mbar_init(&s.bar, 1);
+            mbar_fence_init();
+            mbar_expect_tx(&s.bar, TORSO_TF32_BYTES);
+            bulk_g2s(s.w, a.w_tf32, TORSO_TF32_BYTES, &s.bar);
+        }
         for (int i = tid; i < 2 * 64; i += NT) s.wd2[i] = a.w_def2[i];
         for (int i = tid; i < 4 * 32; i += NT) s.wc2[i] = a.w_can2[i];
     }
     __syncthreads();
-    const int ty = tid >> 4, tx = tid & 15;
-    const int slot = tid & (TP - 1), lg = tid >> 7;
+    bool w_ready = false;
+    const int slot = tid & (TP - 1);
+    // MMA-phase rows of this thread (tc.cuh: tf32 A fragment)
+    const int r0 = 64 * (tid >> 7) + 16 * ((tid >> 5) & 3) + ((tid & 31) >> 2), r1 = r0 + 8;
+    const uint32_t w_base = smem_u32(s.w);
 
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int f = tile / tiles_per_frame;
@@ -89,90 +171,103 @@ __global__ void __launch_bounds__(256, 2) k_epilogue(const __grid_constant__ Tor
         if (tid < TP) s.mask[tid] = m;
         const int any = __syncthreads_or(m);
         if (any) {
-            // ---- enc_x = freq10(shrink * bg_coord) -> E[:, 0:42] and A[:, 0:42]; pad cols 42,43 = 0 ----
-            {
-                float x[2] = {0.f, 0.f};
-                if (in_range) { x[0] = __fmul_rn(a.bg_coords[2 * n], a.torso_shrink); x[1] = __fmul_rn(a.bg_coords[2 * n + 1], a.torso_shrink); }
-                for (int c = lg * 22; c < lg * 22 + 22; ++c) {
-                    const float v = c < 42 ? freq_entry(x, 2, c) : 0.f;
-                    s.E[slot * LDE + c] = v;
-                    s.A[slot * LDT + c] = v;
-                }
-                if (lg == 0) { s.x2[slot] = x[0]; s.x2[TP + slot] = x[1]; }
-            }
-            __syncthreads();
-            // ---- deform net 104 -> 64 -> 64 -> 2 (radnerf_torso.py:60-76) ----
-            {
-                float acc[8][4] = {};
-                small_gemm<4, KD0, LDT>(acc, s.A, s.wd0, ty, tx);
-                __syncthreads();
-                store_relu<4, LDT>(acc, s.A, a.bias_def + (size_t)f * 64, ty, tx);
-                __syncthreads();
-            }
-            {
-                float acc[8][4] = {};
-                small_gemm<4, 64, LDT>(acc, s.A, s.wd1, ty, tx);
-                __syncthreads();
-                store_relu<4, LDT>(acc, s.A, nullptr, ty, tx);
-                __syncthreads();
-            }
-            {
-                const int row = tid >> 1, half = tid & 1;
-                float v0 = 0.f, v1 = 0.f;
-                for (int k = half * 32; k < half * 32 + 32; ++k) {
-                    const float xk = s.A[row * LDT + k];
-                    v0 = fmaf(xk, s.wd2[k], v0);
-                    v1 = fmaf(xk, s.wd2[64 + k], v1);
-                }
-                v0 += __shfl_xor_sync(0xffffffffu, v0, 1);
-                v1 += __shfl_xor_sync(0xffffffffu, v1, 1);
-                if (half == 0) {
-                    s.dxy[row] = v0; s.dxy[TP + row] = v1;
-                    // x = (x + dx).clamp(-1, 1)
-                    s.x2[row] = fminf(fmaxf(s.x2[row] + v0, -1.f), 1.f);
-                    s.x2[TP + row] = fminf(fmaxf(s.x2[TP + row] + v1, -1.f), 1.f);
-                }
-            }
-            __syncthreads();
-            // ---- canonical input: [tiled2D(x) 32 | enc_x 42 | pad 2] ----
-            {
-                const float u = __fdiv_rn(__fadd_rn(s.x2[slot], 1.0f), 2.0f), v = __fdiv_rn(__fadd_rn(s.x2[TP + slot], 1.0f), 2.0f);
-#pragma unroll 2
-                for (int l = lg * 8; l < lg * 8 + 8; ++l)
-                    *reinterpret_cast<float2 *>(s.A + slot * LDT + 2 * l) = grid_lookup2(a.tor_gm, a.tor_tab, l, u, v);
-                for (int c = lg * 22; c < lg * 22 + 22; ++c) s.A[slot * LDT + 32 + c] = s.E[slot * LDE + c];
-            }
-            __syncthreads();
-            // ---- canonical net 136 -> 32 -> 32 -> 4, sigmoid (radnerf_torso.py:77-82) ----
-            {
-                float acc[8][2] = {};
-                small_gemm<2, KC0, LDT>(acc, s.A, s.wc0, ty, tx);
-                __syncthreads();
-                store_relu<2, LDT>(acc, s.A, a.bias_can + (size_t)f * 32, ty, tx);
-                __syncthreads();
-            }
-            {
-                float acc[8][2] = {};
-                small_gemm<2, 32, LDT>(acc, s.A, s.wc1, ty, tx);
-                __syncthreads();
-                store_relu<2, LDT>(acc, s.A, nullptr, ty, tx);
-                __syncthreads();
-            }
-            {
-                const int row = tid >> 1, half = tid & 1;
-                float v[4] = {0.f, 0.f, 0.f, 0.f};
-                for (int k = half * 16; k < half * 16 + 16; ++k) {
-                    const float xk = s.A[row * LDT + k];
+            if (!w_ready) { mbar_wait(&s.bar, 0); w_ready = true; }
+            // K position of the thread's A values, read here: hoisted out of the tile loop, the per-column constants derived
+            // from it (frequency, phase, bias and weight offsets) would not fit the register budget beside the fragments
+            int q;
+            asm volatile("mov.u32 %0, %%laneid;" : "=r"(q));
+            q &= 3;
+            // x = shrink * bg_coord of rows r0, r1
+            float x[2][2];
 #pragma unroll
-                    for (int o = 0; o < 4; ++o) v[o] = fmaf(xk, s.wc2[o * 32 + k], v[o]);
-                }
+            for (int r = 0; r < 2; ++r) {
+                const int nr = n0 + (r ? r1 : r0);
+                x[r][0] = x[r][1] = 0.f;
+                if (nr < a.n_rays) { x[r][0] = __fmul_rn(a.bg_coords[2 * nr], a.torso_shrink); x[r][1] = __fmul_rn(a.bg_coords[2 * nr + 1], a.torso_shrink); }
+            }
+            // ---- deform net 104 -> 64 -> 64 -> 2 (radnerf_torso.py:60-76); L0's A = enc_x = freq10(x) [42 | 0 x 6] ----
+            float dd[2][2];
+            {
 #pragma unroll
-                for (int o = 0; o < 4; ++o) v[o] += __shfl_xor_sync(0xffffffffu, v[o], 1);
-                if (half == 0) {
-                    s.alpha[row] = 1.0f / (1.0f + expf(-v[0]));
-                    s.col[row] = 1.0f / (1.0f + expf(-v[1]));
-                    s.col[TP + row] = 1.0f / (1.0f + expf(-v[2]));
-                    s.col[2 * TP + row] = 1.0f / (1.0f + expf(-v[3]));
+                for (int j = 0; j < 6; ++j) {
+                    const int k0 = 8 * j + q, k1 = k0 + 4;
+                    s.ex[4 * j][tid] = k0 < 42 ? enc_x_entry(x[0], k0) : 0.f;
+                    s.ex[4 * j + 1][tid] = k0 < 42 ? enc_x_entry(x[1], k0) : 0.f;
+                    s.ex[4 * j + 2][tid] = k1 < 42 ? enc_x_entry(x[0], k1) : 0.f;
+                    s.ex[4 * j + 3][tid] = k1 < 42 ? enc_x_entry(x[1], k1) : 0.f;
+                }
+                // split after the sinf: the hi / lo fragments are not live across its slow path
+                uint32_t ahi[6][4], alo[6][4];
+#pragma unroll
+                for (int j = 0; j < 6; ++j) {
+                    const float ev[4] = {s.ex[4 * j][tid], s.ex[4 * j + 1][tid], s.ex[4 * j + 2][tid], s.ex[4 * j + 3][tid]};
+                    split_tf32(ev, ahi[j], alo[j]);
+                }
+                float d[32];
+                wgmma_tf32x3<64, 6>(d, ahi, alo, w_base + TORSO_TF32_D0.hi, w_base + TORSO_TF32_D0.hi + 64 * 48 * 4, 0u);
+                wg_wait<0>();
+                acc_fence(d);
+                uint32_t hhi[8][4], hlo[8][4];
+                relu_to_a<64>(d, a.bias_def + (size_t)f * 64, q, hhi, hlo);
+                wgmma_tf32x3<64, 8>(d, hhi, hlo, w_base + TORSO_TF32_D1.hi, w_base + TORSO_TF32_D1.hi + 64 * 64 * 4, 0u);
+                wg_wait<0>();
+                acc_fence(d);
+                narrow_out<64, 2>(d, s.wd2, q, dd);
+            }
+            // x = (x + dx).clamp(-1, 1)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                x[r][0] = fminf(fmaxf(x[r][0] + dd[r][0], -1.f), 1.f);
+                x[r][1] = fminf(fmaxf(x[r][1] + dd[r][1], -1.f), 1.f);
+            }
+            if (q == 0) {
+                s.dxy[r0] = dd[0][0]; s.dxy[TP + r0] = dd[0][1];
+                s.dxy[r1] = dd[1][0]; s.dxy[TP + r1] = dd[1][1];
+            }
+            // ---- canonical net 136 -> 32 -> 32 -> 4, sigmoid (radnerf_torso.py:77-82); L0's A = [enc_x 42 | 0 x 6 | grid 32] ----
+            {
+                // K block [enc_x | 0 x 6] first: its MMAs run while the grid lookups below wait on memory
+                float c[16];
+                uint32_t ahi[6][4], alo[6][4];
+#pragma unroll
+                for (int j = 0; j < 6; ++j) {
+                    const float ev[4] = {s.ex[4 * j][tid], s.ex[4 * j + 1][tid], s.ex[4 * j + 2][tid], s.ex[4 * j + 3][tid]};
+                    split_tf32(ev, ahi[j], alo[j]);
+                }
+                wgmma_tf32x3<32, 6>(c, ahi, alo, w_base + TORSO_TF32_C0.hi, w_base + TORSO_TF32_C0.hi + 32 * 80 * 4, 0u);
+                float u[2], v[2];
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    u[r] = __fdiv_rn(__fadd_rn(x[r][0], 1.0f), 2.0f);
+                    v[r] = __fdiv_rn(__fadd_rn(x[r][1], 1.0f), 2.0f);
+                }
+                uint32_t ghi[4][4], glo[4][4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {   // k-step 6 + j: level 4j + q, both features, of both rows
+                    const float2 g0 = grid_lookup2(a.tor_gm, a.tor_tab, 4 * j + q, u[0], v[0]);
+                    const float2 g1 = grid_lookup2(a.tor_gm, a.tor_tab, 4 * j + q, u[1], v[1]);
+                    const float gv[4] = {g0.x, g1.x, g0.y, g1.y};
+                    split_tf32(gv, ghi[j], glo[j]);
+                }
+                wgmma_tf32x3<32, 4>(c, ghi, glo, w_base + TORSO_TF32_C0.hi + 6 * 32 * 32, w_base + TORSO_TF32_C0.hi + 32 * 80 * 4 + 6 * 32 * 32, 1u);
+                wg_wait<0>();
+                acc_fence(c);
+                uint32_t hhi[4][4], hlo[4][4];
+                relu_to_a<32>(c, a.bias_can + (size_t)f * 32, q, hhi, hlo);
+                wgmma_tf32x3<32, 4>(c, hhi, hlo, w_base + TORSO_TF32_C1.hi, w_base + TORSO_TF32_C1.hi + 32 * 32 * 4, 0u);
+                wg_wait<0>();
+                acc_fence(c);
+                float o[2][4];
+                narrow_out<32, 4>(c, s.wc2, q, o);
+                if (q == 0) {
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        const int row = r ? r1 : r0;
+                        s.alpha[row] = 1.0f / (1.0f + expf(-o[r][0]));
+                        s.col[row] = 1.0f / (1.0f + expf(-o[r][1]));
+                        s.col[TP + row] = 1.0f / (1.0f + expf(-o[r][2]));
+                        s.col[2 * TP + row] = 1.0f / (1.0f + expf(-o[r][3]));
+                    }
                 }
             }
             __syncthreads();
@@ -205,6 +300,9 @@ __global__ void __launch_bounds__(256, 2) k_epilogue(const __grid_constant__ Tor
         }
         __syncthreads();
     }
+    // the weight copy must land before the CTA exits, also when none of its tiles had a torso pixel: its shared memory is
+    // released at exit and may already belong to the next CTA on this SM
+    if (a.has_torso && !w_ready) mbar_wait(&s.bar, 0);
 }
 
 // dst[k][n] = src[(row0 + n) * ld + col0 + k] for k < K, zero for K <= k < Kpad   (k-major repack of nn.Linear weights)
@@ -213,6 +311,36 @@ __global__ void k_pack_kmajor(const float *__restrict__ src, int ld, int row0, i
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Kpad * N; i += gridDim.x * blockDim.x) {
         const int k = i / N, n = i - k * N;
         dst[i] = k < K ? src[(size_t)(row0 + n) * ld + col0 + k] : 0.f;
+    }
+}
+
+// source column of K position k of tf32 torso layer `layer` (0 deform L0, 1 deform L1, 2 canonical L0, 3 canonical L1), -1 for
+// a zero row.  Accumulator-fragment order inside every 8 (the grid block and the hidden layers): position p < 4 takes column
+// 2p, position p >= 4 takes column 2(p - 4) + 1.
+__device__ __forceinline__ int tf32_src_col(int layer, int k) {
+    const int p = k & 7, perm = (k & ~7) + (p < 4 ? 2 * p : 2 * p - 7);
+    if (layer == 0) return k < 42 ? k : -1;
+    if (layer == 2) return k < 42 ? 32 + k : k < 48 ? -1 : perm - 48;   // [enc_x = source columns 32..73 | 0 x 6 | grid 0..31]
+    return perm;
+}
+
+// tf32 hi / lo images of the four wide torso layers (torso_kernel.cuh layout) from the nn.Linear weights [out, in]
+__global__ void k_pack_tf32(const float *__restrict__ w_def0, int ld_def0, const float *__restrict__ w_def1,
+                            const float *__restrict__ w_can0, int ld_can0, const float *__restrict__ w_can1, unsigned char *__restrict__ dst) {
+    constexpr int n_el = 64 * 48 + 64 * 64 + 32 * 80 + 32 * 32;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_el; i += gridDim.x * blockDim.x) {
+        int layer = 0, r = i, N = 64, K = 48, hi = TORSO_TF32_D0.hi, ld = ld_def0;
+        const float *src = w_def0;
+        if (r >= 64 * 48) { r -= 64 * 48; layer = 1; K = 64; hi = TORSO_TF32_D1.hi; ld = 64; src = w_def1;
+            if (r >= 64 * 64) { r -= 64 * 64; layer = 2; N = 32; K = 80; hi = TORSO_TF32_C0.hi; ld = ld_can0; src = w_can0;
+                if (r >= 32 * 80) { r -= 32 * 80; layer = 3; K = 32; hi = TORSO_TF32_C1.hi; ld = 32; src = w_can1; } } }
+        const int n = r / K, k = r - n * K;
+        const int c = tf32_src_col(layer, k);
+        const float w = c >= 0 ? src[(size_t)n * ld + c] : 0.f;
+        const uint32_t h = rna_tf32(w), l = rna_tf32(w - __uint_as_float(h));
+        const uint32_t off = (uint32_t)((k >> 3) * N * 32) + k16_off(n, (k & 7) >> 2) + 4u * (uint32_t)(k & 3);
+        *reinterpret_cast<uint32_t *>(dst + hi + off) = h;
+        *reinterpret_cast<uint32_t *>(dst + hi + N * K * 4 + off) = l;
     }
 }
 
@@ -256,6 +384,11 @@ cudaError_t launch_epilogue(const TorsoArgs &a, cudaStream_t st) {
 
 cudaError_t launch_pack_kmajor(const float *src, int ld, int row0, int col0, int N, int K, int Kpad, float *dst, cudaStream_t st) {
     k_pack_kmajor<<<grid_for((uint64_t)Kpad * N, 256), 256, 0, st>>>(src, ld, row0, col0, N, K, Kpad, dst);
+    return cudaGetLastError();
+}
+cudaError_t launch_pack_tf32(const float *w_def0, int ld_def0, const float *w_def1, const float *w_can0, int ld_can0,
+                             const float *w_can1, unsigned char *dst, cudaStream_t st) {
+    k_pack_tf32<<<grid_for(64 * 48 + 64 * 64 + 32 * 80 + 32 * 32, 256), 256, 0, st>>>(w_def0, ld_def0, w_def1, w_can0, ld_can0, w_can1, dst);
     return cudaGetLastError();
 }
 cudaError_t launch_pack_rows(const float *src, int ld, int row0, int n_rows, int K, int dst_ld, float *dst, cudaStream_t st) {
