@@ -85,7 +85,7 @@ class TorsoSrFrames(ctypes.Structure):
 class Outputs(ctypes.Structure):
     _fields_ = [("rgb_map", c_void_p), ("depth_map", c_void_p), ("weights_sum", c_void_p),
                 ("torso_alpha_map", c_void_p), ("torso_rgb_map", c_void_p), ("torso_deform", c_void_p),
-                ("stats", c_void_p), ("rgb_u8", c_void_p)]
+                ("stats", c_void_p), ("rgb_u8", c_void_p), ("alpha_map", c_void_p), ("rgba_u8", c_void_p)]
 
 
 EXPORTS = [

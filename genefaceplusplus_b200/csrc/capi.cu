@@ -634,7 +634,8 @@ int gfpp_render_frames(const gfpp_model *model, const gfpp_frames *fr, const gfp
     ModelHost m;
     memcpy(&m, model, sizeof(m));
     if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "render_frames: model handle not initialised by gfpp_model_pack%s");
-    if ((!out->rgb_map && !out->rgb_u8) || !fr->cond_feat) return fail(GFPP_ERR_INVALID, "render_frames: rgb_map (or rgb_u8) and cond_feat are required%s");
+    if ((!out->rgb_map && !out->rgb_u8 && !out->rgba_u8) || !fr->cond_feat) return fail(GFPP_ERR_INVALID, "render_frames: rgb_map (or rgb_u8) and cond_feat are required%s");
+    if ((uintptr_t)out->rgba_u8 & 3) return fail(GFPP_ERR_INVALID, "render_frames: rgba_u8 must be 4-byte aligned%s");
     if (fr->n_frames == 0 || fr->n_rays == 0) return fail(GFPP_ERR_INVALID, "render_frames: empty clip%s");
     if ((uint64_t)fr->n_frames * fr->n_rays >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "render_frames: F*N must be < 2^31%s");
     if (fr->max_steps < 1 || fr->max_steps > 4096) return fail(GFPP_ERR_UNSUPPORTED, "render_frames: max_steps must be in 1..4096%s");
@@ -691,6 +692,8 @@ int gfpp_render_frames(const gfpp_model *model, const gfpp_frames *fr, const gfp
     t.image = a.image; t.wsum = a.wsum;
     t.rgb_map = out->rgb_map;
     t.rgb_u8 = out->rgb_u8;
+    t.alpha_map = out->alpha_map;
+    t.rgba_u8 = out->rgba_u8;
     t.bg_color = fr->bg_color;
     t.P_count = (int *)(ws + W.pcount);
     if (m.has_torso) {

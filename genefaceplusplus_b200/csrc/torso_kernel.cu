@@ -135,7 +135,10 @@ __global__ void k_torso_frame_bias(TorsoArgs a, const float *__restrict__ w_def0
     }
 }
 
-__global__ void __launch_bounds__(256, 2) k_epilogue(const __grid_constant__ TorsoArgs a) {
+// MATTE: the composite tail also writes alpha_map / rgba_u8.  A compile-time switch, not a runtime branch: the kernel without it
+// compiles to the same instructions as before the matte existed (a runtime branch reschedules the MMA section around it)
+template <bool MATTE>
+__device__ __forceinline__ void epilogue_body(const TorsoArgs &a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Smem &s = *reinterpret_cast<Smem *>(smem_raw);
     const int tid = threadIdx.x;
@@ -294,6 +297,21 @@ __global__ void __launch_bounds__(256, 2) k_epilogue(const __grid_constant__ Tor
                 if (a.rgb_u8) a.rgb_u8[3 * g + c] = (unsigned char)(int)__fmul_rn(vc, 255.0f);
                 if (a.torso_rgb) a.torso_rgb[3 * g + c] = bg;
             }
+            // the matte: premultiplied P = clamp(image + (1 - ws) * (torso_color * alpha)) and coverage A = ws + (1 - ws) * alpha,
+            // without the background, so that P + (1 - A) * B is the frame over any B (bg = 0 above gives the same P bits)
+            if constexpr (MATTE) {
+                const float A = __fadd_rn(ws, __fmul_rn(__fsub_rn(1.0f, ws), ta));
+                if (a.alpha_map) a.alpha_map[g] = A;
+                if (a.rgba_u8) {
+                    uint32_t px = (uint32_t)(unsigned char)(int)__fmul_rn(A, 255.0f) << 24;
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) {
+                        const float p = __fadd_rn(a.image[3 * g + c], __fmul_rn(__fsub_rn(1.0f, ws), __fmul_rn(tc[c], ta)));
+                        px |= (uint32_t)(unsigned char)(int)__fmul_rn(fminf(fmaxf(p, 0.f), 1.f), 255.0f) << (8 * c);
+                    }
+                    reinterpret_cast<uint32_t *>(a.rgba_u8)[g] = px;   // one 32-bit store per pixel: the warp's stores coalesce
+                }
+            }
             if (a.torso_alpha) a.torso_alpha[g] = ta;
             if (a.deform) { a.deform[2 * g] = dx; a.deform[2 * g + 1] = dy; }
             if (a.P_count && any && s.mask[tid]) atomicAdd(a.P_count + f, 1);
@@ -304,6 +322,9 @@ __global__ void __launch_bounds__(256, 2) k_epilogue(const __grid_constant__ Tor
     // released at exit and may already belong to the next CTA on this SM
     if (a.has_torso && !w_ready) mbar_wait(&s.bar, 0);
 }
+
+__global__ void __launch_bounds__(256, 2) k_epilogue(const __grid_constant__ TorsoArgs a) { epilogue_body<false>(a); }
+__global__ void __launch_bounds__(256, 2) k_epilogue_matte(const __grid_constant__ TorsoArgs a) { epilogue_body<true>(a); }
 
 // dst[k][n] = src[(row0 + n) * ld + col0 + k] for k < K, zero for K <= k < Kpad   (k-major repack of nn.Linear weights)
 __global__ void k_pack_kmajor(const float *__restrict__ src, int ld, int row0, int col0, int N, int K, int Kpad,
@@ -373,12 +394,13 @@ cudaError_t launch_torso_frame_bias(const TorsoArgs &a, const float *w_def0, con
 
 cudaError_t launch_epilogue(const TorsoArgs &a, cudaStream_t st) {
     // function attributes are per device: set on every launch (a few microseconds), never cached process-wide
-    cudaError_t e = cudaFuncSetAttribute(k_epilogue, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem));
+    const auto kernel = a.alpha_map || a.rgba_u8 ? k_epilogue_matte : k_epilogue;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem));
     if (e != cudaSuccess) return e;
     const int tiles = a.n_frames * ((a.n_rays + TP - 1) / TP);
     int blocks = 2 * sm_count();
     if (tiles < blocks) blocks = tiles > 0 ? tiles : 1;
-    k_epilogue<<<blocks, NT, sizeof(Smem), st>>>(a);
+    kernel<<<blocks, NT, sizeof(Smem), st>>>(a);
     return cudaGetLastError();
 }
 

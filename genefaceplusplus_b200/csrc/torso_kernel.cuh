@@ -28,6 +28,8 @@ struct TorsoArgs {
     const float *wsum;      // [F,N]
     float *rgb_map;         // [F,N,3] or nullptr
     unsigned char *rgb_u8;  // [F,N,3] (uint8)(int)(rgb*255) or nullptr
+    float *alpha_map;       // [F,N] coverage A = ws + (1 - ws) * torso_alpha, or nullptr
+    unsigned char *rgba_u8; // [F,N,4] 4-byte aligned: (uint8)(int)(P*255) x 3, (uint8)(int)(A*255); or nullptr
     float *torso_alpha;     // [F,N] or nullptr
     float *torso_rgb;       // [F,N,3] or nullptr
     float *deform;          // [F,N,2] or nullptr

@@ -18,10 +18,15 @@ change is
 
 For the `low_memory_usage` mode (:449-470), `iter_video_frames` yields the frames as host uint8 chunks for `writer.append_data`,
 with only two chunks of frames alive at any time.
+
+With as_rgba=True both return alpha-matte frames [..,H,W,4] instead (non-SR models): premultiplied colour P and coverage A as
+`(x*255).int()`, with no background in them (the batch's `bg_img` is not read), so that P + (1 - A) * B puts the head over any
+background B, e.g. a different one per frame.
 """
 import torch
 
 from .dist import to_uint8
+from .renderer import _no_sr_matte
 
 
 def cond_feat_from_windows(model, cond_wins, eye_area_percent=None):
@@ -66,19 +71,27 @@ def _render_kw(model, T_thresh, dt_gamma, max_steps):
             "T_thresh": T_thresh}
 
 
-def _render_chunk(model, batch, feat, s, e, kw, out=None, out_u8=None, sr_noise_mode="random"):
+def _check_formats(model, as_uint8, as_rgba):
+    if as_rgba and as_uint8:
+        raise ValueError("as_rgba and as_uint8 are two different frame formats: pick one")
+    _no_sr_matte(as_rgba and _is_sr(model))
+
+
+def _render_chunk(model, batch, feat, s, e, kw, out=None, out_u8=None, out_rgba=None, sr_noise_mode="random"):
     """Frames [s, e) of the batch in one libgfpp call per stage.  Non-SR models: returns render_frames' result (`rgb_map` [n,N,3];
-    with out_u8 [n,N,3] the uint8 frames go there instead).  SR models: the clamped 512x512 frames go into out [n,3,512,512]
-    and/or out_u8 [n,512,512,3] -- what render()'s `sr_rgb_map` gives frame by frame: the head field with the frame's rays
-    (torso-SR: on a zero background, then the torso field + composite with its `lm68` row over `bg_img`), then the SR head."""
+    with out_u8 [n,N,3] the uint8 frames go there instead; with out_rgba [n,N,4] the matte frames, without the background).
+    SR models: the clamped 512x512 frames go into out [n,3,512,512] and/or out_u8 [n,512,512,3] -- what render()'s `sr_rgb_map`
+    gives frame by frame: the head field with the frame's rays (torso-SR: on a zero background, then the torso field + composite
+    with its `lm68` row over `bg_img`), then the SR head."""
     N = batch["rays_o"][0].numel() // 3
     rays_o = torch.stack([batch["rays_o"][i].reshape(N, 3) for i in range(s, e)])
     rays_d = torch.stack([batch["rays_d"][i].reshape(N, 3) for i in range(s, e)])
     if not _is_sr(model):
         pose6 = torch.stack([batch["poses"][i].reshape(6) for i in range(s, e)]) if model.has_torso else None
+        bufs = {"rgba_out": out_rgba} if out_rgba is not None else {} if out_u8 is None else {"u8_out": out_u8}
         return model.render_frames(feat[s:e], rays_o=rays_o, rays_d=rays_d, pose6=pose6,
-                                   bg_coords=batch["bg_coords"] if model.has_torso else None, bg_color=batch.get("bg_img"),
-                                   **kw, want_torso_maps=False, **({} if out_u8 is None else {"u8_out": out_u8}))
+                                   bg_coords=batch["bg_coords"] if model.has_torso else None,
+                                   bg_color=batch.get("bg_img") if out_rgba is None else None, **kw, want_torso_maps=False, **bufs)
     dev = model.density_bitfield.device
     with torch.autocast(dev.type, enabled=False):
         if hasattr(model, "torso_composite_native"):
@@ -93,10 +106,12 @@ def _render_chunk(model, batch, feat, s, e, kw, out=None, out_u8=None, sr_noise_
 
 @torch.no_grad()
 def render_driver_batch(model, batch, T_thresh=1e-2, frames_per_call=32, dt_gamma=None, max_steps=None, as_uint8=False,
-                        sr_noise_mode="random"):
+                        sr_noise_mode="random", as_rgba=False):
     """-> [T,3,H,W] fp32 in [0,1] on the model's device (H = W = sqrt(N); SR models: the 512x512 `sr_rgb_map` frames), or with
-    as_uint8 the video frames uint8 [T,H,W,3] `(rgb*255).int()`, written by the last kernel itself.  SR models take the batch's
-    `lm68` [T,136] (torso-SR) and render at most SR_FRAMES_PER_CALL frames per call; sr_noise_mode as render()'s."""
+    as_uint8 the video frames uint8 [T,H,W,3] `(rgb*255).int()`, written by the last kernel itself, or with as_rgba (non-SR models)
+    the alpha-matte frames uint8 [T,H,W,4] of render_frames' rgba_out.  SR models take the batch's `lm68` [T,136] (torso-SR) and
+    render at most SR_FRAMES_PER_CALL frames per call; sr_noise_mode as render()'s."""
+    _check_formats(model, as_uint8, as_rgba)
     T = len(batch["poses"])
     dev = model.density_bitfield.device
     feat = cond_feat_from_windows(model, batch["cond_wins"], batch.get("eye_area_percent"))
@@ -111,14 +126,17 @@ def render_driver_batch(model, batch, T_thresh=1e-2, frames_per_call=32, dt_gamm
                           sr_noise_mode=sr_noise_mode)
         return out
     N = H * W
-    out = torch.empty(T, N, 3, device=dev, dtype=torch.uint8 if as_uint8 else torch.float32)
+    C = 4 if as_rgba else 3
+    out = torch.empty(T, N, C, device=dev, dtype=torch.uint8 if as_uint8 or as_rgba else torch.float32)
     for s in range(0, T, frames_per_call):
         e = min(T, s + frames_per_call)
-        if as_uint8:
+        if as_rgba:
+            _render_chunk(model, batch, feat, s, e, kw, out_rgba=out[s:e])
+        elif as_uint8:
             _render_chunk(model, batch, feat, s, e, kw, out_u8=out[s:e])
         else:
             out[s:e] = _render_chunk(model, batch, feat, s, e, kw)["rgb_map"]
-    return out.view(T, H, W, 3) if as_uint8 else out.view(T, H, W, 3).permute(0, 3, 1, 2)
+    return out.view(T, H, W, C) if as_uint8 or as_rgba else out.view(T, H, W, 3).permute(0, 3, 1, 2)
 
 
 def _pinned(shape):
@@ -126,14 +144,17 @@ def _pinned(shape):
 
 
 @torch.no_grad()
-def iter_video_frames(model, batch, frames_per_call=8, T_thresh=1e-2, dt_gamma=None, max_steps=None, sr_noise_mode="random"):
+def iter_video_frames(model, batch, frames_per_call=8, T_thresh=1e-2, dt_gamma=None, max_steps=None, sr_noise_mode="random",
+                      as_rgba=False):
     """The `low_memory_usage` loop of forward_secc2video (genefacepp_infer.py:449-470) for all four model classes: yields the
     clip's video frames -- what render_driver_batch(..., as_uint8=True) returns -- as host uint8 [n,H,W,3] chunks in frame order
     (n <= frames_per_call; SR models: <= SR_FRAMES_PER_CALL), e.g. `for c in iter_video_frames(...): for f in c.numpy(): writer.append_data(f)`.
+    as_rgba (non-SR models): the alpha-matte frames of render_driver_batch(..., as_rgba=True) instead, as [n,H,W,4] chunks.
 
     Two device and two pinned host buffers: chunk k+1 renders on the current stream while chunk k is copied to the host on a
     side stream and handed to the caller.  A yielded chunk stays valid until the generator is advanced.  When the generator
     ends, fails or is closed early, it waits for both streams: no queued work is left behind."""
+    _check_formats(model, False, as_rgba)
     T = len(batch["poses"])
     dev = model.density_bitfield.device
     feat = cond_feat_from_windows(model, batch["cond_wins"], batch.get("eye_area_percent"))
@@ -144,8 +165,9 @@ def iter_video_frames(model, batch, frames_per_call=8, T_thresh=1e-2, dt_gamma=N
     compute = torch.cuda.current_stream(dev)
     side = torch.cuda.Stream(dev)
     rows = min(fpc, T)
-    dbuf = [torch.empty(rows, H, W, 3, device=dev, dtype=torch.uint8) for _ in range(2)]
-    hbuf = [_pinned((rows, H, W, 3)) for _ in range(2)]
+    C = 4 if as_rgba else 3
+    dbuf = [torch.empty(rows, H, W, C, device=dev, dtype=torch.uint8) for _ in range(2)]
+    hbuf = [_pinned((rows, H, W, C)) for _ in range(2)]
     rendered = [torch.cuda.Event() for _ in range(2)]
     copied = [torch.cuda.Event() for _ in range(2)]
 
@@ -154,7 +176,8 @@ def iter_video_frames(model, batch, frames_per_call=8, T_thresh=1e-2, dt_gamma=N
         s, b = starts[k], k % 2
         e = min(T, s + fpc)
         compute.wait_event(copied[b])           # chunk k-2 has left device buffer b
-        _render_chunk(model, batch, feat, s, e, kw, out_u8=dbuf[b][:e - s], sr_noise_mode=sr_noise_mode)
+        dst = {"out_rgba": dbuf[b][:e - s]} if as_rgba else {"out_u8": dbuf[b][:e - s]}
+        _render_chunk(model, batch, feat, s, e, kw, sr_noise_mode=sr_noise_mode, **dst)
         rendered[b].record(compute)
         side.wait_event(rendered[b])
         with torch.cuda.stream(side):

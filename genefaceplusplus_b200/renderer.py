@@ -365,7 +365,8 @@ class RADNeRF(nn.Module):
     # ------------------------------------------------------------------ core call
     def render_frames(self, cond_feat, *, rays_o=None, rays_d=None, poses_c2w=None, intrinsics=None, H=None, W=None,
                       pose6=None, bg_coords=None, bg_color=None, dt_gamma=0.0, max_steps=1024, T_thresh=1e-4,
-                      want_torso_maps=True, want_stats=False, rgb_out=None, u8_out=None, want_aux=True, noise=None):
+                      want_torso_maps=True, want_stats=False, rgb_out=None, u8_out=None, want_aux=True, noise=None, alpha_out=None,
+                      rgba_out=None):
         """Render F frames with one call into libgfpp.  Returns a dict of device tensors with a leading F axis.
 
         Either (rays_o, rays_d) [F,N,3] or (poses_c2w [F,4,4], intrinsics, H, W) must be given.
@@ -375,10 +376,14 @@ class RADNeRF(nn.Module):
         rgb_out: optional contiguous fp32 [F,N,3] device view the kernel writes `rgb_map` into (e.g. a slice of the clip buffer:
         no copy afterwards); u8_out: optional contiguous uint8 [F,N,3] view that receives the video frame `(rgb*255).int()`
         straight from the epilogue kernel -- with u8_out and no rgb_out no fp32 frame is written at all.
+        The frame's alpha matte, written by the same kernel and independent of bg_color (include/gfpp.h, gfpp_outputs): alpha_out,
+        optional contiguous fp32 [F,N] view, receives the coverage A = weights_sum + (1 - weights_sum) * torso_alpha (result key
+        `alpha_map`); rgba_out, optional contiguous uint8 [F,N,4] view (4-byte aligned), receives the premultiplied colour P as
+        (P*255).int() in the first three bytes and (A*255).int() in the fourth (result key `rgba_u8`).  P + (1 - A) * B is the frame
+        over a background B.  rgba_out alone is a complete call: no RGB frame is written then.
         want_aux=False skips the depth / weights_sum result tensors (they stay in the workspace)."""
         if self.training:
             raise NotImplementedError("libgfpp implements the inference branch only (renderer.py:340-384)")
-        _, packed, model, _keep = self._ensure_packed()
         dev = self.density_bitfield.device
         L = _capi.lib()
         f32 = torch.float32
@@ -439,13 +444,24 @@ class RADNeRF(nn.Module):
             if rgb_out.dtype != f32 or not rgb_out.is_contiguous() or rgb_out.numel() != Fn * N * 3 or rgb_out.device != dev:
                 raise ValueError(f"rgb_out must be a contiguous fp32 [{Fn},{N},3] tensor on {dev}")
             res["rgb_map"] = rgb_out.view(Fn, N, 3)
-        elif u8_out is None:
+        elif u8_out is None and rgba_out is None:
             res["rgb_map"] = torch.empty(Fn, N, 3, device=dev, dtype=f32)
         if u8_out is not None:
             if u8_out.dtype != torch.uint8 or not u8_out.is_contiguous() or u8_out.numel() != Fn * N * 3 or u8_out.device != dev:
                 raise ValueError(f"u8_out must be a contiguous uint8 [{Fn},{N},3] tensor on {dev}")
             res["rgb_u8"] = u8_out.view(Fn, N, 3)
             out.rgb_u8 = u8_out.data_ptr()
+        if alpha_out is not None:
+            if alpha_out.dtype != f32 or not alpha_out.is_contiguous() or alpha_out.numel() != Fn * N or alpha_out.device != dev:
+                raise ValueError(f"alpha_out must be a contiguous fp32 [{Fn},{N}] tensor on {dev}")
+            res["alpha_map"] = alpha_out.view(Fn, N)
+            out.alpha_map = alpha_out.data_ptr()
+        if rgba_out is not None:
+            if (rgba_out.dtype != torch.uint8 or not rgba_out.is_contiguous() or rgba_out.numel() != Fn * N * 4 or rgba_out.device != dev
+                    or rgba_out.data_ptr() % 4):
+                raise ValueError(f"rgba_out must be a contiguous, 4-byte aligned uint8 [{Fn},{N},4] tensor on {dev}")
+            res["rgba_u8"] = rgba_out.view(Fn, N, 4)
+            out.rgba_u8 = rgba_out.data_ptr()
         if "rgb_map" in res:
             out.rgb_map = res["rgb_map"].data_ptr()
         if want_aux:
@@ -460,6 +476,7 @@ class RADNeRF(nn.Module):
         if want_stats:
             res["stats"] = torch.empty(Fn, 4, device=dev, dtype=torch.int32)
             out.stats = res["stats"].data_ptr()
+        _, packed, model, _keep = self._ensure_packed()   # after the argument checks: a bad call launches nothing
         need = L.gfpp_render_workspace_bytes(Fn, N, int(max_steps))
         if self._workspace is None or self._workspace.numel() < need or self._workspace.device != dev:
             self._workspace = torch.empty(need, dtype=torch.uint8, device=dev)
@@ -784,35 +801,45 @@ class RADNeRF(nn.Module):
     @torch.no_grad()
     def render_clip(self, poses_c2w, intrinsics, H, W, cond_seq=None, cond_feat=None, bg_color=None, bg_coords=None, pose6=None,
                     dt_gamma=None, max_steps=None, T_thresh=1e-2, frames_per_call=64, out=None, want_stats=False,
-                    eye_area_percent=None, as_uint8=False):
+                    eye_area_percent=None, as_uint8=False, as_rgba=False):
         """Render a clip: poses_c2w [T,4,4], cond_seq [T,1,C] (or precomputed cond_feat [T,64]); eye_area_percent [T] for
         add_eye_blink_cond models.  Returns rgb [T,H*W,3] on the model's device: fp32 clamped to [0,1], or -- as_uint8 -- the
-        uint8 video frames `(rgb*255).int()` (genefacepp_infer.py:469,505) written by the epilogue kernel itself.  `out`: optional
-        preallocated result buffer of that dtype; every call writes its frames straight into it."""
+        uint8 video frames `(rgb*255).int()` (genefacepp_infer.py:469,505) written by the epilogue kernel itself, or -- as_rgba --
+        uint8 [T,H*W,4] alpha-matte frames: premultiplied colour P and coverage A, each `(x*255).int()`, so that P + (1 - A) * B is
+        the frame over any background B (render_frames' rgba_out).  The matte is defined without a background: as_rgba with
+        bg_color, or with as_uint8, raises ValueError.  `out`: optional preallocated result buffer of that dtype and shape; every
+        call writes its frames straight into it."""
+        if as_rgba and as_uint8:
+            raise ValueError("as_rgba and as_uint8 are two different frame formats: pick one")
+        if as_rgba and bg_color is not None:
+            raise ValueError("as_rgba returns the frame's matte, which does not depend on a background: composite P + (1 - A) * B "
+                             "instead of passing bg_color")
         dev = self.density_bitfield.device
         T = poses_c2w.shape[0]
         hp = self.hparams
         dt_gamma = hp["dt_gamma"] if dt_gamma is None else dt_gamma
         max_steps = hp["max_steps"] if max_steps is None else max_steps
+        N = H * W
+        odt = torch.uint8 if as_uint8 or as_rgba else torch.float32
+        C = 4 if as_rgba else 3
+        rgb = out if out is not None else torch.empty(T, N, C, device=dev, dtype=odt)
+        if rgb.dtype != odt or rgb.numel() != T * N * C or not rgb.is_contiguous():
+            raise ValueError(f"out must be a contiguous {odt} [{T},{N},{C}] tensor")
+        rgb = rgb.view(T, N, C)
         if cond_feat is None:
             cond_feat = self.cal_cond_feat_clip(cond_seq.to(dev), eye_area_percent=eye_area_percent if self.forwards_eye_area else None)
         poses_c2w = poses_c2w.to(dev, torch.float32)
         if self.has_torso and pose6 is None:
             from .scene import convert_poses
             pose6 = convert_poses(poses_c2w.cpu()).to(dev)
-        N = H * W
-        odt = torch.uint8 if as_uint8 else torch.float32
-        rgb = out if out is not None else torch.empty(T, N, 3, device=dev, dtype=odt)
-        if rgb.dtype != odt or rgb.numel() != T * N * 3 or not rgb.is_contiguous():
-            raise ValueError(f"out must be a contiguous {odt} [{T},{N},3] tensor")
-        rgb = rgb.view(T, N, 3)
+        dst = "rgba_out" if as_rgba else "u8_out" if as_uint8 else "rgb_out"
         stats = []
         for s in range(0, T, frames_per_call):
             e = min(T, s + frames_per_call)
             res = self.render_frames(cond_feat[s:e], poses_c2w=poses_c2w[s:e], intrinsics=intrinsics, H=H, W=W,
                                      pose6=pose6[s:e] if self.has_torso else None, bg_coords=bg_coords, bg_color=bg_color,
                                      dt_gamma=dt_gamma, max_steps=max_steps, T_thresh=T_thresh, want_torso_maps=False,
-                                     want_stats=want_stats, want_aux=False, **({"u8_out": rgb[s:e]} if as_uint8 else {"rgb_out": rgb[s:e]}))
+                                     want_stats=want_stats, want_aux=False, **{dst: rgb[s:e]})
             if want_stats:
                 stats.append(res["stats"])
         if want_stats:
@@ -821,6 +848,14 @@ class RADNeRF(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------ head model + super-resolution
+def _no_sr_matte(as_rgba):
+    """The SR head is not linear in its input, so no alpha composes its 512x512 frame from the NeRF's matte: the SR models have
+    no as_rgba output."""
+    if as_rgba:
+        raise ValueError("as_rgba is not available for the SR models: the SR head is not linear in its input, so no alpha matte "
+                         "composes its 512x512 frame")
+
+
 class RADNeRFwithSR(RADNeRF):
     """modules/radnerfs/radnerf_sr.py:50-210: the same head field rendered at 256x256 plus the `sr_net` 256 -> 512 head
     (genefaceplusplus_b200/superres.py).  Same extra state (`sr_net.*`, `lambda_ambient`) and result keys: `rgb_map` becomes
@@ -848,12 +883,15 @@ class RADNeRFwithSR(RADNeRF):
         return results
 
     @torch.no_grad()
-    def render_clip(self, poses_c2w, intrinsics, H=256, W=256, *args, sr_noise_mode="random", sr_frames_per_call=8, as_uint8=False, **kwargs):
+    def render_clip(self, poses_c2w, intrinsics, H=256, W=256, *args, sr_noise_mode="random", sr_frames_per_call=8, as_uint8=False,
+                    as_rgba=False, **kwargs):
         """Clip API: NeRF at 256x256 for all frames (libgfpp), then the SR head over chunks of frames.
         Returns the clamped 512x512 frames [T,3,512,512]; `intrinsics` are those of the 256x256 camera.
         as_uint8: returns the video frames uint8 [T,512,512,3] (HWC) `(rgb*255).int()` instead, written by the SR head's last
         kernel chunk by chunk into `out` (optional preallocated buffer of that shape); the NeRF stage still renders fp32, the
-        SR head's input.  Without as_uint8, `out` is the NeRF clip's buffer ([T,256*256,3] fp32), as in RADNeRF.render_clip."""
+        SR head's input.  Without as_uint8, `out` is the NeRF clip's buffer ([T,256*256,3] fp32), as in RADNeRF.render_clip.
+        as_rgba raises ValueError (_no_sr_matte)."""
+        _no_sr_matte(as_rgba)
         from .dist import to_uint8
         R = self.sr_input_resolution
         if (H, W) != (R, R):
@@ -1291,13 +1329,15 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
     @torch.no_grad()
     def render_clip(self, poses_c2w, intrinsics, H=256, W=256, cond_seq=None, bg_color=None, bg_coords=None, lm68_seq=None,
                     eye_area_percent=None, dt_gamma=None, max_steps=None, T_thresh=1e-2, sr_noise_mode="random", cond_feat=None,
-                    as_uint8=False, **unused):
+                    as_uint8=False, as_rgba=False, **unused):
         """Clip API of the torso-SR model -> the clamped 512x512 frames [T,3,512,512].  With the native backends (the default) every
         stage runs in libgfpp chunk by chunk -- head field with rays generated in-kernel, torso-SR field + composite, SR head -- with
         no per-frame host work; with a "torch" backend it falls back to frame-by-frame `render()`.  poses_c2w [T,4,4] (c2w,
         dataset.poses), cond_seq [T,1,C] (or cond_feat [T,64] precomputed), lm68_seq [T,136], eye_area_percent [T] or None.
         as_uint8: returns the video frames uint8 [T,512,512,3] (HWC) `(rgb*255).int()` instead, written by the SR head's last kernel
-        chunk by chunk into `out` (optional preallocated buffer of that shape); no fp32 512x512 frame is written then."""
+        chunk by chunk into `out` (optional preallocated buffer of that shape); no fp32 512x512 frame is written then.
+        as_rgba raises ValueError (_no_sr_matte)."""
+        _no_sr_matte(as_rgba)
         from .dist import to_uint8
         from .scene import cond_window, convert_poses, get_rays
         R = self.sr_input_resolution

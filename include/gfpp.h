@@ -205,6 +205,17 @@ typedef struct {
     uint8_t *rgb_u8;              /* [F,N,3] the frame as the video writer wants it, (uint8)(int)(rgb * 255) of the clamped colour
                                    * (inference/genefacepp_infer.py:469,505), written by the epilogue kernel itself; or NULL.
                                    * rgb_map may be NULL when rgb_u8 is given (then no fp32 frame is written at all) */
+    /* The frame's alpha matte, for compositing over something other than one static background.  With ws = weights_sum, image
+     * the premultiplied head colour and ta, tc the torso alpha and colour (both 0 outside the torso mask and for head-only models):
+     *   coverage               A = ws + (1 - ws) * ta
+     *   premultiplied colour   P = clamp(image + (1 - ws) * (tc * ta), 0, 1)
+     * fp32, rounded at the same sites as the composite.  Head-only models: A = ws, P = clamp(image).  P + (1 - A) * B is the
+     * frame rendered with bg_color = B (up to fp32 rounding wherever that composite was not clamped); P is that frame's colour
+     * for B = 0 bit for bit.  Both ignore bg_color, so a call may ask for the frame over bg_color and for the matte together. */
+    float *alpha_map;             /* [F,N] A, or NULL */
+    uint8_t *rgba_u8;             /* [F,N,4] 4-byte aligned, written as one 32-bit store per pixel: (uint8)(int)(P * 255) per colour
+                                   * channel (the truncation of rgb_u8) and (uint8)(int)(A * 255) in the fourth byte; or NULL.
+                                   * At least one of rgb_map, rgb_u8 and rgba_u8 must be given. */
 } gfpp_outputs;
 
 GFPP_API size_t gfpp_render_workspace_bytes(uint32_t n_frames, uint32_t n_rays, uint32_t max_steps);
