@@ -103,16 +103,38 @@ static_assert(smem_bytes<false>() <= 227 * 1024 && smem_bytes<true>() <= 227 * 1
 
 // Epilogue of one M = 64 half (rows 64*half ..) of a 128-wide layer from the accumulator fragment: (+bias) -> (ReLU) ->
 // operand tiles h0|h1 (cols 0-63 | 64-127) and, when LO, the residual images l0|l1.  BIAS: shared-memory vector (color L0).
+// Without LO the pairs of two 8-column blocks go out in one stmatrix: 8 stores per thread instead of 32.
 template <bool RELU, bool BIAS, bool LO>
 __device__ __forceinline__ void epilogue_half(const float (&d)[64], unsigned char *h, unsigned char *l, int half, int lane, int wwarp,
                                               const float *bias) {
+    if constexpr (LO) {
 #pragma unroll
-    for (int i = 0; i < 64; i += 2) {
-        const int row = 64 * half + frag_row(i, lane, wwarp), col = frag_col(i, lane);
-        float x0 = d[i], x1 = d[i + 1];
-        if (BIAS) { x0 += bias[col]; x1 += bias[col + 1]; }
-        if (RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-        store_pair<false, LO>(h + (col >> 6) * V2_TILE_BYTES, l + (LO ? (col >> 6) * V2_TILE_BYTES : 0), row, col & 63, x0, x1);
+        for (int i = 0; i < 64; i += 2) {
+            const int row = 64 * half + frag_row(i, lane, wwarp), col = frag_col(i, lane);
+            float x0 = d[i], x1 = d[i + 1];
+            if (BIAS) { x0 += bias[col]; x1 += bias[col + 1]; }
+            if (RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+            store_pair<false, LO>(h + (col >> 6) * V2_TILE_BYTES, l + (col >> 6) * V2_TILE_BYTES, row, col & 63, x0, x1);
+        }
+    } else {
+        // matrix j of a store is the 8 x 8 block of rows +8 (j & 1), column block cb + (j >> 1): fragment pairs 4 cb + 2 j, +1.
+        // Lane l addresses row l % 8 of matrix l / 8
+        const int m = lane >> 3, arow = 64 * half + 16 * wwarp + 8 * (m & 1) + (lane & 7);
+        const uint32_t h_u = smem_u32(h);
+#pragma unroll
+        for (int cb = 0; cb < 16; cb += 2) {
+            uint32_t q[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int i = 4 * cb + 2 * j, col = frag_col(i, lane);
+                float x0 = d[i], x1 = d[i + 1];
+                if (BIAS) { x0 += bias[col]; x1 += bias[col + 1]; }
+                if (RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+                q[j] = pack2<false>(x0, x1);
+            }
+            const int c = cb + (m >> 1);
+            stmatrix_x4(h_u + (uint32_t)(c >> 3) * V2_TILE_BYTES + sw128_off(arow, c & 7), q[0], q[1], q[2], q[3]);
+        }
     }
 }
 

@@ -185,6 +185,12 @@ __device__ __forceinline__ void store_pair(unsigned char *hi_tile, unsigned char
     *reinterpret_cast<uint32_t *>(hi_tile + off) = pack2<BF16>(a, b);
     if (SPLIT) *reinterpret_cast<uint32_t *>(lo_tile + off) = pack2<BF16>(a - round16<BF16>(a), b - round16<BF16>(b));
 }
+// four 8x8 matrices of 16-bit pairs, one warp: lane l gives the shared address of row l%8 of matrix l/8 (16 contiguous bytes), and
+// register j holds the pair at row l/4, columns 2*(l%4) .. +1 of matrix j -- the layout of an accumulator fragment's pairs
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
 
 // ---- transposed (MN-major) operands: D[64 x N] (+)= A^T * B with A [K x 64] and B [K x N] both row-major over K ----
 // A [rows x 64 elements] SW128 tile read along its rows is the canonical MN-major SW128 layout as it stands: one 128-byte row per
