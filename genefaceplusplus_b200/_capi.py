@@ -107,6 +107,7 @@ EXPORTS = [
     "gfpp_torso_sr_field_workspace_bytes", "gfpp_torso_sr_field_forward", "gfpp_torso_sr_field_backward",
     "gfpp_frozen_head_workspace_bytes", "gfpp_frozen_head",
     "gfpp_grid_encode_forward_half", "gfpp_grid_encode_backward_half",
+    "gfpp_torso_pass_workspace_bytes", "gfpp_torso_mask", "gfpp_torso_composite_forward", "gfpp_torso_composite_backward",
 ]
 
 
@@ -208,6 +209,11 @@ def lib():
         L.gfpp_torso_sr_field_forward.argtypes = [ctypes.POINTER(TorsoSrDesc), P, c_u32, P, P, P, P, P, P, P, P, c_size_t, P]
         L.gfpp_torso_sr_field_backward.argtypes = [ctypes.POINTER(TorsoSrDesc), P, c_u32, P, P, P, P, P, P, P, ctypes.POINTER(P * 3),
                                                    ctypes.POINTER(P * 3), ctypes.POINTER(P * 3), ctypes.POINTER(P * 3), P, P, P, c_size_t, P]
+        L.gfpp_torso_pass_workspace_bytes.restype = c_size_t
+        L.gfpp_torso_pass_workspace_bytes.argtypes = [c_u32]
+        L.gfpp_torso_mask.argtypes = [P, c_u32, c_f, P, c_u32, P, P, P, P, P, P, P, P, P, c_size_t, P]
+        L.gfpp_torso_composite_forward.argtypes = [P, c_u32, c_u32, P, P, P, P, P, c_u32, P, P, P, P]
+        L.gfpp_torso_composite_backward.argtypes = [P, c_u32, c_u32, P, P, P, P, P, c_u32, P, P, P, P, P, P]
         _lib = L
     return _lib
 

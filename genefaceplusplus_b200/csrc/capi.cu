@@ -64,6 +64,14 @@ cudaError_t launch_grid_refresh_tail(const float *, uint32_t, uint32_t, float, f
 cudaError_t launch_mark_untrained(const float *, uint32_t, float, float, const float *, const float *, uint32_t, uint32_t, float *, cudaStream_t);
 uint32_t torso_dilate_ema_blocks(uint32_t H);
 cudaError_t launch_torso_grid_tail(const float *, uint32_t, float, float, float *, double *, float *, float *, int *, cudaStream_t);
+// torso_pass_kernels.cu
+uint32_t torso_mask_tiles(uint32_t N);
+cudaError_t launch_torso_mask(const float *, uint32_t, float, const float *, const float *, const float *, uint32_t, int32_t *, int32_t *,
+                              float *, float *, float *, int32_t *, int *, cudaStream_t);
+cudaError_t launch_torso_composite_fwd(const int32_t *, uint32_t, const float *, const float *, const float *, const float *, const float *,
+                                       uint32_t, float *, float *, float *, cudaStream_t);
+cudaError_t launch_torso_composite_bwd(const int32_t *, uint32_t, const float *, const float *, const float *, const float *, const float *,
+                                       uint32_t, const float *, const float *, const float *, float *, float *, cudaStream_t);
 }  // namespace gfpp
 
 using namespace gfpp;
@@ -2022,6 +2030,74 @@ int gfpp_frozen_head(const gfpp_model *model, const float *rays_o, const float *
         CK(launch_cond_images(cond_feat, 1, ws + W.cond, ws + W.cond + 128, st));
         CK(launch_head_v2(a, v2, m.mlp_precision, st, true));
     } else CK(launch_head_tc(a, m.tc, m.mlp_precision, -1, st, true));
+    return GFPP_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------- (M) torso pass of the torso training steps
+extern "C" {
+
+size_t gfpp_torso_pass_workspace_bytes(uint32_t N) {
+    if (N == 0 || N >= (1u << 31)) return 0;
+    return ((size_t)torso_mask_tiles(N) * 4 + 255) / 256 * 256;
+}
+
+int gfpp_torso_mask(const float *density_grid_torso, uint32_t G, float thr, const float *bg_coords, uint32_t N, const float *image,
+                    const float *weights_sum, int32_t *idx, int32_t *slot, float *xy, float *image_m, float *weights_sum_m, int32_t *count,
+                    void *workspace, size_t workspace_bytes, void *stream) {
+    if (!density_grid_torso || !bg_coords || !idx || !slot || !xy || !count || !workspace) return fail(GFPP_ERR_INVALID, "torso_mask: null pointer%s");
+    if ((image == nullptr) != (weights_sum == nullptr) || (image == nullptr) != (image_m == nullptr) || (image == nullptr) != (weights_sum_m == nullptr))
+        return fail(GFPP_ERR_INVALID, "torso_mask: image, weights_sum and their gathers must all be given or all be NULL%s");
+    if (N == 0) return fail(GFPP_ERR_INVALID, "torso_mask: no pixels%s");
+    if (N >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_mask: N must be < 2^31%s");
+    if (G < 2 || G > 4096) return fail(GFPP_ERR_UNSUPPORTED, "torso_mask: grid_size must be in 2..4096%s");
+    if ((((uintptr_t)bg_coords | (uintptr_t)xy) & 7u) != 0) return fail(GFPP_ERR_INVALID, "torso_mask: bg_coords and xy must be 8-byte aligned%s");
+    if (workspace_bytes < gfpp_torso_pass_workspace_bytes(N)) return fail(GFPP_ERR_WORKSPACE, "torso_mask: workspace too small%s");
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_mask: workspace must be 256-byte aligned%s");
+    g_launches = 0;
+    CK(launch_torso_mask(density_grid_torso, G, thr, bg_coords, image, weights_sum, N, idx, slot, xy, image_m, weights_sum_m, count,
+                         (int *)workspace, (cudaStream_t)stream));
+    g_launches = 3;
+    return GFPP_OK;
+}
+
+// the checks the composite's two directions share; no CUDA call
+static int torso_composite_check(const char *who, uint32_t N, uint32_t M, const float *alpha, const float *color, const float *image,
+                                 const float *weights_sum, const float *bg_color, uint32_t bg_mode) {
+    if (!image || !weights_sum) return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
+    if (M > 0 && (!alpha || !color)) return fail(GFPP_ERR_INVALID, "%s: alpha and color must be given when M > 0", who);
+    if (N == 0) return fail(GFPP_ERR_INVALID, "%s: no pixels", who);
+    if (N >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: N must be < 2^31", who);
+    if (M > N) return fail(GFPP_ERR_INVALID, "%s: more masked points than pixels", who);
+    if (bg_mode > 2) return fail(GFPP_ERR_INVALID, "%s: bg_mode must be 0 (scalar 1), 1 (one colour) or 2 (per pixel)", who);
+    if ((bg_color == nullptr) != (bg_mode == 0)) return fail(GFPP_ERR_INVALID, "%s: bg_color must be given iff bg_mode > 0", who);
+    return GFPP_OK;
+}
+
+int gfpp_torso_composite_forward(const int32_t *slot, uint32_t N, uint32_t M, const float *alpha, const float *color, const float *image,
+                                 const float *weights_sum, const float *bg_color, uint32_t bg_mode, float *torso_alpha_map,
+                                 float *torso_rgb_map, float *rgb_map, void *stream) {
+    if (!slot || !torso_alpha_map || !torso_rgb_map || !rgb_map) return fail(GFPP_ERR_INVALID, "torso_composite_forward: null pointer%s");
+    const int rc = torso_composite_check("torso_composite_forward", N, M, alpha, color, image, weights_sum, bg_color, bg_mode);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    CK(launch_torso_composite_fwd(slot, N, alpha, color, image, weights_sum, bg_color, bg_mode, torso_alpha_map, torso_rgb_map, rgb_map,
+                                  (cudaStream_t)stream));
+    return GFPP_OK;
+}
+
+int gfpp_torso_composite_backward(const int32_t *idx, uint32_t N, uint32_t M, const float *alpha, const float *color, const float *image,
+                                  const float *weights_sum, const float *bg_color, uint32_t bg_mode, const float *grad_torso_alpha_map,
+                                  const float *grad_torso_rgb_map, const float *grad_rgb_map, float *grad_alpha, float *grad_color,
+                                  void *stream) {
+    const int rc = torso_composite_check("torso_composite_backward", N, M, alpha, color, image, weights_sum, bg_color, bg_mode);
+    if (rc != GFPP_OK) return rc;
+    if (M > 0 && (!idx || !grad_alpha || !grad_color)) return fail(GFPP_ERR_INVALID, "torso_composite_backward: null pointer%s");
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    CK(launch_torso_composite_bwd(idx, M, alpha, color, image, weights_sum, bg_color, bg_mode, grad_torso_alpha_map, grad_torso_rgb_map,
+                                  grad_rgb_map, grad_alpha, grad_color, (cudaStream_t)stream));
     return GFPP_OK;
 }
 

@@ -427,4 +427,35 @@ __device__ __forceinline__ void sh4(float x, float y, float z, float *o) {
     o[15] = 0.59004358992664352f * x * (-x2 + 3.0f * y2);
 }
 
+// Exclusive sum of v over the CTA (blockDim.x a multiple of 32, at most 1024); total <- the CTA's sum.  smem_warp: 65 ints of
+// shared memory.  Every thread of the CTA must call it (it synchronises).  Used by the deterministic compactions (the ray
+// scan of march_rays_train, the torso mask).
+__device__ __forceinline__ int block_exclusive_scan(int v, int *smem_warp, int &total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += u;
+    }
+    if (lane == 31) smem_warp[warp] = inc;
+    __syncthreads();
+    if (warp == 0) {
+        int w = lane < (int)(blockDim.x >> 5) ? smem_warp[lane] : 0;
+        int winc = w;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, winc, o);
+            if (lane >= o) winc += u;
+        }
+        smem_warp[32 + lane] = winc - w;   // exclusive warp bases
+        if (lane == 31) smem_warp[64] = winc;
+    }
+    __syncthreads();
+    total = smem_warp[64];
+    const int r = smem_warp[32 + warp] + inc - v;
+    __syncthreads();
+    return r;
+}
+
 }  // namespace gfpp

@@ -60,7 +60,10 @@ __device__ __forceinline__ void store_relu(const float (&acc)[8][NC], float *sA,
 }
 
 // F.grid_sample(grid[1,1,G,G], coords, align_corners=True, bilinear, zeros padding) at one point
-// (ATen grid_sampler_2d: unnormalise ((c+1)/2)*(size-1); weights nw,ne,sw,se in that order).
+// (ATen grid_sampler_2d: unnormalise ((c+1)/2)*(size-1); weights nw,ne,sw,se in that order).  ATen's CUDA kernel accumulates with
+// `out += v * w`, which nvcc contracts to an FMA: kFma = true restates that exactly on any grid (the training mask, gfpp_torso_mask);
+// the default rounds each product, which is the same wherever v * w is exact -- a 0 / 1 grid -- and is what the render epilogues use.
+template <bool kFma = false>
 __device__ __forceinline__ float sample_density(const float *__restrict__ grid, int G, float cx, float cy) {
     const float ix = __fmul_rn(__fdiv_rn(__fadd_rn(cx, 1.0f), 2.0f), (float)(G - 1));
     const float iy = __fmul_rn(__fdiv_rn(__fadd_rn(cy, 1.0f), 2.0f), (float)(G - 1));
@@ -70,11 +73,12 @@ __device__ __forceinline__ float sample_density(const float *__restrict__ grid, 
     const float sw = __fmul_rn(__fsub_rn(x1, ix), __fsub_rn(iy, y0)), se = __fmul_rn(__fsub_rn(ix, x0), __fsub_rn(iy, y0));
     const int ix0 = (int)x0, iy0 = (int)y0, ix1 = ix0 + 1, iy1 = iy0 + 1;
     auto at = [&](int yy, int xx) -> float { return (xx >= 0 && xx < G && yy >= 0 && yy < G) ? __ldg(grid + yy * G + xx) : 0.0f; };
+    auto acc = [](float o, float v, float w) { return kFma ? __fmaf_rn(v, w, o) : __fadd_rn(o, __fmul_rn(v, w)); };
     float out = 0.f;
-    out = __fadd_rn(out, __fmul_rn(at(iy0, ix0), nw));
-    out = __fadd_rn(out, __fmul_rn(at(iy0, ix1), ne));
-    out = __fadd_rn(out, __fmul_rn(at(iy1, ix0), sw));
-    out = __fadd_rn(out, __fmul_rn(at(iy1, ix1), se));
+    out = acc(out, at(iy0, ix0), nw);
+    out = acc(out, at(iy0, ix1), ne);
+    out = acc(out, at(iy1, ix0), sw);
+    out = acc(out, at(iy1, ix1), se);
     return out;
 }
 

@@ -49,34 +49,6 @@ __global__ void k_march_train_count(MarchConst mc, const float *__restrict__ ray
 }
 
 // ---- exclusive scan of rays[.,2] into rays[.,1]: tile sums, scan of the tile sums (one CTA), tile-local scan + base ----
-__device__ __forceinline__ int block_exclusive_scan(int v, int *smem_warp, int &total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += u;
-    }
-    if (lane == 31) smem_warp[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-        int w = lane < (int)(blockDim.x >> 5) ? smem_warp[lane] : 0;
-        int winc = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, winc, o);
-            if (lane >= o) winc += u;
-        }
-        smem_warp[32 + lane] = winc - w;   // exclusive warp bases
-        if (lane == 31) smem_warp[64] = winc;
-    }
-    __syncthreads();
-    total = smem_warp[64];
-    const int r = smem_warp[32 + warp] + inc - v;
-    __syncthreads();
-    return r;
-}
-
 __global__ void __launch_bounds__(SCAN_NT) k_scan_tile_sums(const int *__restrict__ rays, uint32_t N, int *__restrict__ tile_sums) {
     __shared__ int sw[65];
     const uint32_t base = blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_ITEMS;

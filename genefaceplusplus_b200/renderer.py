@@ -1025,6 +1025,35 @@ class _TorsoGrid:
         self.last_launch_count = int(_capi.lib().gfpp_last_launch_count())
         return mean
 
+    def torso_pass(self, image, weights_sum, bg_coords, poses, c, bg_color=None, lm68=None):
+        """The torso part of the torso training step (radnerf_torso.py:165-193, radnerf_torso_sr.py:196-221) between frozen_head()
+        and the loss, fused on libgfpp (gfpp.h section M around the training field of section H or I):
+
+            weights_sum, image = model.frozen_head(rays_o, rays_d, cond_feat, model.individual_embeddings[idx], perturb=True, max_steps=16)
+            res = model.torso_pass(image, weights_sum, bg_coords, pose6, model.torso_individual_codes[idx], bg_color=bg)        # RADNeRFTorso
+            res = sr.torso_pass(image, weights_sum, bg_coords, None, sr.torso_individual_codes[idx], bg_color=bg, lm68=lm68)  # torso-SR
+
+        image [N,3] / weights_sum [N] the head's premultiplied colour and alpha, bg_coords [...,2] with N pixels, poses the head pose
+        [1,6] (convert_poses; RADNeRFTorso) or unused (RADNeRFTorsowithSR, conditioned on lm68, 136 values), c the code row
+        torso_individual_codes[idx] or None without codes, bg_color None (1), one colour (3 values) or one per pixel (N x 3).
+        Returns the composed recipe's flat maps: torso_alpha_map [N,1], torso_rgb_map [N,3], rgb_map [N,3] (clamped), weights_sum [N]
+        and, iff some pixel is masked, deform [M,2].  The SR task reshapes rgb_map to [1,3,R,R] for its SR head, as the reference does.
+        The maps are bit-identical to the composed recipe (README); gradients reach the same parameters as forward_torso's (the
+        torso MLPs, the torso table, the code row, head_color_weights_encoder with torso_head_aware), deform's included.  One host
+        sync (the count of masked pixels, from a pinned buffer); fp32, with autocast disabled inside; train or eval mode.  With no
+        masked pixel no field runs and no output requires grad.  Inputs other than the parameters that require grad raise
+        NotImplementedError, as forward_torso does."""
+        dev = self._require_cuda()
+        if any(torch.is_tensor(t) and t.requires_grad for t in (image, weights_sum, bg_coords, poses, lm68, bg_color)):
+            raise NotImplementedError("gradients w.r.t. the head image, weights_sum, bg_coords, the pose, lm68 or bg_color are not implemented")
+        dim = self.torso_individual_embedding_dim
+        if (c is None) != (dim == 0) or (c is not None and (not torch.is_tensor(c) or c.numel() != dim)):
+            raise ValueError(f"c must hold {dim} values (None iff the model has no torso_individual_codes)")
+        field, head_aware = self._torso_pass_field(poses, None if c is None else c.to(dev), lm68, dev)
+        from . import train_ops
+        with torch.autocast("cuda", enabled=False):
+            return train_ops.torso_pass(self, image, weights_sum, bg_coords, bg_color, field, head_aware)
+
     @torch.no_grad()
     def update_extra_state(self, decay=0.95, S=128, *, pose_index=None, noise=None):
         """radnerf_torso.py:201-242 / radnerf_torso_sr.py:246-288: refreshes density_grid_torso and mean_density_torso only.  The
@@ -1162,6 +1191,15 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
                              lay.base_resolution, 1, False, 0)
         h = self._mlp(torch.cat([xf, h], dim=-1), self.torso_canonicial_net)
         return torch.sigmoid(h[..., :1]), torch.sigmoid(h[..., 1:]), dx
+
+    def _torso_pass_field(self, poses, c, lm68, dev):
+        """torso_pass's field: (xy, image, weights_sum) -> forward_torso's training field at the masked pixels; head-aware inputs iff
+        torso_head_aware.  `poses` is unused, as in forward_torso."""
+        if not torch.is_tensor(lm68) or lm68.numel() != 136:
+            raise ValueError("the torso-SR field is conditioned on lm68: one frame's 68 2-D landmarks (136 values)")
+        from . import train_ops
+        lm, params = lm68.to(dev), train_ops.torso_sr_params(self)
+        return (lambda xy, image, ws: train_ops.torso_sr_field(self, xy, lm, c, image, ws, *params)), self.torso_head_aware
 
     def _torso_native_state(self):
         """gfpp_torso_sr_pack once per (device, parameter versions)."""
@@ -1450,12 +1488,23 @@ class RADNeRFTorso(_TorsoGrid, RADNeRF):
             if (torch.is_tensor(x) and x.requires_grad) or (torch.is_tensor(poses) and poses.requires_grad):
                 raise NotImplementedError("gradients w.r.t. the torso positions or the head pose are not implemented")
             from . import train_ops
-            params = ([self.torso_deform_net.net[i].weight for i in range(3)] + [self.torso_canonicial_net.net[i].weight for i in range(3)] +
-                      [self.torso_embedder.embeddings])
             with torch.autocast("cuda", enabled=False):
-                return train_ops.torso_field(self, x.to(dev), poses.to(dev), None if c is None else c.to(dev), *params)
+                return train_ops.torso_field(self, x.to(dev), poses.to(dev), None if c is None else c.to(dev), *self._torso_field_params())
         with torch.no_grad():
             return self._forward_torso_eval(x, poses, c, dev)
+
+    def _torso_field_params(self):
+        """The parameters train_ops.torso_field takes: the six torso MLP weights, then the torso grid table."""
+        return ([self.torso_deform_net.net[i].weight for i in range(3)] + [self.torso_canonicial_net.net[i].weight for i in range(3)] +
+                [self.torso_embedder.embeddings])
+
+    def _torso_pass_field(self, poses, c, lm68, dev):
+        """torso_pass's field: (xy, image, weights_sum) -> forward_torso's training field at the masked pixels (no head-aware inputs)."""
+        if not torch.is_tensor(poses) or poses.numel() != 6:
+            raise ValueError("RADNeRFTorso.torso_pass takes one head pose [1,6] (convert_poses)")
+        from . import train_ops
+        p6, params = poses.to(dev), self._torso_field_params()
+        return (lambda xy, image, ws: train_ops.torso_field(self, xy, p6, c, *params)), False
 
     def _forward_torso_eval(self, x, poses, c, dev):
         _, _, model, _ = self._ensure_packed()

@@ -544,3 +544,115 @@ class _torso_sr_field(Function):
 
 
 torso_sr_field = _torso_sr_field.apply
+
+
+# ------------------------------------------------------------------------------------------------ the torso pass of the torso steps
+def _composite_forward(slot, M, alpha, color, img, ws, bg, bg_mode):
+    """gfpp_torso_composite_forward: (torso_alpha_map [N,1], torso_rgb_map [N,3], rgb_map [N,3]); alpha / color None iff M == 0."""
+    N, dev = slot.shape[0], slot.device
+    ta = torch.empty(N, 1, dtype=torch.float32, device=dev)
+    trgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
+    rgb = torch.empty(N, 3, dtype=torch.float32, device=dev)
+    _capi.check(_capi.lib().gfpp_torso_composite_forward(slot.data_ptr(), N, M, None if alpha is None else alpha.data_ptr(),
+                                                         None if color is None else color.data_ptr(), img.data_ptr(), ws.data_ptr(),
+                                                         None if bg is None else bg.data_ptr(), bg_mode, ta.data_ptr(), trgb.data_ptr(),
+                                                         rgb.data_ptr(), _capi.stream_ptr(dev)), "gfpp_torso_composite_forward")
+    return ta, trgb, rgb
+
+
+class _torso_composite(Function):
+    """The three-way composite of the torso steps (radnerf_torso.py:172-193) over gfpp_torso_composite_forward / _backward: the field's
+    alpha [M,1] and color [M,3] at the masked pixels (slot [N], idx [M] of gfpp_torso_mask), the head image [N,3], weights_sum [N] and
+    the background (bg_mode 0: None, 1: bg [3], 2: bg [N,3]) -> (torso_alpha_map [N,1], torso_rgb_map [N,3], rgb_map [N,3]).  Gradients
+    reach alpha and color only (the caller rejects other inputs that require one)."""
+
+    @staticmethod
+    def forward(ctx, slot, idx, img, ws, bg, bg_mode, alpha, color):
+        a, c = alpha.contiguous().reshape(-1), color.contiguous().reshape(-1, 3)
+        with torch.cuda.device(slot.device):
+            out = _composite_forward(slot, a.shape[0], a, c, img, ws, bg, bg_mode)
+        ctx.bg_mode = bg_mode
+        ctx.save_for_backward(idx, img, ws, bg if bg is not None else torch.empty(0, device=slot.device), a, c)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_ta, g_trgb, g_rgb):
+        idx, img, ws, bg, a, c = ctx.saved_tensors
+        N, M, dev = ws.shape[0], a.shape[0], a.device
+        grad_alpha = torch.empty(M, 1, dtype=torch.float32, device=dev)
+        grad_color = torch.empty(M, 3, dtype=torch.float32, device=dev)
+        ups = [None if g is None else _cuda_f32(g) for g in (g_ta, g_trgb, g_rgb)]
+        with torch.cuda.device(dev):
+            _capi.check(_capi.lib().gfpp_torso_composite_backward(
+                idx.data_ptr(), N, M, a.data_ptr(), c.data_ptr(), img.data_ptr(), ws.data_ptr(), bg.data_ptr() if ctx.bg_mode else None,
+                ctx.bg_mode, *[None if g is None else g.data_ptr() for g in ups], grad_alpha.data_ptr(), grad_color.data_ptr(),
+                _capi.stream_ptr(dev)), "gfpp_torso_composite_backward")
+        return None, None, None, None, None, None, grad_alpha, grad_color
+
+
+def _count_host(model):
+    """A pinned host int32 that receives M (kept on the model across calls)."""
+    h = model.__dict__.get("_torso_pass_count")
+    if h is None:
+        h = model.__dict__["_torso_pass_count"] = torch.empty(1, dtype=torch.int32, pin_memory=True)
+    return h
+
+
+def torso_pass(model, image, weights_sum, bg_coords, bg_color, field, head_aware):
+    """The torso part of the torso training steps (radnerf_torso.py:165-193, radnerf_torso_sr.py:196-221) on gfpp.h section M:
+    mask + compaction (gfpp_torso_mask), one device-to-host read of M, field(xy [M,2], image [M,3], weights_sum [M]) -> (alpha [M,1],
+    color [M,3], deform [M,2]) on the masked pixels (the autograd Function of section H or I; image and weights_sum gathered iff
+    head_aware, None otherwise), then the composite (_torso_composite).  Returns the composed recipe's dict: torso_alpha_map [N,1],
+    torso_rgb_map [N,3], rgb_map [N,3] (clamped), weights_sum [N] and, iff M > 0, deform [M,2].  With M == 0 no field runs and no
+    output requires grad (the reference's `if mask.any()`).  Sets model.last_launch_count.  Shapes are checked (ValueError) before
+    anything reaches the device; the caller has checked that nothing but the field's parameters requires grad."""
+    N = bg_coords.numel() // 2
+    if N == 0 or bg_coords.numel() != 2 * N or bg_coords.shape[-1] != 2:
+        raise ValueError(f"bg_coords must be [...,2] with at least one pixel, got shape {tuple(bg_coords.shape)}")
+    if image.numel() != 3 * N or weights_sum.numel() != N:
+        raise ValueError(f"image must hold {N}x3 values and weights_sum {N} (one per pixel of bg_coords), got shapes "
+                         f"{tuple(image.shape)} and {tuple(weights_sum.shape)}")
+    bg_mode = 0
+    if bg_color is not None:
+        bg_mode = 1 if bg_color.numel() == 3 else 2 if bg_color.numel() == 3 * N else -1
+        if bg_mode < 0:
+            raise ValueError(f"bg_color must be None, one colour (3 values) or one per pixel ({N}x3), got shape {tuple(bg_color.shape)}")
+    L = _capi.lib()
+    dev = model.density_bitfield.device
+    f32 = torch.float32
+    grid = model.density_grid_torso
+    if grid.dtype != f32 or not grid.is_contiguous() or grid.device != dev:
+        raise ValueError("density_grid_torso must be a contiguous fp32 buffer on the model's device")
+    xy = bg_coords.detach().to(dev, f32).reshape(N, 2).contiguous()
+    img = image.detach().to(dev, f32).reshape(N, 3).contiguous()
+    ws = weights_sum.detach().to(dev, f32).reshape(N).contiguous()
+    bg = None if bg_color is None else bg_color.detach().to(dev, f32).reshape(-1).contiguous()
+    i32 = torch.int32
+    idx, slot, count = torch.empty(N, dtype=i32, device=dev), torch.empty(N, dtype=i32, device=dev), torch.empty(1, dtype=i32, device=dev)
+    xy_m = torch.empty(N, 2, dtype=f32, device=dev)
+    img_m = torch.empty(N, 3, dtype=f32, device=dev) if head_aware else None
+    ws_m = torch.empty(N, dtype=f32, device=dev) if head_aware else None
+    work = _workspace(model, "_torso_pass_ws", L.gfpp_torso_pass_workspace_bytes, N, "the torso pass")
+    # the mask threshold as PyTorch compares it: the Python float min() rounded to float32 (the c_float argument)
+    thr = float(min(model.density_thresh_torso, model.mean_density_torso))
+    host = _count_host(model)
+    with torch.cuda.device(dev):
+        _capi.check(L.gfpp_torso_mask(grid.data_ptr(), model.grid_size, thr, xy.data_ptr(), N, img.data_ptr() if head_aware else None,
+                                      ws.data_ptr() if head_aware else None, idx.data_ptr(), slot.data_ptr(), xy_m.data_ptr(),
+                                      None if img_m is None else img_m.data_ptr(), None if ws_m is None else ws_m.data_ptr(), count.data_ptr(),
+                                      work.data_ptr(), work.numel(), _capi.stream_ptr(dev)), "gfpp_torso_mask")
+        launches = int(L.gfpp_last_launch_count())
+        host.copy_(count, non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+        done.synchronize()               # the one host sync of the pass: M sizes the field's launch and its outputs
+        M = int(host[0])
+        if M == 0:
+            ta, trgb, rgb = _composite_forward(slot, 0, None, None, img, ws, bg, bg_mode)
+            model.last_launch_count = launches + 1
+            return {"torso_alpha_map": ta, "torso_rgb_map": trgb, "rgb_map": rgb, "weights_sum": ws}
+    alpha, color, deform = field(xy_m[:M], None if img_m is None else img_m[:M], None if ws_m is None else ws_m[:M])
+    launches += int(L.gfpp_last_launch_count())
+    ta, trgb, rgb = _torso_composite.apply(slot, idx[:M], img, ws, bg, bg_mode, alpha, color)
+    model.last_launch_count = launches + 1
+    return {"torso_alpha_map": ta, "torso_rgb_map": trgb, "rgb_map": rgb, "weights_sum": ws, "deform": deform}

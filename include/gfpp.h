@@ -45,6 +45,8 @@
  *  (K) the frozen head of the torso training steps.
  *
  *  (L) the grid encoder ops of (A) and (D) on half tables, as the reference runs them under autocast.
+ *
+ *  (M) the torso pass of the torso training steps: mask, compaction and composite between (K) and the fields of (H) / (I).
  */
 #ifndef GFPP_H_
 #define GFPP_H_
@@ -649,6 +651,51 @@ GFPP_API int gfpp_grid_encode_backward_half(const uint16_t *grad, const float *i
                                             uint16_t *grad_embeddings, uint32_t B, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H,
                                             const uint16_t *dy_dx, uint16_t *grad_inputs, uint32_t gridtype, int align_corners,
                                             uint32_t interp, void *stream);
+
+/* ------------------------------------------------------------------ (M) torso pass of the torso training steps
+ *
+ * The per-pixel code between the frozen head (K) and the torso fields (H) / (I) in the torso training steps of both torso models
+ * (radnerf_torso.py:165-193, radnerf_torso_sr.py:196-221): the grid_sample mask of density_grid_torso, the compaction of the
+ * masked pixels, and the three-way composite forward and backward.  The entry points take the grid and plain arrays, no model
+ * descriptor; the fields run unchanged on the compacted points with a host M.  A step is: gfpp_torso_mask, one read of *count,
+ * the field's forward, gfpp_torso_composite_forward; then gfpp_torso_composite_backward and the field's backward.
+ *
+ * gfpp_torso_mask: pixel i of bg_coords [N,2] (8-byte aligned) is masked iff grid_sample(density_grid_torso [G,G], bg_coords[i],
+ *   align_corners=True, bilinear, zeros padding) > thr, in ATen's grid_sampler_2d arithmetic.  thr is the fp32 value of
+ *   min(density_thresh_torso, mean_density_torso): PyTorch compares a float32 tensor with a Python float scalar in float32, so the
+ *   double is rounded to the nearest float first (what a C float argument does).  Outputs, with M the number of masked pixels:
+ *     idx [N] (first M written): the masked pixel indices in ascending order -- the order of bg_coords[mask];
+ *     slot [N]: the compacted row of each pixel, or -1;  xy [M,2] (8-byte aligned) = bg_coords[mask];
+ *     image_m [M,3] = image[mask] and weights_sum_m [M] = weights_sum[mask]: the SR field's head-aware inputs, all four of image
+ *       [N,3], weights_sum [N], image_m and weights_sum_m given, or all NULL;
+ *     *count = M (device int32).
+ *   Three launches (tile counts, a one-CTA scan of the counts, a tile-local scan that writes); no atomics, so every output is
+ *   bit-identical from run to run.  Workspace: gfpp_torso_pass_workspace_bytes(N), 256-byte aligned (the tile counts).
+ * gfpp_torso_composite_forward: one thread per pixel; a = alpha[slot[i]] and c = color[slot[i]] (alpha [M], color [M,3]; 0 where
+ *   slot is -1; both may be NULL iff M == 0), bg the scalar 1 (bg_mode 0, bg_color NULL: bg_color=None), one colour (bg_mode 1,
+ *   bg_color [3]) or one colour per pixel (bg_mode 2, bg_color [N,3]):
+ *     torso_alpha_map [N] = a;  torso_rgb_map [N,3] = c*a + bg*(1-a);  rgb_map [N,3] = clamp(image + (1-weights_sum)*torso_rgb_map, 0, 1)
+ *   in PyTorch's op order with every product and sum rounded separately: bit-identical to the composed recipe (zeros, index_put,
+ *   the composite and the clamp in eager PyTorch).
+ * gfpp_torso_composite_backward: one thread per masked point j < M, pixel idx[j]: given the upstream gradients of torso_alpha_map
+ *   [N], torso_rgb_map [N,3] and rgb_map [N,3] (each may be NULL: zero), writes grad_alpha [M] and grad_color [M,3], the inputs of
+ *   the fields' backward.  The clamp passes the gradient where 0 <= x <= 1 (torch.clamp), x recomputed with the forward's
+ *   arithmetic.  M == 0 returns GFPP_OK without touching the device (idx and the gradient pointers may then be NULL).
+ * Validation (before any CUDA call): NULL pointers, N == 0 -> GFPP_ERR_INVALID; N >= 2^31, G outside 2..4096 ->
+ * GFPP_ERR_UNSUPPORTED; M > N, bg_mode outside 0..2 or bg_color given iff bg_mode == 0 -> GFPP_ERR_INVALID; a workspace below
+ * gfpp_torso_pass_workspace_bytes(N) -> GFPP_ERR_WORKSPACE, or not 256-byte aligned -> GFPP_ERR_INVALID.  Stream-ordered, no host
+ * sync, no allocation.  gfpp_torso_pass_workspace_bytes returns 0 for N == 0 or N >= 2^31. */
+GFPP_API size_t gfpp_torso_pass_workspace_bytes(uint32_t N);
+GFPP_API int gfpp_torso_mask(const float *density_grid_torso, uint32_t G, float thr, const float *bg_coords, uint32_t N, const float *image,
+                             const float *weights_sum, int32_t *idx, int32_t *slot, float *xy, float *image_m, float *weights_sum_m,
+                             int32_t *count, void *workspace, size_t workspace_bytes, void *stream);
+GFPP_API int gfpp_torso_composite_forward(const int32_t *slot, uint32_t N, uint32_t M, const float *alpha, const float *color,
+                                          const float *image, const float *weights_sum, const float *bg_color, uint32_t bg_mode,
+                                          float *torso_alpha_map, float *torso_rgb_map, float *rgb_map, void *stream);
+GFPP_API int gfpp_torso_composite_backward(const int32_t *idx, uint32_t N, uint32_t M, const float *alpha, const float *color,
+                                           const float *image, const float *weights_sum, const float *bg_color, uint32_t bg_mode,
+                                           const float *grad_torso_alpha_map, const float *grad_torso_rgb_map, const float *grad_rgb_map,
+                                           float *grad_alpha, float *grad_color, void *stream);
 
 #ifdef __cplusplus
 }
