@@ -108,6 +108,7 @@ EXPORTS = [
     "gfpp_frozen_head_workspace_bytes", "gfpp_frozen_head",
     "gfpp_grid_encode_forward_half", "gfpp_grid_encode_backward_half",
     "gfpp_torso_pass_workspace_bytes", "gfpp_torso_mask", "gfpp_torso_composite_forward", "gfpp_torso_composite_backward",
+    "gfpp_rgb_u8_to_i420",
 ]
 
 
@@ -214,6 +215,7 @@ def lib():
         L.gfpp_torso_mask.argtypes = [P, c_u32, c_f, P, c_u32, P, P, P, P, P, P, P, P, P, c_size_t, P]
         L.gfpp_torso_composite_forward.argtypes = [P, c_u32, c_u32, P, P, P, P, P, c_u32, P, P, P, P]
         L.gfpp_torso_composite_backward.argtypes = [P, c_u32, c_u32, P, P, P, P, P, c_u32, P, P, P, P, P, P]
+        L.gfpp_rgb_u8_to_i420.argtypes = [P, c_u32, c_u32, c_u32, P, P]
         _lib = L
     return _lib
 

@@ -72,6 +72,8 @@ cudaError_t launch_torso_composite_fwd(const int32_t *, uint32_t, const float *,
                                        uint32_t, float *, float *, float *, cudaStream_t);
 cudaError_t launch_torso_composite_bwd(const int32_t *, uint32_t, const float *, const float *, const float *, const float *, const float *,
                                        uint32_t, const float *, const float *, const float *, float *, float *, cudaStream_t);
+// video_kernels.cu
+cudaError_t launch_rgb_u8_to_i420(const uint8_t *, uint32_t, uint32_t, uint32_t, uint8_t *, cudaStream_t);
 }  // namespace gfpp
 
 using namespace gfpp;
@@ -2098,6 +2100,21 @@ int gfpp_torso_composite_backward(const int32_t *idx, uint32_t N, uint32_t M, co
     if (M == 0) return GFPP_OK;
     CK(launch_torso_composite_bwd(idx, M, alpha, color, image, weights_sum, bg_color, bg_mode, grad_torso_alpha_map, grad_torso_rgb_map,
                                   grad_rgb_map, grad_alpha, grad_color, (cudaStream_t)stream));
+    return GFPP_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------- (N) planar I420 video frames
+extern "C" {
+
+int gfpp_rgb_u8_to_i420(const uint8_t *rgb, uint32_t F, uint32_t H, uint32_t W, uint8_t *out, void *stream) {
+    if (!rgb || !out) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: null pointer%s");
+    if (F == 0) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: no frames%s");
+    if (H == 0 || W == 0 || (H | W) & 1u) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: H and W must be even and non-zero (4:2:0 subsampling)%s");
+    if ((uint64_t)H * W > SIZE_MAX / 3 / F) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: F*H*W*3 bytes overflow size_t%s");
+    g_launches = 0;
+    CK(launch_rgb_u8_to_i420(rgb, F, H, W, out, (cudaStream_t)stream));
     return GFPP_OK;
 }
 

@@ -97,7 +97,10 @@ def render_clip_sharded(model, poses_c2w, intrinsics, H, W, cond_seq, *, bg_colo
     `cond_seq` (and `eye_area_percent` [T] for the blink-conditioned models) is the FULL sequence on every rank -- the +-2-frame
     smoothing window needs its halo; it is tiny -- so conditioning features at block edges equal the single-GPU ones.  Per-frame
     inputs of the SR models (`lm68_seq` [T,136]) are sliced to the rank's block; `render_kw` goes to `render_clip` unchanged
-    (`sr_noise_mode=...`).  Works for all four model classes: [T,N,3] frames for the plain models, [T,3,512,512] for the SR ones."""
+    (`sr_noise_mode=...`).  Works for all four model classes: [T,N,3] frames for the plain models, [T,3,512,512] for the SR ones.
+    The I420 frames of render_clip(as_yuv420=True) are not offered here: convert gathered uint8 frames with video.rgb_u8_to_i420."""
+    if render_kw.get("as_yuv420"):
+        raise ValueError("render_clip_sharded does not produce I420 frames: convert gathered uint8 frames with video.rgb_u8_to_i420")
     T = poses_c2w.shape[0]
     world = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
     rank = dist.get_rank(group) if world > 1 else 0

@@ -22,9 +22,13 @@ with only two chunks of frames alive at any time.
 With as_rgba=True both return alpha-matte frames [..,H,W,4] instead (non-SR models): premultiplied colour P and coverage A as
 `(x*255).int()`, with no background in them (the batch's `bg_img` is not read), so that P + (1 - A) * B puts the head over any
 background B, e.g. a different one per frame.
+
+With as_yuv420=True both return the as_uint8 frames as planar I420 [.., H*W*3/2] (all four model classes; video.py), ready for
+`ffmpeg -f rawvideo -pix_fmt yuv420p -s WxH -r 25 -i -` at half the bytes per frame.
 """
 import torch
 
+from . import video
 from .dist import to_uint8
 from .renderer import _no_sr_matte
 
@@ -71,10 +75,14 @@ def _render_kw(model, T_thresh, dt_gamma, max_steps):
             "T_thresh": T_thresh}
 
 
-def _check_formats(model, as_uint8, as_rgba):
+def _check_formats(model, batch, as_uint8, as_rgba, as_yuv420):
     if as_rgba and as_uint8:
         raise ValueError("as_rgba and as_uint8 are two different frame formats: pick one")
+    if as_yuv420 and (as_uint8 or as_rgba):
+        raise ValueError("as_yuv420 is a frame format of its own: it cannot be combined with as_uint8 or as_rgba")
     _no_sr_matte(as_rgba and _is_sr(model))
+    if as_yuv420:
+        video.check_i420_size(*_frame_hw(model, batch))
 
 
 def _render_chunk(model, batch, feat, s, e, kw, out=None, out_u8=None, out_rgba=None, sr_noise_mode="random"):
@@ -104,19 +112,34 @@ def _render_chunk(model, batch, feat, s, e, kw, out=None, out_u8=None, out_rgba=
         model.sr_net.forward_native(img, noise_mode=sr_noise_mode, clamp=True, out=out, u8_out=out_u8, frames_per_call=e - s)
 
 
+def _render_chunk_i420(model, batch, feat, s, e, kw, H, W, out, sr_noise_mode):
+    """Frames [s, e) as I420 into out [e-s, H*W*3/2]: _render_chunk's uint8 frames, written to the model's scratch buffer, converted."""
+    frames = video.frame_scratch(model, (e - s, H, W, 3))
+    _render_chunk(model, batch, feat, s, e, kw, out_u8=frames, sr_noise_mode=sr_noise_mode)
+    video.rgb_u8_to_i420(frames, H, W, out=out)
+
+
 @torch.no_grad()
 def render_driver_batch(model, batch, T_thresh=1e-2, frames_per_call=32, dt_gamma=None, max_steps=None, as_uint8=False,
-                        sr_noise_mode="random", as_rgba=False):
+                        sr_noise_mode="random", as_rgba=False, as_yuv420=False):
     """-> [T,3,H,W] fp32 in [0,1] on the model's device (H = W = sqrt(N); SR models: the 512x512 `sr_rgb_map` frames), or with
     as_uint8 the video frames uint8 [T,H,W,3] `(rgb*255).int()`, written by the last kernel itself, or with as_rgba (non-SR models)
-    the alpha-matte frames uint8 [T,H,W,4] of render_frames' rgba_out.  SR models take the batch's `lm68` [T,136] (torso-SR) and
-    render at most SR_FRAMES_PER_CALL frames per call; sr_noise_mode as render()'s."""
-    _check_formats(model, as_uint8, as_rgba)
+    the alpha-matte frames uint8 [T,H,W,4] of render_frames' rgba_out, or with as_yuv420 the as_uint8 frames as planar I420
+    uint8 [T,H*W*3/2] (H and W even).  SR models take the batch's `lm68` [T,136] (torso-SR) and render at most SR_FRAMES_PER_CALL
+    frames per call; sr_noise_mode as render()'s."""
+    _check_formats(model, batch, as_uint8, as_rgba, as_yuv420)
     T = len(batch["poses"])
     dev = model.density_bitfield.device
     feat = cond_feat_from_windows(model, batch["cond_wins"], batch.get("eye_area_percent"))
     H, W = _frame_hw(model, batch)
     kw = _render_kw(model, T_thresh, dt_gamma, max_steps)
+    if as_yuv420:
+        fpc = min(frames_per_call, SR_FRAMES_PER_CALL) if _is_sr(model) else frames_per_call
+        out = torch.empty(T, video.i420_frame_bytes(H, W), device=dev, dtype=torch.uint8)
+        for s in range(0, T, fpc):
+            e = min(T, s + fpc)
+            _render_chunk_i420(model, batch, feat, s, e, kw, H, W, out[s:e], sr_noise_mode)
+        return out
     if _is_sr(model):
         fpc = min(frames_per_call, SR_FRAMES_PER_CALL)
         out = torch.empty((T, H, W, 3) if as_uint8 else (T, 3, H, W), device=dev, dtype=torch.uint8 if as_uint8 else torch.float32)
@@ -145,16 +168,18 @@ def _pinned(shape):
 
 @torch.no_grad()
 def iter_video_frames(model, batch, frames_per_call=8, T_thresh=1e-2, dt_gamma=None, max_steps=None, sr_noise_mode="random",
-                      as_rgba=False):
+                      as_rgba=False, as_yuv420=False):
     """The `low_memory_usage` loop of forward_secc2video (genefacepp_infer.py:449-470) for all four model classes: yields the
     clip's video frames -- what render_driver_batch(..., as_uint8=True) returns -- as host uint8 [n,H,W,3] chunks in frame order
     (n <= frames_per_call; SR models: <= SR_FRAMES_PER_CALL), e.g. `for c in iter_video_frames(...): for f in c.numpy(): writer.append_data(f)`.
     as_rgba (non-SR models): the alpha-matte frames of render_driver_batch(..., as_rgba=True) instead, as [n,H,W,4] chunks.
+    as_yuv420: the I420 frames of render_driver_batch(..., as_yuv420=True), as [n,H*W*3/2] chunks, each one write to an ffmpeg
+    rawvideo pipe (`proc.stdin.write(c.numpy().tobytes())`).
 
     Two device and two pinned host buffers: chunk k+1 renders on the current stream while chunk k is copied to the host on a
     side stream and handed to the caller.  A yielded chunk stays valid until the generator is advanced.  When the generator
     ends, fails or is closed early, it waits for both streams: no queued work is left behind."""
-    _check_formats(model, False, as_rgba)
+    _check_formats(model, batch, False, as_rgba, as_yuv420)
     T = len(batch["poses"])
     dev = model.density_bitfield.device
     feat = cond_feat_from_windows(model, batch["cond_wins"], batch.get("eye_area_percent"))
@@ -165,9 +190,9 @@ def iter_video_frames(model, batch, frames_per_call=8, T_thresh=1e-2, dt_gamma=N
     compute = torch.cuda.current_stream(dev)
     side = torch.cuda.Stream(dev)
     rows = min(fpc, T)
-    C = 4 if as_rgba else 3
-    dbuf = [torch.empty(rows, H, W, C, device=dev, dtype=torch.uint8) for _ in range(2)]
-    hbuf = [_pinned((rows, H, W, C)) for _ in range(2)]
+    shape = (rows, video.i420_frame_bytes(H, W)) if as_yuv420 else (rows, H, W, 4 if as_rgba else 3)
+    dbuf = [torch.empty(shape, device=dev, dtype=torch.uint8) for _ in range(2)]
+    hbuf = [_pinned(shape) for _ in range(2)]
     rendered = [torch.cuda.Event() for _ in range(2)]
     copied = [torch.cuda.Event() for _ in range(2)]
 
@@ -176,8 +201,11 @@ def iter_video_frames(model, batch, frames_per_call=8, T_thresh=1e-2, dt_gamma=N
         s, b = starts[k], k % 2
         e = min(T, s + fpc)
         compute.wait_event(copied[b])           # chunk k-2 has left device buffer b
-        dst = {"out_rgba": dbuf[b][:e - s]} if as_rgba else {"out_u8": dbuf[b][:e - s]}
-        _render_chunk(model, batch, feat, s, e, kw, sr_noise_mode=sr_noise_mode, **dst)
+        if as_yuv420:
+            _render_chunk_i420(model, batch, feat, s, e, kw, H, W, dbuf[b][:e - s], sr_noise_mode)
+        else:
+            dst = {"out_rgba": dbuf[b][:e - s]} if as_rgba else {"out_u8": dbuf[b][:e - s]}
+            _render_chunk(model, batch, feat, s, e, kw, sr_noise_mode=sr_noise_mode, **dst)
         rendered[b].record(compute)
         side.wait_event(rendered[b])
         with torch.cuda.stream(side):

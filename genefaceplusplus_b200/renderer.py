@@ -30,7 +30,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import _capi
+from . import _capi, video
 from .config import GridLayout, cascade_count
 
 
@@ -801,45 +801,54 @@ class RADNeRF(nn.Module):
     @torch.no_grad()
     def render_clip(self, poses_c2w, intrinsics, H, W, cond_seq=None, cond_feat=None, bg_color=None, bg_coords=None, pose6=None,
                     dt_gamma=None, max_steps=None, T_thresh=1e-2, frames_per_call=64, out=None, want_stats=False,
-                    eye_area_percent=None, as_uint8=False, as_rgba=False):
+                    eye_area_percent=None, as_uint8=False, as_rgba=False, as_yuv420=False):
         """Render a clip: poses_c2w [T,4,4], cond_seq [T,1,C] (or precomputed cond_feat [T,64]); eye_area_percent [T] for
         add_eye_blink_cond models.  Returns rgb [T,H*W,3] on the model's device: fp32 clamped to [0,1], or -- as_uint8 -- the
         uint8 video frames `(rgb*255).int()` (genefacepp_infer.py:469,505) written by the epilogue kernel itself, or -- as_rgba --
         uint8 [T,H*W,4] alpha-matte frames: premultiplied colour P and coverage A, each `(x*255).int()`, so that P + (1 - A) * B is
-        the frame over any background B (render_frames' rgba_out).  The matte is defined without a background: as_rgba with
-        bg_color, or with as_uint8, raises ValueError.  `out`: optional preallocated result buffer of that dtype and shape; every
-        call writes its frames straight into it."""
+        the frame over any background B (render_frames' rgba_out), or -- as_yuv420 -- uint8 [T,H*W*3/2] planar I420 frames, the
+        as_uint8 frames converted on the GPU (video.rgb_u8_to_i420; H and W must be even).  The matte is defined without a
+        background: as_rgba with bg_color raises ValueError, as does asking for two of the three formats.  `out`: optional
+        preallocated result buffer of that dtype and shape; every call writes its frames straight into it (as_yuv420: each call's
+        uint8 frames go to a scratch buffer the model keeps, then are converted into `out`)."""
         if as_rgba and as_uint8:
             raise ValueError("as_rgba and as_uint8 are two different frame formats: pick one")
+        if as_yuv420 and (as_uint8 or as_rgba):
+            raise ValueError("as_yuv420 is a frame format of its own: it cannot be combined with as_uint8 or as_rgba")
         if as_rgba and bg_color is not None:
             raise ValueError("as_rgba returns the frame's matte, which does not depend on a background: composite P + (1 - A) * B "
                              "instead of passing bg_color")
+        if as_yuv420:
+            video.check_i420_size(H, W)
         dev = self.density_bitfield.device
         T = poses_c2w.shape[0]
         hp = self.hparams
         dt_gamma = hp["dt_gamma"] if dt_gamma is None else dt_gamma
         max_steps = hp["max_steps"] if max_steps is None else max_steps
         N = H * W
-        odt = torch.uint8 if as_uint8 or as_rgba else torch.float32
-        C = 4 if as_rgba else 3
-        rgb = out if out is not None else torch.empty(T, N, C, device=dev, dtype=odt)
-        if rgb.dtype != odt or rgb.numel() != T * N * C or not rgb.is_contiguous():
-            raise ValueError(f"out must be a contiguous {odt} [{T},{N},{C}] tensor")
-        rgb = rgb.view(T, N, C)
+        odt = torch.uint8 if as_uint8 or as_rgba or as_yuv420 else torch.float32
+        shape = (T, video.i420_frame_bytes(H, W)) if as_yuv420 else (T, N, 4 if as_rgba else 3)
+        rgb = out if out is not None else torch.empty(shape, device=dev, dtype=odt)
+        if rgb.dtype != odt or rgb.numel() != math.prod(shape) or not rgb.is_contiguous():
+            raise ValueError(f"out must be a contiguous {odt} [{','.join(map(str, shape))}] tensor")
+        rgb = rgb.view(shape)
         if cond_feat is None:
             cond_feat = self.cal_cond_feat_clip(cond_seq.to(dev), eye_area_percent=eye_area_percent if self.forwards_eye_area else None)
         poses_c2w = poses_c2w.to(dev, torch.float32)
         if self.has_torso and pose6 is None:
             from .scene import convert_poses
             pose6 = convert_poses(poses_c2w.cpu()).to(dev)
-        dst = "rgba_out" if as_rgba else "u8_out" if as_uint8 else "rgb_out"
+        dst = "rgba_out" if as_rgba else "u8_out" if as_uint8 or as_yuv420 else "rgb_out"
         stats = []
         for s in range(0, T, frames_per_call):
             e = min(T, s + frames_per_call)
+            buf = video.frame_scratch(self, (e - s, N, 3)) if as_yuv420 else rgb[s:e]
             res = self.render_frames(cond_feat[s:e], poses_c2w=poses_c2w[s:e], intrinsics=intrinsics, H=H, W=W,
                                      pose6=pose6[s:e] if self.has_torso else None, bg_coords=bg_coords, bg_color=bg_color,
                                      dt_gamma=dt_gamma, max_steps=max_steps, T_thresh=T_thresh, want_torso_maps=False,
-                                     want_stats=want_stats, want_aux=False, **{dst: rgb[s:e]})
+                                     want_stats=want_stats, want_aux=False, **{dst: buf})
+            if as_yuv420:
+                video.rgb_u8_to_i420(buf, H, W, out=rgb[s:e])
             if want_stats:
                 stats.append(res["stats"])
         if want_stats:
@@ -848,6 +857,15 @@ class RADNeRF(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------ head model + super-resolution
+def _i420_out(out, T, S, dev):
+    """The I420 result buffer [T,S*S*3/2] of an SR clip (S = 512): `out` checked, or a new one."""
+    shape = (T, video.i420_frame_bytes(S, S))
+    out = out if out is not None else torch.empty(shape, device=dev, dtype=torch.uint8)
+    if out.shape != shape or out.dtype != torch.uint8 or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous uint8 [{T},{shape[1]}] tensor")
+    return out
+
+
 def _no_sr_matte(as_rgba):
     """The SR head is not linear in its input, so no alpha composes its 512x512 frame from the NeRF's matte: the SR models have
     no as_rgba output."""
@@ -884,20 +902,26 @@ class RADNeRFwithSR(RADNeRF):
 
     @torch.no_grad()
     def render_clip(self, poses_c2w, intrinsics, H=256, W=256, *args, sr_noise_mode="random", sr_frames_per_call=8, as_uint8=False,
-                    as_rgba=False, **kwargs):
+                    as_rgba=False, as_yuv420=False, **kwargs):
         """Clip API: NeRF at 256x256 for all frames (libgfpp), then the SR head over chunks of frames.
         Returns the clamped 512x512 frames [T,3,512,512]; `intrinsics` are those of the 256x256 camera.
         as_uint8: returns the video frames uint8 [T,512,512,3] (HWC) `(rgb*255).int()` instead, written by the SR head's last
         kernel chunk by chunk into `out` (optional preallocated buffer of that shape); the NeRF stage still renders fp32, the
-        SR head's input.  Without as_uint8, `out` is the NeRF clip's buffer ([T,256*256,3] fp32), as in RADNeRF.render_clip.
-        as_rgba raises ValueError (_no_sr_matte)."""
+        SR head's input.  as_yuv420: the same frames as planar I420, uint8 [T,512*512*3/2] (video.rgb_u8_to_i420), each SR chunk's
+        uint8 frames converted from a scratch buffer the model keeps into `out`; the noise planes are drawn as with as_uint8.
+        Without either, `out` is the NeRF clip's buffer ([T,256*256,3] fp32), as in RADNeRF.render_clip.
+        as_rgba raises ValueError (_no_sr_matte), and so does as_yuv420 with as_uint8."""
         _no_sr_matte(as_rgba)
+        if as_yuv420 and as_uint8:
+            raise ValueError("as_yuv420 is a frame format of its own: it cannot be combined with as_uint8 or as_rgba")
         from .dist import to_uint8
         R = self.sr_input_resolution
         if (H, W) != (R, R):
             raise ValueError(f"SR models render the NeRF at {R}x{R} (radnerf_sr.py:205)")
         want_stats = kwargs.get("want_stats", False)
-        u8 = kwargs.pop("out", None) if as_uint8 else None
+        u8 = kwargs.pop("out", None) if as_uint8 or as_yuv420 else None
+        if as_yuv420:
+            u8 = _i420_out(u8, poses_c2w.shape[0], 2 * R, self.density_bitfield.device)
         res = super().render_clip(poses_c2w, intrinsics, H, W, *args, **kwargs)
         rgb, stats = res if want_stats else (res, None)
         T = rgb.shape[0]
@@ -906,9 +930,16 @@ class RADNeRFwithSR(RADNeRF):
             if u8.shape != (T, 2 * R, 2 * R, 3) or u8.dtype != torch.uint8 or not u8.is_contiguous():
                 raise ValueError(f"out must be a contiguous uint8 [{T},{2 * R},{2 * R},3] tensor")
         native = rgb.is_cuda and self.sr_net.backend == "native"
-        out = None if as_uint8 and native else torch.empty(T, 3, 2 * R, 2 * R, device=rgb.device, dtype=torch.float32)
+        out = None if (as_uint8 or as_yuv420) and native else torch.empty(T, 3, 2 * R, 2 * R, device=rgb.device, dtype=torch.float32)
         with torch.autocast(rgb.device.type, enabled=False):
-            if native:
+            if native and as_yuv420:
+                # chunk by chunk as forward_native would go, so the noise planes are drawn in the same order and shapes
+                for s in range(0, T, sr_frames_per_call):
+                    e = min(T, s + sr_frames_per_call)
+                    frames = video.frame_scratch(self, (e - s, 2 * R, 2 * R, 3))
+                    self.sr_net.forward_native(rgb[s:e], noise_mode=sr_noise_mode, clamp=True, frames_per_call=sr_frames_per_call, u8_out=frames)
+                    video.rgb_u8_to_i420(frames, 2 * R, 2 * R, out=u8[s:e])
+            elif native:
                 # libgfpp's SR kernels read the renderer's [T,N,3] frames as they are and clamp in their last epilogue
                 self.sr_net.forward_native(rgb, noise_mode=sr_noise_mode, clamp=True, out=out, frames_per_call=sr_frames_per_call, u8_out=u8)
             else:
@@ -917,7 +948,9 @@ class RADNeRFwithSR(RADNeRF):
                     out[s:e] = self.sr_net(rgb[s:e].view(e - s, R, R, 3).permute(0, 3, 1, 2), noise_mode=sr_noise_mode).clamp(0, 1)
                     if as_uint8:
                         u8[s:e] = to_uint8(out[s:e].permute(0, 2, 3, 1))
-        out = u8 if as_uint8 else out
+                    elif as_yuv420:
+                        video.rgb_u8_to_i420(to_uint8(out[s:e].permute(0, 2, 3, 1)).contiguous(), 2 * R, 2 * R, out=u8[s:e])
+        out = u8 if as_uint8 or as_yuv420 else out
         return (out, stats) if want_stats else out
 
 
@@ -1367,15 +1400,19 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
     @torch.no_grad()
     def render_clip(self, poses_c2w, intrinsics, H=256, W=256, cond_seq=None, bg_color=None, bg_coords=None, lm68_seq=None,
                     eye_area_percent=None, dt_gamma=None, max_steps=None, T_thresh=1e-2, sr_noise_mode="random", cond_feat=None,
-                    as_uint8=False, as_rgba=False, **unused):
+                    as_uint8=False, as_rgba=False, as_yuv420=False, **unused):
         """Clip API of the torso-SR model -> the clamped 512x512 frames [T,3,512,512].  With the native backends (the default) every
         stage runs in libgfpp chunk by chunk -- head field with rays generated in-kernel, torso-SR field + composite, SR head -- with
         no per-frame host work; with a "torch" backend it falls back to frame-by-frame `render()`.  poses_c2w [T,4,4] (c2w,
         dataset.poses), cond_seq [T,1,C] (or cond_feat [T,64] precomputed), lm68_seq [T,136], eye_area_percent [T] or None.
         as_uint8: returns the video frames uint8 [T,512,512,3] (HWC) `(rgb*255).int()` instead, written by the SR head's last kernel
         chunk by chunk into `out` (optional preallocated buffer of that shape); no fp32 512x512 frame is written then.
-        as_rgba raises ValueError (_no_sr_matte)."""
+        as_yuv420: the same frames as planar I420, uint8 [T,512*512*3/2] (video.rgb_u8_to_i420), each chunk's uint8 frames
+        converted from a scratch buffer the model keeps into `out`; the noise planes are drawn as with as_uint8.
+        as_rgba raises ValueError (_no_sr_matte), and so does as_yuv420 with as_uint8."""
         _no_sr_matte(as_rgba)
+        if as_yuv420 and as_uint8:
+            raise ValueError("as_yuv420 is a frame format of its own: it cannot be combined with as_uint8 or as_rgba")
         from .dist import to_uint8
         from .scene import cond_window, convert_poses, get_rays
         R = self.sr_input_resolution
@@ -1391,7 +1428,8 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
             u8 = u8 if u8 is not None else torch.empty(T, 2 * R, 2 * R, 3, device=dev, dtype=torch.uint8)
             if u8.shape != (T, 2 * R, 2 * R, 3) or u8.dtype != torch.uint8 or not u8.is_contiguous():
                 raise ValueError(f"out must be a contiguous uint8 [{T},{2 * R},{2 * R},3] tensor")
-        out = None if as_uint8 and native else torch.empty(T, 3, 2 * R, 2 * R, device=dev, dtype=torch.float32)
+        yuv = _i420_out(unused.get("out"), T, 2 * R, dev) if as_yuv420 else None
+        out = None if (as_uint8 or as_yuv420) and native else torch.empty(T, 3, 2 * R, 2 * R, device=dev, dtype=torch.float32)
         if native:
             # everything in libgfpp, chunk by chunk: head field (rays generated in-kernel, background 0 => premultiplied colour),
             # torso-SR field + composite, SR head; no per-frame host work
@@ -1408,9 +1446,12 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
                                             max_steps=hp["max_steps"] if max_steps is None else max_steps, T_thresh=T_thresh)
                     tr = self.torso_composite_native(hd["rgb_map"], hd["weights_sum"], lm68_seq[s:e].reshape(e - s, 136), bg_coords, bg_color,
                                                      want_maps=False)
+                    frames = video.frame_scratch(self, (e - s, 2 * R, 2 * R, 3)) if as_yuv420 else None if u8 is None else u8[s:e]
                     self.sr_net.forward_native(tr["rgb_map"], noise_mode=sr_noise_mode, clamp=True, out=None if out is None else out[s:e],
-                                               frames_per_call=fpc, u8_out=None if u8 is None else u8[s:e])
-            return u8 if as_uint8 else out
+                                               frames_per_call=fpc, u8_out=frames)
+                    if as_yuv420:
+                        video.rgb_u8_to_i420(frames, 2 * R, 2 * R, out=yuv[s:e])
+            return yuv if as_yuv420 else u8 if as_uint8 else out
         if cond_seq is None:
             raise ValueError("the frame-by-frame host path of the torso-SR clip needs cond_seq (cond_feat is only taken by the all-native path)")
         for t in range(T):
@@ -1424,7 +1465,9 @@ class RADNeRFTorsowithSR(_TorsoGrid, RADNeRF):
             out[t] = res["sr_rgb_map"][0]
             if as_uint8:
                 u8[t] = to_uint8(out[t].permute(1, 2, 0))
-        return u8 if as_uint8 else out
+            elif as_yuv420:
+                video.rgb_u8_to_i420(to_uint8(out[t].permute(1, 2, 0)).contiguous(), 2 * R, 2 * R, out=yuv[t:t + 1])
+        return yuv if as_yuv420 else u8 if as_uint8 else out
 
 
 # ------------------------------------------------------------------------------------------------ torso model

@@ -697,6 +697,24 @@ GFPP_API int gfpp_torso_composite_backward(const int32_t *idx, uint32_t N, uint3
                                            const float *grad_torso_alpha_map, const float *grad_torso_rgb_map, const float *grad_rgb_map,
                                            float *grad_alpha, float *grad_color, void *stream);
 
+/* ------------------------------------------------------------------ (N) planar I420 video frames
+ *
+ * gfpp_rgb_u8_to_i420 converts F interleaved uint8 RGB frames rgb [F,H,W,3] (the rgb_u8 frames of gfpp_render_frames, the video
+ * frames of gfpp_sr_forward_video) to F planar yuv420p frames, ffmpeg's rawvideo layout, one after the other in out:
+ *   frame f at out + f*H*W*3/2:  Y [H,W], then U [H/2,W/2], then V [H/2,W/2].
+ * BT.601 limited range in integer arithmetic (>> is an arithmetic shift, i.e. floor division by 256):
+ *   Y = ((66 R + 129 G + 25 B + 128) >> 8) + 16                          per pixel, 16..235
+ *   R', G', B' = (sum of the 2x2 block's four values + 2) >> 2           per 2x2 block and channel (box average)
+ *   U = ((-38 R' - 74 G' + 112 B' + 128) >> 8) + 128                     per 2x2 block, 16..240
+ *   V = ((112 R' - 94 G' - 18 B' + 128) >> 8) + 128
+ * The chroma of a block is its box average, so it is sited at the centre of its four luma samples (MPEG-1 / JPEG siting, not the
+ * left siting that H.264 decoders assume by default).  The bytes are not those of ffmpeg's swscale conversion, whose rounding and
+ * chroma filter differ.  rgb and out must not overlap.  Rows whose width is a multiple of 4 with both buffers 4-byte aligned are
+ * read and written with 32-bit accesses; any other even width or alignment takes a byte-wise kernel with the same results.
+ * Validation (before any CUDA call): NULL pointers, F == 0, H or W zero or odd, or F*H*W*3 bytes beyond SIZE_MAX ->
+ * GFPP_ERR_INVALID.  One launch, stream-ordered, no host sync, no allocation. */
+GFPP_API int gfpp_rgb_u8_to_i420(const uint8_t *rgb, uint32_t F, uint32_t H, uint32_t W, uint8_t *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
