@@ -162,8 +162,8 @@ class Superresolution(nn.Module):
 
     # ------------------------------------------------------------------ host half of the native path
     @torch.no_grad()
-    def folded_weights(self):
-        """The six layers as plain convolutions / GEMM matrices (fp32, on the parameters' device), given the constant
+    def folded_weights(self, dtype=torch.float32):
+        """The six layers as plain convolutions / GEMM matrices (fp32, or `dtype`, on the parameters' device), given the constant
         latent w = 1 (radnerf_sr.py:33-34); layouts as gfpp_sr_desc (include/gfpp.h) wants them:
 
           conv_in_w [27,128]    block0.conv0, k = (ky*3+kx)*3 + ci                      (cross-correlation taps, padding 1)
@@ -179,11 +179,11 @@ class Superresolution(nn.Module):
         # computed on the host from CPU copies of the (small) parameters -- a few hundred tiny tensor ops that would otherwise be a
         # few hundred kernel launches per (re)pack -- and moved to the parameters' device at the end
         dev = self.block0.conv0.weight.device
-        w = torch.ones(self.w_dim, dtype=torch.float32)
+        w = torch.ones(self.w_dim, dtype=dtype)
         b0, b1 = self.block0, self.block1
 
         def c(t):
-            return t.detach().float().cpu()
+            return t.detach().to(dtype).cpu()
 
         def mod_w(layer):     # _ModConv.modulated_weight on the CPU copies
             s_ = torch.addmv(c(layer.affine.bias), c(layer.affine.weight) * layer.affine.weight_gain, w)
@@ -219,7 +219,7 @@ class Superresolution(nn.Module):
         fw = {
             "conv_in_w": k00.permute(2, 3, 1, 0).reshape(27, 128).contiguous(),
             "conv0_w": k01.permute(0, 2, 3, 1).reshape(128, 9 * 128).contiguous(),
-            "up_w": K.permute(0, 1, 2, 4, 5, 3).reshape(4 * O, 9 * I).float().contiguous(),
+            "up_w": K.permute(0, 1, 2, 4, 5, 3).reshape(4 * O, 9 * I).to(dtype).contiguous(),
             "conv1_w": k11.permute(0, 2, 3, 1).reshape(64, 9 * 64).contiguous(),
             "bias": [c(b0.conv0.bias).contiguous(), c(b0.conv1.bias).contiguous(), c(b1.conv0.bias).contiguous(), c(b1.conv1.bias).contiguous()],
             "rgb_w": [r0w, r1w], "rgb_b": [r0b, r1b],
