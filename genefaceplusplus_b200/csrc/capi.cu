@@ -1,5 +1,6 @@
 // capi.cu -- extern "C" boundary of libgfpp.so (see include/gfpp.h for the contract).
 #include <math.h>
+#include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -13,68 +14,12 @@
 #include "grid_half.cuh"
 #include "head_kernel.cuh"
 #include "launch.cuh"
+#include "ops.cuh"
 #include "sr_kernel.cuh"
 #include "torso_grid_kernel.cuh"
 #include "torso_kernel.cuh"
 #include "torso_sr_kernel.cuh"
 #include "torso_train_kernel.cuh"
-
-namespace gfpp {
-// ops_kernels.cu
-cudaError_t launch_near_far(const float *, const float *, const float *, uint32_t, float, float *, float *, cudaStream_t);
-cudaError_t launch_march_rays(const MarchConst &, uint32_t, uint32_t, const int32_t *, const float *, const float *,
-                              const float *, const float *, float *, float *, float *, const float *, cudaStream_t);
-cudaError_t launch_composite_rays(uint32_t, uint32_t, float, int32_t *, float *, const float *, const float *,
-                                  const float *, float *, float *, float *, cudaStream_t);
-cudaError_t launch_grid_encode(const GridMeta &, const float *, const float *, float *, uint32_t, cudaStream_t);
-cudaError_t launch_sh_encode(const float *, float *, uint32_t, uint32_t, cudaStream_t);
-cudaError_t launch_freq_encode(const float *, uint32_t, uint32_t, uint32_t, float *, cudaStream_t);
-cudaError_t launch_occupancy_bounds(const uint8_t *, uint32_t, uint32_t, int *, cudaStream_t);
-cudaError_t launch_coarse_occupancy(const uint8_t *, uint32_t, uint32_t, uint32_t *, cudaStream_t);
-cudaError_t launch_pack_quads(const GridMeta &, const float *, float *, uint32_t, cudaStream_t);
-cudaError_t launch_pack_octs(const GridMeta &, const float *, void *, uint32_t, cudaStream_t);
-cudaError_t launch_pack_octs_i16(const GridMeta &, const float *, void *, uint32_t, uint32_t *, float *, cudaStream_t);
-// tc_pack.cu
-cudaError_t launch_pack_tc_tile(const float *, int, int, int, int, int, int, int, int, unsigned char *, unsigned char *, cudaStream_t);
-cudaError_t launch_pack_fold_tile(const float *, int, int, const float *, unsigned char *, int, cudaStream_t);
-cudaError_t launch_tc_selftest(const float *, int, const unsigned char *, const unsigned char *, int, int, int, int, float *, cudaStream_t);
-// train_kernels.cu
-size_t march_train_scratch_bytes(uint32_t N);
-cudaError_t launch_march_rays_train(const MarchConst &, const float *, const float *, const float *, const float *, const float *, uint32_t,
-                                    uint32_t, uint32_t, float *, float *, float *, int *, int *, int *, int *, cudaStream_t);
-cudaError_t launch_march_rays_train_backward(const float *, const float *, const int *, const float *, uint32_t, uint32_t, float *, float *,
-                                             cudaStream_t);
-cudaError_t launch_composite_train_forward(const float *, const float *, const float *, const float *, const int *, uint32_t, uint32_t, float,
-                                           float *, float *, float *, float *, cudaStream_t);
-cudaError_t launch_composite_train_backward(const float *, const float *, const float *, const float *, const float *, const float *,
-                                            const float *, const int *, const float *, const float *, const float *, uint32_t, uint32_t, float,
-                                            float *, float *, float *, cudaStream_t);
-cudaError_t launch_grid_encode_dydx(const GridMeta &, const float *, const float *, float *, float *, uint32_t, cudaStream_t);
-cudaError_t launch_grid_backward(const GridMeta &, const float *, const float *, float *, const float *, float *, uint32_t, int *, cudaStream_t);
-cudaError_t launch_grad_tv(const GridMeta &, const float *, const float *, float *, float, uint32_t, cudaStream_t);
-cudaError_t launch_packbits(const float *, uint32_t, float, uint8_t *, cudaStream_t);
-cudaError_t launch_morton3D(const int *, uint32_t, int *, cudaStream_t);
-cudaError_t launch_morton3D_invert(const int *, uint32_t, int *, cudaStream_t);
-cudaError_t launch_morton3D_dilation(const float *, uint32_t, uint32_t, float *, cudaStream_t);
-cudaError_t launch_sph_from_ray(const float *, const float *, float, uint32_t, float *, cudaStream_t);
-// grid_kernels.cu
-uint32_t dilate_ema_blocks(uint32_t C, uint32_t H);
-cudaError_t launch_grid_refresh_tail(const float *, uint32_t, uint32_t, float, float, float *, double *, float *, float *, uint8_t *, int *,
-                                     cudaStream_t);
-cudaError_t launch_mark_untrained(const float *, uint32_t, float, float, const float *, const float *, uint32_t, uint32_t, float *, cudaStream_t);
-uint32_t torso_dilate_ema_blocks(uint32_t H);
-cudaError_t launch_torso_grid_tail(const float *, uint32_t, float, float, float *, double *, float *, float *, int *, cudaStream_t);
-// torso_pass_kernels.cu
-uint32_t torso_mask_tiles(uint32_t N);
-cudaError_t launch_torso_mask(const float *, uint32_t, float, const float *, const float *, const float *, uint32_t, int32_t *, int32_t *,
-                              float *, float *, float *, int32_t *, int *, cudaStream_t);
-cudaError_t launch_torso_composite_fwd(const int32_t *, uint32_t, const float *, const float *, const float *, const float *, const float *,
-                                       uint32_t, float *, float *, float *, cudaStream_t);
-cudaError_t launch_torso_composite_bwd(const int32_t *, uint32_t, const float *, const float *, const float *, const float *, const float *,
-                                       uint32_t, const float *, const float *, const float *, float *, float *, cudaStream_t);
-// video_kernels.cu
-cudaError_t launch_rgb_u8_to_i420(const uint8_t *, uint32_t, uint32_t, uint32_t, uint8_t *, cudaStream_t);
-}  // namespace gfpp
 
 using namespace gfpp;
 
@@ -88,23 +33,51 @@ thread_local unsigned long long *g_phase = nullptr;
 thread_local cudaEvent_t g_ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
 thread_local int g_ev_dev = -1;                      // device the events were created on
 
-int fail(int code, const char *fmt, const char *detail = "") {
-    snprintf(g_err, sizeof(g_err), fmt, detail);
+__attribute__((format(printf, 2, 3))) int fail(int code, const char *fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(g_err, sizeof(g_err), fmt, ap);
+    va_end(ap);
     return code;
 }
 
 // CK: a kernel launch (counted in gfpp_last_launch_count); CKN: any other runtime call
-#define CK(expr)                                                                      \
-    do {                                                                              \
-        cudaError_t e__ = (expr);                                                     \
-        if (e__ != cudaSuccess) return fail(GFPP_ERR_CUDA, #expr ": %s", cudaGetErrorString(e__)); \
-        ++g_launches;                                                                 \
+#define CK(expr)                                                                              \
+    do {                                                                                      \
+        cudaError_t e__ = (expr);                                                             \
+        if (e__ != cudaSuccess) return fail(GFPP_ERR_CUDA, "%s: %s", #expr, cudaGetErrorString(e__)); \
+        ++g_launches;                                                                         \
     } while (0)
-#define CKN(expr)                                                                     \
-    do {                                                                              \
-        cudaError_t e__ = (expr);                                                     \
-        if (e__ != cudaSuccess) return fail(GFPP_ERR_CUDA, #expr ": %s", cudaGetErrorString(e__)); \
+#define CKN(expr)                                                                             \
+    do {                                                                                      \
+        cudaError_t e__ = (expr);                                                             \
+        if (e__ != cudaSuccess) return fail(GFPP_ERR_CUDA, "%s: %s", #expr, cudaGetErrorString(e__)); \
     } while (0)
+
+// Bump allocator of the packed-buffer and workspace layouts: each take() starts where the previous one ended and reserves
+// `bytes` rounded up to a multiple of `align`.
+struct Bump {
+    size_t end = 0;
+    size_t take(size_t bytes, size_t align = 256) {
+        const size_t r = end;
+        end += (bytes + align - 1) / align * align;
+        return r;
+    }
+};
+
+// the workspace checks of the entry points whose kernels need a 256-byte aligned workspace
+int check_workspace(const char *who, const void *workspace, size_t workspace_bytes, size_t need) {
+    if (workspace_bytes < need) return fail(GFPP_ERR_WORKSPACE, "%s: workspace too small", who);
+    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
+    return GFPP_OK;
+}
+
+// The host struct behind an opaque handle (ModelHost, SrHost, TorsoSrHost), if the handle's own pack call filled it.
+template <class Host> int unpack(const char *who, const typename Host::Handle *model, Host &m) {
+    memcpy(&m, model, sizeof(m));
+    if (m.magic != Host::kMagic) return fail(GFPP_ERR_INVALID, "%s: model handle not initialised by %s", who, Host::kPacker);
+    return GFPP_OK;
+}
 
 // Level constants exactly as the reference kernel derives them (gridencoder.cu:137-139, :66-84), computed once on
 // the host with the same libm calls as oracle/native_ops.c.
@@ -144,10 +117,22 @@ int fill_grid_meta(GridMeta &gm, const int32_t *offsets, uint32_t D, uint32_t L,
     return 0;
 }
 
+// The level constants of the grid-encoder ops; the reference throws std::runtime_error for unsupported C / D (gridencoder.cu:380, 397).
+int grid_op_meta(GridMeta &gm, const int32_t *offsets, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, uint32_t gridtype,
+                 int align_corners, uint32_t interp) {
+    if (C != 2) return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: this build supports C == 2 only");
+    if (fill_grid_meta(gm, offsets, D, L, S, H, gridtype, align_corners, interp) != 0)
+        return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: D must be 2 or 3 and L <= 16");
+    return GFPP_OK;
+}
+
 // ---------------------------------------------------------------- packed model
 constexpr int kChunkK[HEAD_NCHUNK] = {48, 48, 64, 64, 64, 64, 64, 64, 64, 72, 72};
 
 struct ModelHost {
+    using Handle = gfpp_model;
+    static constexpr uint32_t kMagic = 0x67667070u;  // "gfpp"
+    static constexpr const char *kPacker = "gfpp_model_pack";
     uint32_t magic;
     int has_torso;
     GridMeta pos_gm, amb_gm, tor_gm;
@@ -181,7 +166,6 @@ struct ModelHost {
     const unsigned char *tor_tf32;  // tf32 hi / lo images of the wide torso layers (k_epilogue)
 };
 static_assert(sizeof(ModelHost) <= sizeof(gfpp_model), "gfpp_model opaque storage too small");
-constexpr uint32_t kMagic = 0x67667070u;  // "gfpp"
 
 struct PackedLayout {
     size_t wide, narrow, wd0, wd1, wd2, wc0, wc1, wc2, tor_tf32, occ, coarse, tc_hi, tc_lo, v2_stream, v2_res, v2_step, pos_quads, amb_quads, total;
@@ -199,31 +183,30 @@ inline size_t coarse_words_for(uint32_t cascade, uint32_t grid_size) {
 
 PackedLayout packed_layout(uint32_t cascade = 8, uint32_t grid_size = 128, size_t pos_entries = 0, size_t amb_entries = 0) {
     PackedLayout L;
-    size_t o = 0;
-    auto take = [&](size_t floats) { size_t r = o; o += (floats * 4 + 255) / 256 * 256; return r; };
+    Bump b;
     size_t wide = 0;
     for (int c = 0; c < HEAD_NCHUNK; ++c) wide += (size_t)kChunkK[c] * 128;
-    L.wide = take(wide);
-    L.narrow = take(8 * 128);
-    L.wd0 = take(44 * 64);
-    L.wd1 = take(64 * 64);
-    L.wd2 = take(2 * 64);
-    L.wc0 = take(76 * 32);
-    L.wc1 = take(32 * 32);
-    L.wc2 = take(4 * 32);
-    L.tor_tf32 = take(TORSO_TF32_BYTES / 4);
-    L.occ = take(8);
-    L.coarse = take(coarse_words_for(cascade, grid_size));
+    L.wide = b.take(wide * 4);
+    L.narrow = b.take(8 * 128 * 4);
+    L.wd0 = b.take(44 * 64 * 4);
+    L.wd1 = b.take(64 * 64 * 4);
+    L.wd2 = b.take(2 * 64 * 4);
+    L.wc0 = b.take(76 * 32 * 4);
+    L.wc1 = b.take(32 * 32 * 4);
+    L.wc2 = b.take(4 * 32 * 4);
+    L.tor_tf32 = b.take(TORSO_TF32_BYTES);
+    L.occ = b.take(8 * 4);
+    L.coarse = b.take(coarse_words_for(cascade, grid_size) * 4);
     size_t tcb = 0;
     for (int c = 0; c < HEAD_TC_NCHUNK; ++c) tcb += (size_t)tc_chunk_bytes(c);
-    L.tc_hi = take(tcb / 4);
-    L.tc_lo = take(tcb / 4);
-    L.v2_stream = take((size_t)V2_NTILE_ROBUST * V2_TILE_BYTES / 4);
-    L.v2_res = take(V2_RES_BYTES / 4);
-    L.v2_step = take(64);          // 16 steps + 16 words of scratch for the per-level maxima
-    L.pos_quads = take(pos_entries * 8);   // 32 bytes per entry
-    L.amb_quads = take(amb_entries * 8);
-    L.total = o;
+    L.tc_hi = b.take(tcb);
+    L.tc_lo = b.take(tcb);
+    L.v2_stream = b.take((size_t)V2_NTILE_ROBUST * V2_TILE_BYTES);
+    L.v2_res = b.take(V2_RES_BYTES);
+    L.v2_step = b.take(64 * 4);          // 16 steps + 16 words of scratch for the per-level maxima
+    L.pos_quads = b.take(pos_entries * 32);
+    L.amb_quads = b.take(amb_entries * 32);
+    L.total = b.end;
     return L;
 }
 
@@ -234,27 +217,76 @@ struct WorkLayout {
 
 WorkLayout work_layout(uint32_t F, uint32_t N, uint32_t max_steps) {
     WorkLayout W;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
+    Bump b;
     const size_t FN = (size_t)F * N;
-    W.image = take(FN * 3 * 4);
-    W.rays_t = take(FN * 4);
-    W.wsum = take(FN * 4);
-    W.depth = take(FN * 4);
-    W.survivors = take(FN * 4);
-    W.hits = take(FN * 64);   // HitRecord (head_common.cuh)
-    W.zero_begin = o;
-    W.hist = take((size_t)F * (max_steps + 2) * 4);
-    W.counters = take(16 * 4);
-    W.B_total = take((size_t)F * 4);
-    W.valid = take((size_t)F * 4);
-    W.pcount = take((size_t)F * 4);
-    W.zero_end = o;
-    W.bias_def = take((size_t)F * 64 * 4);
-    W.bias_can = take((size_t)F * 32 * 4);
-    W.bias_amb = take((size_t)F * 64 * 2 * 2);   // fp16 hi + lo images of the conditioning vectors (v2 head kernel)
-    W.total = o;
+    W.image = b.take(FN * 3 * 4);
+    W.rays_t = b.take(FN * 4);
+    W.wsum = b.take(FN * 4);
+    W.depth = b.take(FN * 4);
+    W.survivors = b.take(FN * 4);
+    W.hits = b.take(FN * 64);   // HitRecord (head_common.cuh)
+    W.zero_begin = b.end;
+    W.hist = b.take((size_t)F * (max_steps + 2) * 4);
+    W.counters = b.take(16 * 4);
+    W.B_total = b.take((size_t)F * 4);
+    W.valid = b.take((size_t)F * 4);
+    W.pcount = b.take((size_t)F * 4);
+    W.zero_end = b.end;
+    W.bias_def = b.take((size_t)F * 64 * 4);
+    W.bias_can = b.take((size_t)F * 32 * 4);
+    W.bias_amb = b.take((size_t)F * 64 * 2 * 2);   // fp16 hi + lo images of the conditioning vectors (v2 head kernel)
+    W.total = b.end;
     return W;
+}
+
+// The occupied-box shortcut (HeadArgs::use_occ_box) assumes that no sample position is clamped to the cube: it holds for an
+// aabb only if that lies inside the cube of the model's single cascade.
+int occ_box_ok(const float aabb[6], float bound, uint32_t cascade) {
+    return (cascade == 1 && aabb[0] >= -bound && aabb[1] >= -bound && aabb[2] >= -bound && aabb[3] <= bound && aabb[4] <= bound &&
+            aabb[5] <= bound) ? 1 : 0;
+}
+
+// The head field of a packed model, the model half of HeadArgs that every head kernel and k_density read: the grid tables
+// (quads / octs where the mode packed them) and the fp32 weight chunks; the rest zero.
+HeadArgs head_field_args(const ModelHost &m) {
+    HeadArgs a;
+    memset(&a, 0, sizeof(a));
+    a.pos_gm = m.pos_gm; a.amb_gm = m.amb_gm;
+    a.pos_tab = m.pos_tab; a.amb_tab = m.amb_tab;
+    a.pos_quads = m.pos_quads; a.amb_quads = m.amb_quads;
+    a.pos_octs = m.pos_octs; a.amb_octs = m.amb_octs;
+    a.wide = m.wide; a.narrow = m.narrow;
+    for (int c = 0; c < HEAD_NCHUNK; ++c) { a.chunk_off[c] = m.chunk_off[c]; a.chunk_k[c] = kChunkK[c]; }
+    return a;
+}
+
+// The head kernel a packed model renders with, in gfpp_render_frames and gfpp_frozen_head alike (the frozen head's parity with
+// pass 1 rests on it): fp32 -> k_head; fp16 and robust -> the row-owner kernel k_head_v2 (head_v2_kernel.cu), except that
+// GFPP_HEAD_V1 keeps fp16 on the first-generation k_head_tc for A/B runs; bf16x3 / bf16 -> k_head_tc.
+enum HeadKernel { HEAD_FP32, HEAD_V2, HEAD_TC };
+
+int choose_head_kernel(const char *who, const ModelHost &m, HeadKernel &k) {
+    const bool use_v2 = m.v2_ok && (m.mlp_precision == 4 || (m.mlp_precision == 1 && getenv("GFPP_HEAD_V1") == nullptr));
+    k = m.mlp_precision == 0 ? HEAD_FP32 : use_v2 ? HEAD_V2 : HEAD_TC;
+    if (m.mlp_precision == 4 && !use_v2) return fail(GFPP_ERR_UNSUPPORTED, "%s: robust mode unavailable for this model", who);
+    return GFPP_OK;
+}
+
+// k_head_v2's weight images and the call's conditioning images: fp16 hi then lo, n_frames x 128 bytes each, at cond_images
+HeadV2Args head_v2_args(const ModelHost &m, const char *cond_images, uint32_t n_frames) {
+    HeadV2Args v2;
+    v2.w_stream = m.v2_stream; v2.w_res = m.v2_res; v2.pos_step = m.v2_pos_step;
+    v2.cond_hi = (const unsigned char *)cond_images;
+    v2.cond_lo = v2.cond_hi + (size_t)n_frames * 128;
+    return v2;
+}
+
+// one head pass (a.pass) on the chosen kernel; train: pass 1 with composite_rays_train's termination (gfpp_frozen_head)
+int launch_head_pass(HeadKernel k, const ModelHost &m, const HeadArgs &a, const HeadV2Args &v2, cudaStream_t st, bool train = false) {
+    if (k == HEAD_FP32) CK(launch_head(a, -1, st, train));
+    else if (k == HEAD_V2) CK(launch_head_v2(a, v2, m.mlp_precision, st, train));
+    else CK(launch_head_tc(a, m.tc, m.mlp_precision, -1, st, train));
+    return GFPP_OK;
 }
 
 __global__ void k_init_bounds(int *b) {
@@ -282,11 +314,11 @@ int gfpp_last_launch_count(void) { return g_launches; }
 
 int gfpp_profile_enable(int on) {
     int dev = -1;
-    if (on && cudaGetDevice(&dev) != cudaSuccess) return fail(GFPP_ERR_CUDA, "no CUDA device%s");
+    if (on && cudaGetDevice(&dev) != cudaSuccess) return fail(GFPP_ERR_CUDA, "no CUDA device");
     if (on && (!g_ev[0] || g_ev_dev != dev)) {   // events belong to a device: (re)create them for the current one
         for (int i = 0; i < 5; ++i) {
             if (g_ev[i]) cudaEventDestroy(g_ev[i]);
-            if (cudaEventCreate(&g_ev[i]) != cudaSuccess) return fail(GFPP_ERR_CUDA, "cudaEventCreate failed%s");
+            if (cudaEventCreate(&g_ev[i]) != cudaSuccess) return fail(GFPP_ERR_CUDA, "cudaEventCreate failed");
         }
         g_ev_dev = dev;
     }
@@ -300,7 +332,7 @@ int gfpp_profile_phases(void *dev_u64x32) {
 }
 
 int gfpp_profile_read(float ms[4]) {
-    if (!g_profile || !g_ev[0] || !ms) return fail(GFPP_ERR_INVALID, "profile_read: profiling is not enabled%s");
+    if (!g_profile || !g_ev[0] || !ms) return fail(GFPP_ERR_INVALID, "profile_read: profiling is not enabled");
     CKN(cudaEventSynchronize(g_ev[3]));
     for (int i = 0; i < 3; ++i) CKN(cudaEventElapsedTime(&ms[i], g_ev[i], g_ev[i + 1]));
     CKN(cudaEventElapsedTime(&ms[3], g_ev[4], g_ev[0]));   // everything before the head kernel: memset, torso biases, ray setup
@@ -311,18 +343,16 @@ int gfpp_check_device(void) {
     int dev = 0;
     cudaDeviceProp p;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&p, dev) != cudaSuccess)
-        return fail(GFPP_ERR_CUDA, "no CUDA device%s");
-    if (p.major != 9 || p.minor != 0) {
-        snprintf(g_err, sizeof(g_err), "libgfpp is built for sm_90a only; device is sm_%d%d", p.major, p.minor);
-        return GFPP_ERR_UNSUPPORTED;
-    }
+        return fail(GFPP_ERR_CUDA, "no CUDA device");
+    if (p.major != 9 || p.minor != 0)
+        return fail(GFPP_ERR_UNSUPPORTED, "libgfpp is built for sm_90a only; device is sm_%d%d", p.major, p.minor);
     return GFPP_OK;
 }
 
 // ------------------------------------------------------------------ (A) per-op mirror
 int gfpp_near_far_from_aabb(const float *rays_o, const float *rays_d, const float *aabb, uint32_t N, float min_near,
                             float *nears, float *fars, void *stream) {
-    if (!rays_o || !rays_d || !aabb || !nears || !fars) return fail(GFPP_ERR_INVALID, "near_far_from_aabb: null pointer%s");
+    if (!rays_o || !rays_d || !aabb || !nears || !fars) return fail(GFPP_ERR_INVALID, "near_far_from_aabb: null pointer");
     g_launches = 0;
     CK(launch_near_far(rays_o, rays_d, aabb, N, min_near, nears, fars, (cudaStream_t)stream));
     return GFPP_OK;
@@ -334,8 +364,8 @@ int gfpp_march_rays(uint32_t n_alive, uint32_t n_step, const int32_t *rays_alive
                     float *deltas, const float *noises, void *stream) {
     (void)nears;
     if (!rays_alive || !rays_t || !rays_o || !rays_d || !grid || !fars || !xyzs || !dirs || !deltas || !noises)
-        return fail(GFPP_ERR_INVALID, "march_rays: null pointer%s");
-    if (C < 1 || C > 8 || H < 1 || H > 1024 || max_steps < 1) return fail(GFPP_ERR_INVALID, "march_rays: bad C/H/max_steps%s");
+        return fail(GFPP_ERR_INVALID, "march_rays: null pointer");
+    if (C < 1 || C > 8 || H < 1 || H > 1024 || max_steps < 1) return fail(GFPP_ERR_INVALID, "march_rays: bad C/H/max_steps");
     MarchConst mc;
     march_const_init(mc, bound, dt_gamma, max_steps, C, H, grid);
     g_launches = 0;
@@ -348,7 +378,7 @@ int gfpp_composite_rays(uint32_t n_alive, uint32_t n_step, float T_thresh, int32
                         const float *sigmas, const float *rgbs, const float *deltas, float *weights_sum, float *depth,
                         float *image, void *stream) {
     if (!rays_alive || !rays_t || !sigmas || !rgbs || !deltas || !weights_sum || !depth || !image)
-        return fail(GFPP_ERR_INVALID, "composite_rays: null pointer%s");
+        return fail(GFPP_ERR_INVALID, "composite_rays: null pointer");
     g_launches = 0;
     CK(launch_composite_rays(n_alive, n_step, T_thresh, rays_alive, rays_t, sigmas, rgbs, deltas, weights_sum, depth,
                              image, (cudaStream_t)stream));
@@ -358,20 +388,17 @@ int gfpp_composite_rays(uint32_t n_alive, uint32_t n_step, float T_thresh, int32
 int gfpp_grid_encode_forward(const float *inputs, const float *embeddings, const int32_t *offsets_host, float *outputs,
                              uint32_t B, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, uint32_t gridtype,
                              int align_corners, uint32_t interp, void *stream) {
-    if (!inputs || !embeddings || !offsets_host || !outputs) return fail(GFPP_ERR_INVALID, "grid_encode_forward: null pointer%s");
-    // the reference throws std::runtime_error for unsupported C / D (gridencoder.cu:380, 397)
-    if (C != 2) return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: this build supports C == 2 only%s");
+    if (!inputs || !embeddings || !offsets_host || !outputs) return fail(GFPP_ERR_INVALID, "grid_encode_forward: null pointer");
     GridMeta gm;
-    if (fill_grid_meta(gm, offsets_host, D, L, S, H, gridtype, align_corners, interp) != 0)
-        return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: D must be 2 or 3 and L <= 16%s");
+    if (const int rc = grid_op_meta(gm, offsets_host, D, C, L, S, H, gridtype, align_corners, interp); rc != GFPP_OK) return rc;
     g_launches = 0;
     CK(launch_grid_encode(gm, inputs, embeddings, outputs, B, (cudaStream_t)stream));
     return GFPP_OK;
 }
 
 int gfpp_sh_encode_forward(const float *inputs, float *outputs, uint32_t B, uint32_t D, uint32_t degree, void *stream) {
-    if (!inputs || !outputs) return fail(GFPP_ERR_INVALID, "sh_encode_forward: null pointer%s");
-    if (D != 3 || degree < 1 || degree > 4) return fail(GFPP_ERR_UNSUPPORTED, "SH encoder: D must be 3 and degree in 1..4%s");
+    if (!inputs || !outputs) return fail(GFPP_ERR_INVALID, "sh_encode_forward: null pointer");
+    if (D != 3 || degree < 1 || degree > 4) return fail(GFPP_ERR_UNSUPPORTED, "SH encoder: D must be 3 and degree in 1..4");
     g_launches = 0;
     CK(launch_sh_encode(inputs, outputs, B, degree, (cudaStream_t)stream));
     return GFPP_OK;
@@ -379,8 +406,8 @@ int gfpp_sh_encode_forward(const float *inputs, float *outputs, uint32_t B, uint
 
 int gfpp_freq_encode_forward(const float *inputs, uint32_t B, uint32_t D, uint32_t deg, uint32_t C, float *outputs,
                              void *stream) {
-    if (!inputs || !outputs) return fail(GFPP_ERR_INVALID, "freq_encode_forward: null pointer%s");
-    if (C != D + 2 * D * deg) return fail(GFPP_ERR_INVALID, "freq_encode_forward: C != D + 2*D*deg%s");
+    if (!inputs || !outputs) return fail(GFPP_ERR_INVALID, "freq_encode_forward: null pointer");
+    if (C != D + 2 * D * deg) return fail(GFPP_ERR_INVALID, "freq_encode_forward: C != D + 2*D*deg");
     g_launches = 0;
     CK(launch_freq_encode(inputs, B, D, C, outputs, (cudaStream_t)stream));
     return GFPP_OK;
@@ -388,10 +415,10 @@ int gfpp_freq_encode_forward(const float *inputs, uint32_t B, uint32_t D, uint32
 
 int gfpp_tc_selftest(const float *A, const float *W, uint32_t N, uint32_t K, int k16_tail, int precision, void *scratch,
                      float *out, void *stream) {
-    if (!A || !W || !scratch || !out) return fail(GFPP_ERR_INVALID, "tc_selftest: null pointer%s");
+    if (!A || !W || !scratch || !out) return fail(GFPP_ERR_INVALID, "tc_selftest: null pointer");
     const int k64 = (int)K - (k16_tail ? 16 : 0);
     if ((N != 16 && N != 128 && N != 144) || k64 <= 0 || k64 % 16 || K > 144 || precision < 1 || precision > 3)
-        return fail(GFPP_ERR_INVALID, "tc_selftest: unsupported shape%s");
+        return fail(GFPP_ERR_INVALID, "tc_selftest: unsupported shape");
     const int nt64 = (k64 + 63) / 64;
     cudaStream_t st = (cudaStream_t)stream;
     unsigned char *hi = (unsigned char *)scratch, *lo = hi + 3 * 18432;
@@ -418,37 +445,35 @@ size_t gfpp_model_packed_bytes(const gfpp_model_desc *desc) {
 }
 
 int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes, gfpp_model *model, void *stream) {
-    if (!d || !packed || !model) return fail(GFPP_ERR_INVALID, "model_pack: null pointer%s");
+    if (!d || !packed || !model) return fail(GFPP_ERR_INVALID, "model_pack: null pointer");
     if (d->cascade < 1 || d->cascade > 8 || d->grid_size < 8 || d->grid_size > 1024 || d->grid_size % 4)
-        return fail(GFPP_ERR_UNSUPPORTED, "model_pack: cascade/grid_size out of range%s");
+        return fail(GFPP_ERR_UNSUPPORTED, "model_pack: cascade/grid_size out of range");
     if (!d->position_grid.offsets_host || !d->ambient_grid.offsets_host || d->position_grid.num_levels > 16 || d->ambient_grid.num_levels > 16)
-        return fail(GFPP_ERR_INVALID, "model_pack: grid offsets missing%s");
+        return fail(GFPP_ERR_INVALID, "model_pack: grid offsets missing");
     const size_t pos_entries = (size_t)d->position_grid.offsets_host[d->position_grid.num_levels];
     const size_t amb_entries = (size_t)d->ambient_grid.offsets_host[d->ambient_grid.num_levels];
     const PackedLayout L = packed_layout(d->cascade, d->grid_size, pos_entries, amb_entries);
-    if (packed_bytes < L.total) return fail(GFPP_ERR_WORKSPACE, "model_pack: packed buffer too small%s");
-    if (d->cond_dim != 64 || d->ind_dim > 16) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: cond_dim must be 64, ind_dim <= 16%s");
-    if (d->cascade < 1 || d->cascade > 8 || d->grid_size < 8 || d->grid_size > 1024)
-        return fail(GFPP_ERR_UNSUPPORTED, "model_pack: cascade/grid_size out of range%s");
+    if (packed_bytes < L.total) return fail(GFPP_ERR_WORKSPACE, "model_pack: packed buffer too small");
+    if (d->cond_dim != 64 || d->ind_dim > 16) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: cond_dim must be 64, ind_dim <= 16");
     for (int i = 0; i < 3; ++i)
-        if (!d->ambient_w[i] || !d->sigma_w[i]) return fail(GFPP_ERR_INVALID, "model_pack: null weight%s");
-    if (!d->color_w[0] || !d->color_w[1] || !d->density_bitfield) return fail(GFPP_ERR_INVALID, "model_pack: null weight%s");
+        if (!d->ambient_w[i] || !d->sigma_w[i]) return fail(GFPP_ERR_INVALID, "model_pack: null weight");
+    if (!d->color_w[0] || !d->color_w[1] || !d->density_bitfield) return fail(GFPP_ERR_INVALID, "model_pack: null weight");
     cudaStream_t st = (cudaStream_t)stream;
     ModelHost m;
     memset(&m, 0, sizeof(m));
-    m.magic = kMagic;
+    m.magic = ModelHost::kMagic;
     const gfpp_grid_desc *gd[3] = {&d->position_grid, &d->ambient_grid, &d->torso_grid};
     GridMeta *gm[3] = {&m.pos_gm, &m.amb_gm, &m.tor_gm};
     for (int i = 0; i < (d->has_torso ? 3 : 2); ++i) {
-        if (!gd[i]->embeddings) return fail(GFPP_ERR_INVALID, "model_pack: null grid table%s");
+        if (!gd[i]->embeddings) return fail(GFPP_ERR_INVALID, "model_pack: null grid table");
         if (gd[i]->num_levels != 16)
-            return fail(GFPP_ERR_UNSUPPORTED, "model_pack: grids must have 16 levels x 2 features%s");
+            return fail(GFPP_ERR_UNSUPPORTED, "model_pack: grids must have 16 levels x 2 features");
         if (fill_grid_meta(*gm[i], gd[i]->offsets_host, gd[i]->input_dim, gd[i]->num_levels, gd[i]->log2_per_level_scale,
                            gd[i]->base_resolution, gd[i]->gridtype, gd[i]->align_corners, gd[i]->interp) != 0)
-            return fail(GFPP_ERR_UNSUPPORTED, "model_pack: unsupported grid layout%s");
+            return fail(GFPP_ERR_UNSUPPORTED, "model_pack: unsupported grid layout");
     }
-    if (m.pos_gm.dim != 3) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: position grid must be 3-D%s");
-    if (d->has_torso && m.tor_gm.dim != 2) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: torso grid must be 2-D%s");
+    if (m.pos_gm.dim != 3) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: position grid must be 3-D");
+    if (d->has_torso && m.tor_gm.dim != 2) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: torso grid must be 2-D");
     m.pos_tab = (const float2 *)d->position_grid.embeddings;
     m.amb_tab = (const float2 *)d->ambient_grid.embeddings;
     m.tor_tab = d->has_torso ? (const float2 *)d->torso_grid.embeddings : nullptr;
@@ -459,9 +484,7 @@ int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes,
     m.density_scale = d->density_scale;
     m.cascade = d->cascade;
     m.grid_size = d->grid_size;
-    const float cube = d->bound;
-    m.use_occ_box = (d->cascade == 1 && d->aabb[0] >= -cube && d->aabb[1] >= -cube && d->aabb[2] >= -cube &&
-                     d->aabb[3] <= cube && d->aabb[4] <= cube && d->aabb[5] <= cube) ? 1 : 0;
+    m.use_occ_box = occ_box_ok(d->aabb, d->bound, d->cascade);
 
     char *base = (char *)packed;
     float *wide = (float *)(base + L.wide), *narrow = (float *)(base + L.narrow);
@@ -507,7 +530,7 @@ int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes,
     // packing below because that one clears everything from tc_hi to the END of the packed buffer
     const bool want_quads = getenv("GFPP_NO_QUADS") == nullptr;
     m.mlp_precision = (int)d->mlp_precision;
-    if (d->mlp_precision > 4) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: mlp_precision must be 0..4%s");
+    if (d->mlp_precision > 4) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: mlp_precision must be 0..4");
     const bool robust = d->mlp_precision == 4;
     if (d->mlp_precision != 0) CKN(cudaMemsetAsync(base + L.tc_hi, 0, L.pos_quads - L.tc_hi, st));
     m.amb0_src = d->ambient_w[0];
@@ -588,13 +611,13 @@ int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes,
 
     m.v2_ok = (m.v2_stream && m.pos_octs && m.amb_octs && m.pos_gm.num_levels == 16 && m.amb_gm.num_levels == 16 && amb_dim == 3) ? 1 : 0;
     if (robust && !m.v2_ok)
-        return fail(GFPP_ERR_UNSUPPORTED, "model_pack: the robust mode needs 3-D tiled position and ambient grids (sector-packed tables)%s");
+        return fail(GFPP_ERR_UNSUPPORTED, "model_pack: the robust mode needs 3-D tiled position and ambient grids (sector-packed tables)");
     m.has_torso = d->has_torso;
     if (d->has_torso) {
         for (int i = 0; i < 3; ++i)
-            if (!d->torso_deform_w[i] || !d->torso_canon_w[i]) return fail(GFPP_ERR_INVALID, "model_pack: null torso weight%s");
-        if (!d->density_grid_torso) return fail(GFPP_ERR_INVALID, "model_pack: null density_grid_torso%s");
-        if (d->torso_code_dim > 10) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: torso_code_dim <= 10%s");
+            if (!d->torso_deform_w[i] || !d->torso_canon_w[i]) return fail(GFPP_ERR_INVALID, "model_pack: null torso weight");
+        if (!d->density_grid_torso) return fail(GFPP_ERR_INVALID, "model_pack: null density_grid_torso");
+        if (d->torso_code_dim > 10) return fail(GFPP_ERR_UNSUPPORTED, "model_pack: torso_code_dim <= 10");
         const int din = 42 + 54 + (int)d->torso_code_dim;
         float *wd0 = (float *)(base + L.wd0), *wd1 = (float *)(base + L.wd1), *wd2 = (float *)(base + L.wd2);
         float *wc0 = (float *)(base + L.wc0), *wc1 = (float *)(base + L.wc1), *wc2 = (float *)(base + L.wc2);
@@ -624,7 +647,7 @@ int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes,
 int gfpp_debug_generate_rays(const float *poses_c2w, uint32_t n_frames, float fx, float fy, float cx, float cy, uint32_t img_h,
                              uint32_t img_w, float *rays_o, float *rays_d, void *stream) {
     if (!poses_c2w || !rays_o || !rays_d || n_frames == 0 || img_h == 0 || img_w == 0)
-        return fail(GFPP_ERR_INVALID, "debug_generate_rays: null pointer or empty image%s");
+        return fail(GFPP_ERR_INVALID, "debug_generate_rays: null pointer or empty image");
     HeadArgs a;
     memset(&a, 0, sizeof(a));
     a.n_frames = (int)n_frames; a.n_rays = (int)(img_h * img_w);
@@ -640,35 +663,27 @@ size_t gfpp_render_workspace_bytes(uint32_t n_frames, uint32_t n_rays, uint32_t 
 
 int gfpp_render_frames(const gfpp_model *model, const gfpp_frames *fr, const gfpp_outputs *out, void *workspace,
                        size_t workspace_bytes, void *stream) {
-    if (!model || !fr || !out || !workspace) return fail(GFPP_ERR_INVALID, "render_frames: null pointer%s");
+    if (!model || !fr || !out || !workspace) return fail(GFPP_ERR_INVALID, "render_frames: null pointer");
     ModelHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "render_frames: model handle not initialised by gfpp_model_pack%s");
-    if ((!out->rgb_map && !out->rgb_u8 && !out->rgba_u8) || !fr->cond_feat) return fail(GFPP_ERR_INVALID, "render_frames: rgb_map (or rgb_u8) and cond_feat are required%s");
-    if ((uintptr_t)out->rgba_u8 & 3) return fail(GFPP_ERR_INVALID, "render_frames: rgba_u8 must be 4-byte aligned%s");
-    if (fr->n_frames == 0 || fr->n_rays == 0) return fail(GFPP_ERR_INVALID, "render_frames: empty clip%s");
-    if ((uint64_t)fr->n_frames * fr->n_rays >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "render_frames: F*N must be < 2^31%s");
-    if (fr->max_steps < 1 || fr->max_steps > 4096) return fail(GFPP_ERR_UNSUPPORTED, "render_frames: max_steps must be in 1..4096%s");
-    if ((fr->rays_o == nullptr) != (fr->rays_d == nullptr)) return fail(GFPP_ERR_INVALID, "render_frames: rays_o and rays_d go together%s");
+    if (const int rc = unpack("render_frames", model, m); rc != GFPP_OK) return rc;
+    if ((!out->rgb_map && !out->rgb_u8 && !out->rgba_u8) || !fr->cond_feat) return fail(GFPP_ERR_INVALID, "render_frames: rgb_map (or rgb_u8) and cond_feat are required");
+    if ((uintptr_t)out->rgba_u8 & 3) return fail(GFPP_ERR_INVALID, "render_frames: rgba_u8 must be 4-byte aligned");
+    if (fr->n_frames == 0 || fr->n_rays == 0) return fail(GFPP_ERR_INVALID, "render_frames: empty clip");
+    if ((uint64_t)fr->n_frames * fr->n_rays >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "render_frames: F*N must be < 2^31");
+    if (fr->max_steps < 1 || fr->max_steps > 4096) return fail(GFPP_ERR_UNSUPPORTED, "render_frames: max_steps must be in 1..4096");
+    if ((fr->rays_o == nullptr) != (fr->rays_d == nullptr)) return fail(GFPP_ERR_INVALID, "render_frames: rays_o and rays_d go together");
     if (!fr->rays_o && (!fr->poses_c2w || fr->img_w == 0 || fr->img_h * fr->img_w != fr->n_rays))
-        return fail(GFPP_ERR_INVALID, "render_frames: need rays or (poses_c2w, img_h*img_w == n_rays)%s");
-    if (m.has_torso && (!fr->torso_pose6 || !fr->bg_coords)) return fail(GFPP_ERR_INVALID, "render_frames: torso model needs torso_pose6 and bg_coords%s");
+        return fail(GFPP_ERR_INVALID, "render_frames: need rays or (poses_c2w, img_h*img_w == n_rays)");
+    if (m.has_torso && (!fr->torso_pose6 || !fr->bg_coords)) return fail(GFPP_ERR_INVALID, "render_frames: torso model needs torso_pose6 and bg_coords");
     const WorkLayout W = work_layout(fr->n_frames, fr->n_rays, fr->max_steps);
-    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "render_frames: workspace too small%s");
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "render_frames: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     g_launches = 0;
     if (g_profile) CKN(cudaEventRecord(g_ev[4], st));
     CKN(cudaMemsetAsync(ws + W.zero_begin, 0, W.zero_end - W.zero_begin, st));
 
-    HeadArgs a;
-    memset(&a, 0, sizeof(a));
-    a.pos_gm = m.pos_gm; a.amb_gm = m.amb_gm;
-    a.pos_tab = m.pos_tab; a.amb_tab = m.amb_tab;
-    a.pos_quads = m.pos_quads; a.amb_quads = m.amb_quads;
-    a.pos_octs = m.pos_octs; a.amb_octs = m.amb_octs;
-    a.wide = m.wide; a.narrow = m.narrow;
-    for (int c = 0; c < HEAD_NCHUNK; ++c) { a.chunk_off[c] = m.chunk_off[c]; a.chunk_k[c] = kChunkK[c]; }
+    HeadArgs a = head_field_args(m);
     march_const_init(a.mc, m.bound, fr->dt_gamma, fr->max_steps, m.cascade, m.grid_size, m.bitfield);
     a.occ_bounds = m.occ_bounds;
     a.coarse_bits = m.coarse_bits;
@@ -724,25 +739,17 @@ int gfpp_render_frames(const gfpp_model *model, const gfpp_frames *fr, const gfp
     a.pass = 1;
     a.cursor = counters + 0;
     CK(launch_ray_setup(a, st));
-    // fp16 / robust: the row-owner kernel (head_v2_kernel.cu); GFPP_HEAD_V1 keeps the first-generation fp16 kernel for A/B runs
-    const bool use_v2 = m.v2_ok && (m.mlp_precision == 4 || (m.mlp_precision == 1 && getenv("GFPP_HEAD_V1") == nullptr));
-    if (m.mlp_precision == 4 && !use_v2) return fail(GFPP_ERR_UNSUPPORTED, "render_frames: robust mode unavailable for this model%s");
-    HeadV2Args v2;
-    v2.w_stream = m.v2_stream; v2.w_res = m.v2_res; v2.pos_step = m.v2_pos_step;
-    v2.cond_hi = (const unsigned char *)(ws + W.bias_amb);
-    v2.cond_lo = v2.cond_hi + (size_t)fr->n_frames * 128;
-    if (use_v2) CK(launch_cond_images(fr->cond_feat, a.n_frames, ws + W.bias_amb, ws + W.bias_amb + (size_t)fr->n_frames * 128, st));
+    HeadKernel hk;
+    if (const int rc = choose_head_kernel("render_frames", m, hk); rc != GFPP_OK) return rc;
+    const HeadV2Args v2 = head_v2_args(m, ws + W.bias_amb, fr->n_frames);
+    if (hk == HEAD_V2) CK(launch_cond_images(fr->cond_feat, a.n_frames, ws + W.bias_amb, ws + W.bias_amb + (size_t)fr->n_frames * 128, st));
     if (g_profile) CKN(cudaEventRecord(g_ev[0], st));
-    if (m.mlp_precision == 0) CK(launch_head(a, -1, st));
-    else if (use_v2) CK(launch_head_v2(a, v2, m.mlp_precision, st));
-    else CK(launch_head_tc(a, m.tc, m.mlp_precision, -1, st));
+    if (const int rc = launch_head_pass(hk, m, a, v2, st); rc != GFPP_OK) return rc;
     if (g_profile) CKN(cudaEventRecord(g_ev[1], st));
     CK(launch_schedule(a.hist, a.n_frames, a.n_rays, a.max_steps, a.B_total, st));
     a.pass = 2;
     a.cursor = counters + 1;
-    if (m.mlp_precision == 0) CK(launch_head(a, -1, st));
-    else if (use_v2) CK(launch_head_v2(a, v2, m.mlp_precision, st));
-    else CK(launch_head_tc(a, m.tc, m.mlp_precision, -1, st));
+    if (const int rc = launch_head_pass(hk, m, a, v2, st); rc != GFPP_OK) return rc;
     if (g_profile) CKN(cudaEventRecord(g_ev[2], st));
     CK(launch_epilogue(t, st));
     if (g_profile) CKN(cudaEventRecord(g_ev[3], st));
@@ -759,37 +766,37 @@ int gfpp_render_frames(const gfpp_model *model, const gfpp_frames *fr, const gfp
 // ------------------------------------------------------------------ (C) super-resolution head (sr_kernel.cu)
 namespace {
 struct SrHost {
+    using Handle = gfpp_sr_model;
+    static constexpr uint32_t kMagic = 0x67667372u;  // "gfsr"
+    static constexpr const char *kPacker = "gfpp_sr_pack";
     uint32_t magic;
     const float *conv_in_w, *bias[4], *rgb_w[2], *rgb_b[2];
     const unsigned char *tiles[3];
 };
 static_assert(sizeof(SrHost) <= sizeof(gfpp_sr_model), "gfpp_sr_model opaque storage too small");
-constexpr uint32_t kSrMagic = 0x67667372u;  // "gfsr"
 struct SrPacked { size_t conv_in_w, bias[4], rgb_w[2], rgb_b[2], tiles[3], total; };
 SrPacked sr_packed_layout() {
     SrPacked L;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 1023) / 1024 * 1024; return r; };
-    L.conv_in_w = take(27 * 128 * 4);
+    Bump b;   // 1024-byte blocks: the weight tiles are SW128 operand images
+    L.conv_in_w = b.take(27 * 128 * 4, 1024);
     const int nb[4] = {128, 128, 64, 64};
-    for (int i = 0; i < 4; ++i) L.bias[i] = take((size_t)nb[i] * 4);
-    L.rgb_w[0] = take(3 * 128 * 4); L.rgb_w[1] = take(3 * 64 * 4);
-    L.rgb_b[0] = take(16); L.rgb_b[1] = take(16);
-    for (int l = 0; l < 3; ++l) L.tiles[l] = take((size_t)sr_layer_weight_bytes(l));
-    L.total = o;
+    for (int i = 0; i < 4; ++i) L.bias[i] = b.take((size_t)nb[i] * 4, 1024);
+    L.rgb_w[0] = b.take(3 * 128 * 4, 1024); L.rgb_w[1] = b.take(3 * 64 * 4, 1024);
+    L.rgb_b[0] = b.take(16, 1024); L.rgb_b[1] = b.take(16, 1024);
+    for (int l = 0; l < 3; ++l) L.tiles[l] = b.take((size_t)sr_layer_weight_bytes(l), 1024);
+    L.total = b.end;
     return L;
 }
 struct SrWork { size_t x0a, x0b, img0, x1a, total; };
 SrWork sr_work_layout(uint32_t F, uint32_t R) {
     SrWork W;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
+    Bump b;
     const size_t px = (size_t)F * R * R;
-    W.x0a = take(px * 128 * 2);
-    W.x0b = take(px * 128 * 2);
-    W.img0 = take(px * 3 * 4);
-    W.x1a = take(px * 4 * 64 * 2);
-    W.total = o;
+    W.x0a = b.take(px * 128 * 2);
+    W.x0b = b.take(px * 128 * 2);
+    W.img0 = b.take(px * 3 * 4);
+    W.x1a = b.take(px * 4 * 64 * 2);
+    W.total = b.end;
     return W;
 }
 }  // namespace
@@ -799,13 +806,13 @@ extern "C" {
 size_t gfpp_sr_packed_bytes(void) { return sr_packed_layout().total; }
 
 int gfpp_sr_pack(const gfpp_sr_desc *d, void *packed, size_t packed_bytes, gfpp_sr_model *model, void *stream) {
-    if (!d || !packed || !model) return fail(GFPP_ERR_INVALID, "sr_pack: null pointer%s");
-    if (!d->conv_in_w || !d->conv0_w || !d->up_w || !d->conv1_w) return fail(GFPP_ERR_INVALID, "sr_pack: null weight%s");
-    for (int i = 0; i < 4; ++i) if (!d->bias[i]) return fail(GFPP_ERR_INVALID, "sr_pack: null bias%s");
-    for (int i = 0; i < 2; ++i) if (!d->rgb_w[i] || !d->rgb_b[i]) return fail(GFPP_ERR_INVALID, "sr_pack: null toRGB weight%s");
+    if (!d || !packed || !model) return fail(GFPP_ERR_INVALID, "sr_pack: null pointer");
+    if (!d->conv_in_w || !d->conv0_w || !d->up_w || !d->conv1_w) return fail(GFPP_ERR_INVALID, "sr_pack: null weight");
+    for (int i = 0; i < 4; ++i) if (!d->bias[i]) return fail(GFPP_ERR_INVALID, "sr_pack: null bias");
+    for (int i = 0; i < 2; ++i) if (!d->rgb_w[i] || !d->rgb_b[i]) return fail(GFPP_ERR_INVALID, "sr_pack: null toRGB weight");
     const SrPacked L = sr_packed_layout();
-    if (packed_bytes < L.total) return fail(GFPP_ERR_WORKSPACE, "sr_pack: packed buffer too small%s");
-    if (((uintptr_t)packed & 1023u) != 0) return fail(GFPP_ERR_INVALID, "sr_pack: packed buffer must be 1024-byte aligned%s");
+    if (packed_bytes < L.total) return fail(GFPP_ERR_WORKSPACE, "sr_pack: packed buffer too small");
+    if (((uintptr_t)packed & 1023u) != 0) return fail(GFPP_ERR_INVALID, "sr_pack: packed buffer must be 1024-byte aligned");
     cudaStream_t st = (cudaStream_t)stream;
     char *base = (char *)packed;
     g_launches = 0;
@@ -830,7 +837,7 @@ int gfpp_sr_pack(const gfpp_sr_desc *d, void *packed, size_t packed_bytes, gfpp_
     }
     SrHost m;
     memset(&m, 0, sizeof(m));
-    m.magic = kSrMagic;
+    m.magic = SrHost::kMagic;
     m.conv_in_w = (const float *)(base + L.conv_in_w);
     for (int i = 0; i < 4; ++i) m.bias[i] = (const float *)(base + L.bias[i]);
     for (int i = 0; i < 2; ++i) { m.rgb_w[i] = (const float *)(base + L.rgb_w[i]); m.rgb_b[i] = (const float *)(base + L.rgb_b[i]); }
@@ -851,8 +858,7 @@ static int sr_forward_impl(const char *who, const gfpp_sr_model *model, uint32_t
     if (!model || !rgb_in || (!out && !out_u8) || !workspace) return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
     if (((uintptr_t)out_u8 & 3u) != 0) return fail(GFPP_ERR_INVALID, "%s: out_u8 must be 4-byte aligned", who);
     SrHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kSrMagic) return fail(GFPP_ERR_INVALID, "%s: model handle not initialised by gfpp_sr_pack", who);
+    if (const int rc = unpack(who, model, m); rc != GFPP_OK) return rc;
     if (n_frames == 0 || in_res == 0 || in_res % 128 != 0 || in_res > 1024) return fail(GFPP_ERR_UNSUPPORTED, "%s: in_res must be a multiple of 128 (256 in the reference)", who);
     if ((uint64_t)n_frames * in_res * in_res * 4 >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: too many frames per call", who);
     const SrWork W = sr_work_layout(n_frames, in_res);
@@ -890,7 +896,7 @@ extern "C" {
 
 int gfpp_sr_forward(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in, const float *const noise[4],
                     uint32_t noise_per_frame, float *out, int clamp01, void *workspace, size_t workspace_bytes, void *stream) {
-    if (!out) return fail(GFPP_ERR_INVALID, "sr_forward: null pointer%s");
+    if (!out) return fail(GFPP_ERR_INVALID, "sr_forward: null pointer");
     return sr_forward_impl("sr_forward", model, n_frames, in_res, rgb_in, noise, noise_per_frame, out, nullptr, clamp01, workspace,
                            workspace_bytes, stream);
 }
@@ -906,6 +912,9 @@ int gfpp_sr_forward_video(const gfpp_sr_model *model, uint32_t n_frames, uint32_
 // ------------------------------------------------------------------ (C) torso field of the torso-SR checkpoints (torso_sr_kernel.cu)
 namespace {
 struct TorsoSrHost {
+    using Handle = gfpp_torso_sr_model;
+    static constexpr uint32_t kMagic = 0x67667473u;  // "gfts"
+    static constexpr const char *kPacker = "gfpp_torso_sr_pack";
     uint32_t magic;
     int head_aware;
     GridMeta tor_gm;
@@ -918,27 +927,24 @@ struct TorsoSrHost {
     float density_thresh_torso, torso_shrink;
 };
 static_assert(sizeof(TorsoSrHost) <= sizeof(gfpp_torso_sr_model), "gfpp_torso_sr_model opaque storage too small");
-constexpr uint32_t kTorsoSrMagic = 0x67667473u;  // "gfts"
 struct TorsoSrPacked { size_t wd0, wd1, wd2, wc0, wc1, wc2, ha, total; };
 TorsoSrPacked torso_sr_packed_layout() {
     TorsoSrPacked L;
-    size_t o = 0;
-    auto take = [&](size_t floats) { size_t r = o; o += (floats * 4 + 255) / 256 * 256; return r; };
-    L.wd0 = take(TORSO_SR_KD0 * 64); L.wd1 = take(64 * 64); L.wd2 = take(2 * 64);
-    L.wc0 = take(TORSO_SR_KC0 * 32); L.wc1 = take(32 * 32); L.wc2 = take(4 * 32);
-    L.ha = take(TORSO_SR_HA_FLOATS);
-    L.total = o;
+    Bump b;
+    L.wd0 = b.take(TORSO_SR_KD0 * 64 * 4); L.wd1 = b.take(64 * 64 * 4); L.wd2 = b.take(2 * 64 * 4);
+    L.wc0 = b.take(TORSO_SR_KC0 * 32 * 4); L.wc1 = b.take(32 * 32 * 4); L.wc2 = b.take(4 * 32 * 4);
+    L.ha = b.take(TORSO_SR_HA_FLOATS * 4);
+    L.total = b.end;
     return L;
 }
 struct TorsoSrWork { size_t bias_def, bias_can, pcount, total; };
 TorsoSrWork torso_sr_work_layout(uint32_t F) {
     TorsoSrWork W;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
-    W.bias_def = take((size_t)F * 64 * 4);
-    W.bias_can = take((size_t)F * 32 * 4);
-    W.pcount = take((size_t)F * 4);
-    W.total = o;
+    Bump b;
+    W.bias_def = b.take((size_t)F * 64 * 4);
+    W.bias_can = b.take((size_t)F * 32 * 4);
+    W.pcount = b.take((size_t)F * 4);
+    W.total = b.end;
     return W;
 }
 __global__ void k_copy_ints(const int *src, int n, int32_t *dst) {
@@ -952,24 +958,24 @@ extern "C" {
 size_t gfpp_torso_sr_packed_bytes(void) { return torso_sr_packed_layout().total; }
 
 int gfpp_torso_sr_pack(const gfpp_torso_sr_desc *d, void *packed, size_t packed_bytes, gfpp_torso_sr_model *model, void *stream) {
-    if (!d || !packed || !model) return fail(GFPP_ERR_INVALID, "torso_sr_pack: null pointer%s");
+    if (!d || !packed || !model) return fail(GFPP_ERR_INVALID, "torso_sr_pack: null pointer");
     const TorsoSrPacked L = torso_sr_packed_layout();
-    if (packed_bytes < L.total) return fail(GFPP_ERR_WORKSPACE, "torso_sr_pack: packed buffer too small%s");
+    if (packed_bytes < L.total) return fail(GFPP_ERR_WORKSPACE, "torso_sr_pack: packed buffer too small");
     for (int i = 0; i < 3; ++i)
-        if (!d->torso_deform_w[i] || !d->torso_canon_w[i]) return fail(GFPP_ERR_INVALID, "torso_sr_pack: null torso weight%s");
-    if (!d->density_grid_torso || !d->torso_grid.embeddings || !d->torso_grid.offsets_host) return fail(GFPP_ERR_INVALID, "torso_sr_pack: null grid%s");
-    if (d->torso_code_dim > 10 || (d->torso_code_dim > 0 && !d->torso_code)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_pack: torso_code_dim <= 10 (with a code pointer)%s");
+        if (!d->torso_deform_w[i] || !d->torso_canon_w[i]) return fail(GFPP_ERR_INVALID, "torso_sr_pack: null torso weight");
+    if (!d->density_grid_torso || !d->torso_grid.embeddings || !d->torso_grid.offsets_host) return fail(GFPP_ERR_INVALID, "torso_sr_pack: null grid");
+    if (d->torso_code_dim > 10 || (d->torso_code_dim > 0 && !d->torso_code)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_pack: torso_code_dim <= 10 (with a code pointer)");
     if (d->head_aware)
         for (int i = 0; i < 3; ++i)
-            if (!d->ha_w[i] || !d->ha_b[i]) return fail(GFPP_ERR_INVALID, "torso_sr_pack: null head-aware encoder weight%s");
+            if (!d->ha_w[i] || !d->ha_b[i]) return fail(GFPP_ERR_INVALID, "torso_sr_pack: null head-aware encoder weight");
     TorsoSrHost m;
     memset(&m, 0, sizeof(m));
-    m.magic = kTorsoSrMagic;
+    m.magic = TorsoSrHost::kMagic;
     if (d->torso_grid.num_levels != 16 ||
         fill_grid_meta(m.tor_gm, d->torso_grid.offsets_host, d->torso_grid.input_dim, d->torso_grid.num_levels, d->torso_grid.log2_per_level_scale,
                        d->torso_grid.base_resolution, d->torso_grid.gridtype, d->torso_grid.align_corners, d->torso_grid.interp) != 0 ||
         m.tor_gm.dim != 2)
-        return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_pack: the torso grid must be 2-D with 16 levels x 2 features%s");
+        return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_pack: the torso grid must be 2-D with 16 levels x 2 features");
     cudaStream_t st = (cudaStream_t)stream;
     char *base = (char *)packed;
     g_launches = 0;
@@ -1012,15 +1018,14 @@ size_t gfpp_torso_sr_workspace_bytes(uint32_t n_frames) { return torso_sr_work_l
 int gfpp_torso_sr_composite(const gfpp_torso_sr_model *model, const gfpp_torso_sr_frames *fr, float *rgb_map, float *torso_alpha_map,
                             float *torso_rgb_map, float *torso_deform, int32_t *torso_pixels, void *workspace, size_t workspace_bytes,
                             void *stream) {
-    if (!model || !fr || !rgb_map || !workspace) return fail(GFPP_ERR_INVALID, "torso_sr_composite: null pointer%s");
+    if (!model || !fr || !rgb_map || !workspace) return fail(GFPP_ERR_INVALID, "torso_sr_composite: null pointer");
     TorsoSrHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kTorsoSrMagic) return fail(GFPP_ERR_INVALID, "torso_sr_composite: model handle not initialised by gfpp_torso_sr_pack%s");
-    if (!fr->image || !fr->weights_sum || !fr->lm68 || !fr->bg_coords) return fail(GFPP_ERR_INVALID, "torso_sr_composite: image, weights_sum, lm68 and bg_coords are required%s");
-    if (fr->n_frames == 0 || fr->n_rays == 0) return fail(GFPP_ERR_INVALID, "torso_sr_composite: empty clip%s");
-    if ((uint64_t)fr->n_frames * fr->n_rays >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_composite: F*N must be < 2^31%s");
+    if (const int rc = unpack("torso_sr_composite", model, m); rc != GFPP_OK) return rc;
+    if (!fr->image || !fr->weights_sum || !fr->lm68 || !fr->bg_coords) return fail(GFPP_ERR_INVALID, "torso_sr_composite: image, weights_sum, lm68 and bg_coords are required");
+    if (fr->n_frames == 0 || fr->n_rays == 0) return fail(GFPP_ERR_INVALID, "torso_sr_composite: empty clip");
+    if ((uint64_t)fr->n_frames * fr->n_rays >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_composite: F*N must be < 2^31");
     const TorsoSrWork W = torso_sr_work_layout(fr->n_frames);
-    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "torso_sr_composite: workspace too small%s");
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "torso_sr_composite: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     g_launches = 0;
@@ -1059,10 +1064,10 @@ int gfpp_march_rays_train(const float *rays_o, const float *rays_d, const uint8_
                           float *deltas, int32_t *rays, int32_t *counter, const float *noises, void *scratch, size_t scratch_bytes,
                           void *stream) {
     if (!rays_o || !rays_d || !grid || !nears || !fars || !xyzs || !dirs || !deltas || !rays || !counter || !noises || !scratch)
-        return fail(GFPP_ERR_INVALID, "march_rays_train: null pointer%s");
-    if (C < 1 || C > 8 || H < 1 || H > 1024 || max_steps < 1) return fail(GFPP_ERR_INVALID, "march_rays_train: bad C/H/max_steps%s");
-    if (scratch_bytes < march_train_scratch_bytes(N)) return fail(GFPP_ERR_WORKSPACE, "march_rays_train: scratch too small%s");
-    if (N > (1u << 24)) return fail(GFPP_ERR_UNSUPPORTED, "march_rays_train: N <= 2^24 rays per call%s");
+        return fail(GFPP_ERR_INVALID, "march_rays_train: null pointer");
+    if (C < 1 || C > 8 || H < 1 || H > 1024 || max_steps < 1) return fail(GFPP_ERR_INVALID, "march_rays_train: bad C/H/max_steps");
+    if (scratch_bytes < march_train_scratch_bytes(N)) return fail(GFPP_ERR_WORKSPACE, "march_rays_train: scratch too small");
+    if (N > (1u << 24)) return fail(GFPP_ERR_UNSUPPORTED, "march_rays_train: N <= 2^24 rays per call");
     MarchConst mc;
     march_const_init(mc, bound, dt_gamma, max_steps, C, H, grid);
     g_launches = 0;
@@ -1075,7 +1080,7 @@ int gfpp_march_rays_train(const float *rays_o, const float *rays_d, const uint8_
 
 int gfpp_march_rays_train_backward(const float *grad_xyzs, const float *grad_dirs, const int32_t *rays, const float *deltas, uint32_t N,
                                    uint32_t M, float *grad_rays_o, float *grad_rays_d, void *stream) {
-    if (!grad_xyzs || !grad_dirs || !rays || !deltas || !grad_rays_o || !grad_rays_d) return fail(GFPP_ERR_INVALID, "march_rays_train_backward: null pointer%s");
+    if (!grad_xyzs || !grad_dirs || !rays || !deltas || !grad_rays_o || !grad_rays_d) return fail(GFPP_ERR_INVALID, "march_rays_train_backward: null pointer");
     g_launches = 0;
     CK(launch_march_rays_train_backward(grad_xyzs, grad_dirs, (const int *)rays, deltas, N, M, grad_rays_o, grad_rays_d, (cudaStream_t)stream));
     return GFPP_OK;
@@ -1085,7 +1090,7 @@ int gfpp_composite_rays_train_forward(const float *sigmas, const float *rgbs, co
                                       uint32_t M, uint32_t N, float T_thresh, float *weights_sum, float *ambient_sum, float *depth,
                                       float *image, void *stream) {
     if (!sigmas || !rgbs || !ambient || !deltas || !rays || !weights_sum || !ambient_sum || !depth || !image)
-        return fail(GFPP_ERR_INVALID, "composite_rays_train_forward: null pointer%s");
+        return fail(GFPP_ERR_INVALID, "composite_rays_train_forward: null pointer");
     g_launches = 0;
     CK(launch_composite_train_forward(sigmas, rgbs, ambient, deltas, (const int *)rays, M, N, T_thresh, weights_sum, ambient_sum, depth, image,
                                       (cudaStream_t)stream));
@@ -1098,7 +1103,7 @@ int gfpp_composite_rays_train_backward(const float *grad_weights_sum, const floa
                                        float T_thresh, float *grad_sigmas, float *grad_rgbs, float *grad_ambient, void *stream) {
     if (!grad_weights_sum || !grad_ambient_sum || !grad_image || !sigmas || !rgbs || !ambient || !deltas || !rays || !weights_sum || !ambient_sum ||
         !image || !grad_sigmas || !grad_rgbs || !grad_ambient)
-        return fail(GFPP_ERR_INVALID, "composite_rays_train_backward: null pointer%s");
+        return fail(GFPP_ERR_INVALID, "composite_rays_train_backward: null pointer");
     g_launches = 0;
     CK(launch_composite_train_backward(grad_weights_sum, grad_ambient_sum, grad_image, sigmas, rgbs, ambient, deltas, (const int *)rays,
                                        weights_sum, ambient_sum, image, M, N, T_thresh, grad_sigmas, grad_rgbs, grad_ambient, (cudaStream_t)stream));
@@ -1108,11 +1113,9 @@ int gfpp_composite_rays_train_backward(const float *grad_weights_sum, const floa
 int gfpp_grid_encode_forward_dydx(const float *inputs, const float *embeddings, const int32_t *offsets_host, float *outputs, uint32_t B,
                                   uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, float *dy_dx, uint32_t gridtype, int align_corners,
                                   uint32_t interp, void *stream) {
-    if (!inputs || !embeddings || !offsets_host || !outputs || !dy_dx) return fail(GFPP_ERR_INVALID, "grid_encode_forward_dydx: null pointer%s");
-    if (C != 2) return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: this build supports C == 2 only%s");
+    if (!inputs || !embeddings || !offsets_host || !outputs || !dy_dx) return fail(GFPP_ERR_INVALID, "grid_encode_forward_dydx: null pointer");
     GridMeta gm;
-    if (fill_grid_meta(gm, offsets_host, D, L, S, H, gridtype, align_corners, interp) != 0)
-        return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: D must be 2 or 3 and L <= 16%s");
+    if (const int rc = grid_op_meta(gm, offsets_host, D, C, L, S, H, gridtype, align_corners, interp); rc != GFPP_OK) return rc;
     g_launches = 0;
     CK(launch_grid_encode_dydx(gm, inputs, embeddings, outputs, dy_dx, B, (cudaStream_t)stream));
     return GFPP_OK;
@@ -1122,12 +1125,10 @@ int gfpp_grid_encode_backward(const float *grad, const float *inputs, const floa
                               float *grad_embeddings, uint32_t B, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, const float *dy_dx,
                               float *grad_inputs, uint32_t gridtype, int align_corners, uint32_t interp, void *stream) {
     (void)embeddings;   // the reference passes the table too (gridencoder.h:13) but only uses its dtype
-    if (!grad || !inputs || !offsets_host || !grad_embeddings) return fail(GFPP_ERR_INVALID, "grid_encode_backward: null pointer%s");
-    if ((dy_dx == nullptr) != (grad_inputs == nullptr)) return fail(GFPP_ERR_INVALID, "grid_encode_backward: dy_dx and grad_inputs go together%s");
-    if (C != 2) return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: this build supports C == 2 only%s");
+    if (!grad || !inputs || !offsets_host || !grad_embeddings) return fail(GFPP_ERR_INVALID, "grid_encode_backward: null pointer");
+    if ((dy_dx == nullptr) != (grad_inputs == nullptr)) return fail(GFPP_ERR_INVALID, "grid_encode_backward: dy_dx and grad_inputs go together");
     GridMeta gm;
-    if (fill_grid_meta(gm, offsets_host, D, L, S, H, gridtype, align_corners, interp) != 0)
-        return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: D must be 2 or 3 and L <= 16%s");
+    if (const int rc = grid_op_meta(gm, offsets_host, D, C, L, S, H, gridtype, align_corners, interp); rc != GFPP_OK) return rc;
     g_launches = 0;
     int nl = 0;
     CKN(launch_grid_backward(gm, grad, inputs, grad_embeddings, dy_dx, grad_inputs, B, &nl, (cudaStream_t)stream));
@@ -1137,11 +1138,9 @@ int gfpp_grid_encode_backward(const float *grad, const float *inputs, const floa
 
 int gfpp_grad_total_variation(const float *inputs, const float *embeddings, float *grad, const int32_t *offsets_host, float weight, uint32_t B,
                               uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, uint32_t gridtype, int align_corners, void *stream) {
-    if (!inputs || !embeddings || !grad || !offsets_host) return fail(GFPP_ERR_INVALID, "grad_total_variation: null pointer%s");
-    if (C != 2) return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: this build supports C == 2 only%s");
+    if (!inputs || !embeddings || !grad || !offsets_host) return fail(GFPP_ERR_INVALID, "grad_total_variation: null pointer");
     GridMeta gm;
-    if (fill_grid_meta(gm, offsets_host, D, L, S, H, gridtype, align_corners, 0) != 0)
-        return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: D must be 2 or 3 and L <= 16%s");
+    if (const int rc = grid_op_meta(gm, offsets_host, D, C, L, S, H, gridtype, align_corners, 0); rc != GFPP_OK) return rc;
     g_launches = 0;
     CK(launch_grad_tv(gm, inputs, embeddings, grad, weight, B, (cudaStream_t)stream));
     return GFPP_OK;
@@ -1153,10 +1152,8 @@ namespace {
 // the shape checks of the fp32 ops (fill_grid_meta: D, L, non-empty levels), then the raw level layout for the device
 int half_grid_args(HalfGridArgs &g, const int32_t *offsets, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, uint32_t gridtype,
                    int align_corners, uint32_t interp) {
-    if (C != 2) return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: this build supports C == 2 only%s");
     GridMeta gm;
-    if (fill_grid_meta(gm, offsets, D, L, S, H, gridtype, align_corners, interp) != 0)
-        return fail(GFPP_ERR_UNSUPPORTED, "GridEncoding: D must be 2 or 3 and L <= 16%s");
+    if (const int rc = grid_op_meta(gm, offsets, D, C, L, S, H, gridtype, align_corners, interp); rc != GFPP_OK) return rc;
     memset(&g, 0, sizeof(g));
     for (uint32_t l = 0; l <= L; ++l) g.offset[l] = (uint32_t)offsets[l];
     g.L = L;
@@ -1175,12 +1172,12 @@ bool misaligned4(const void *p) { return ((uintptr_t)p & 3u) != 0; }
 int gfpp_grid_encode_forward_half(const float *inputs, const uint16_t *embeddings, const int32_t *offsets_host, uint16_t *outputs,
                                   uint32_t B, uint32_t D, uint32_t C, uint32_t L, float S, uint32_t H, uint16_t *dy_dx, uint32_t gridtype,
                                   int align_corners, uint32_t interp, void *stream) {
-    if (!inputs || !embeddings || !offsets_host || !outputs) return fail(GFPP_ERR_INVALID, "grid_encode_forward_half: null pointer%s");
+    if (!inputs || !embeddings || !offsets_host || !outputs) return fail(GFPP_ERR_INVALID, "grid_encode_forward_half: null pointer");
     HalfGridArgs g;
     const int rc = half_grid_args(g, offsets_host, D, C, L, S, H, gridtype, align_corners, interp);
     if (rc != GFPP_OK) return rc;
     if (misaligned4(embeddings) || misaligned4(outputs) || misaligned4(dy_dx))
-        return fail(GFPP_ERR_INVALID, "grid_encode_forward_half: half2 buffers must be 4-byte aligned%s");
+        return fail(GFPP_ERR_INVALID, "grid_encode_forward_half: half2 buffers must be 4-byte aligned");
     g_launches = 0;
     if (B == 0) return GFPP_OK;
     CK(launch_grid_half_forward(g, D, inputs, embeddings, outputs, dy_dx, B, (cudaStream_t)stream));
@@ -1192,14 +1189,14 @@ int gfpp_grid_encode_backward_half(const uint16_t *grad, const float *inputs, co
                                    const uint16_t *dy_dx, uint16_t *grad_inputs, uint32_t gridtype, int align_corners, uint32_t interp,
                                    void *stream) {
     (void)embeddings;   // only its dtype matters to the reference (gridencoder.cu:497)
-    if (!grad || !inputs || !offsets_host || !grad_embeddings) return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: null pointer%s");
+    if (!grad || !inputs || !offsets_host || !grad_embeddings) return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: null pointer");
     if ((dy_dx == nullptr) != (grad_inputs == nullptr))
-        return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: dy_dx and grad_inputs go together%s");
+        return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: dy_dx and grad_inputs go together");
     HalfGridArgs g;
     const int rc = half_grid_args(g, offsets_host, D, C, L, S, H, gridtype, align_corners, interp);
     if (rc != GFPP_OK) return rc;
     if (misaligned4(grad) || misaligned4(grad_embeddings) || misaligned4(dy_dx))
-        return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: half2 buffers must be 4-byte aligned%s");
+        return fail(GFPP_ERR_INVALID, "grid_encode_backward_half: half2 buffers must be 4-byte aligned");
     g_launches = 0;
     if (B == 0) return GFPP_OK;
     int nl = 0;
@@ -1209,37 +1206,37 @@ int gfpp_grid_encode_backward_half(const uint16_t *grad, const float *inputs, co
 }
 
 int gfpp_packbits(const float *grid, uint32_t N, float density_thresh, uint8_t *bitfield, void *stream) {
-    if (!grid || !bitfield) return fail(GFPP_ERR_INVALID, "packbits: null pointer%s");
-    if (((uintptr_t)grid & 15u) != 0) return fail(GFPP_ERR_INVALID, "packbits: grid must be 16-byte aligned%s");
+    if (!grid || !bitfield) return fail(GFPP_ERR_INVALID, "packbits: null pointer");
+    if (((uintptr_t)grid & 15u) != 0) return fail(GFPP_ERR_INVALID, "packbits: grid must be 16-byte aligned");
     g_launches = 0;
     CK(launch_packbits(grid, N, density_thresh, bitfield, (cudaStream_t)stream));
     return GFPP_OK;
 }
 
 int gfpp_morton3D(const int32_t *coords, uint32_t N, int32_t *indices, void *stream) {
-    if (!coords || !indices) return fail(GFPP_ERR_INVALID, "morton3D: null pointer%s");
+    if (!coords || !indices) return fail(GFPP_ERR_INVALID, "morton3D: null pointer");
     g_launches = 0;
     CK(launch_morton3D((const int *)coords, N, (int *)indices, (cudaStream_t)stream));
     return GFPP_OK;
 }
 
 int gfpp_morton3D_invert(const int32_t *indices, uint32_t N, int32_t *coords, void *stream) {
-    if (!coords || !indices) return fail(GFPP_ERR_INVALID, "morton3D_invert: null pointer%s");
+    if (!coords || !indices) return fail(GFPP_ERR_INVALID, "morton3D_invert: null pointer");
     g_launches = 0;
     CK(launch_morton3D_invert((const int *)indices, N, (int *)coords, (cudaStream_t)stream));
     return GFPP_OK;
 }
 
 int gfpp_morton3D_dilation(const float *grid, uint32_t C, uint32_t H, float *grid_dilation, void *stream) {
-    if (!grid || !grid_dilation) return fail(GFPP_ERR_INVALID, "morton3D_dilation: null pointer%s");
-    if (C < 1 || C > 8 || H < 1 || H > 1024) return fail(GFPP_ERR_INVALID, "morton3D_dilation: bad C/H%s");
+    if (!grid || !grid_dilation) return fail(GFPP_ERR_INVALID, "morton3D_dilation: null pointer");
+    if (C < 1 || C > 8 || H < 1 || H > 1024) return fail(GFPP_ERR_INVALID, "morton3D_dilation: bad C/H");
     g_launches = 0;
     CK(launch_morton3D_dilation(grid, C, H, grid_dilation, (cudaStream_t)stream));
     return GFPP_OK;
 }
 
 int gfpp_sph_from_ray(const float *rays_o, const float *rays_d, float radius, uint32_t N, float *coords, void *stream) {
-    if (!rays_o || !rays_d || !coords) return fail(GFPP_ERR_INVALID, "sph_from_ray: null pointer%s");
+    if (!rays_o || !rays_d || !coords) return fail(GFPP_ERR_INVALID, "sph_from_ray: null pointer");
     g_launches = 0;
     CK(launch_sph_from_ray(rays_o, rays_d, radius, N, coords, (cudaStream_t)stream));
     return GFPP_OK;
@@ -1261,32 +1258,18 @@ struct GridWork {
 
 GridWork grid_work_layout(uint32_t C, uint32_t H) {
     GridWork W;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
-    W.tmp = take((size_t)C * H * H * H * 4);
-    W.partial = take((size_t)dilate_ema_blocks(C, H) * 8);
-    W.thresh = take(4);
-    W.total = o;
+    Bump b;
+    W.tmp = b.take((size_t)C * H * H * H * 4);
+    W.partial = b.take((size_t)dilate_ema_blocks(C, H) * 8);
+    W.thresh = b.take(4);
+    W.total = b.end;
     return W;
-}
-
-// the head field of a packed model, for k_density: fp32 weight chunks and fp32 tables (quads where the mode packed them)
-HeadArgs density_head_args(const ModelHost &m) {
-    HeadArgs a;
-    memset(&a, 0, sizeof(a));
-    a.pos_gm = m.pos_gm; a.amb_gm = m.amb_gm;
-    a.pos_tab = m.pos_tab; a.amb_tab = m.amb_tab;
-    a.pos_quads = m.pos_quads; a.amb_quads = m.amb_quads;
-    a.pos_octs = m.pos_octs; a.amb_octs = m.amb_octs;
-    a.wide = m.wide; a.narrow = m.narrow;
-    for (int c = 0; c < HEAD_NCHUNK; ++c) { a.chunk_off[c] = m.chunk_off[c]; a.chunk_k[c] = kChunkK[c]; }
-    return a;
 }
 
 // the field the model's mode renders where a query kernel for it exists: fp16 -> wgmma over the fp16 operand images and oct tables;
 // fp32 / bf16x3 / bf16 / robust -> the fp32 FFMA field (robust renders a split-precision approximation of it, DESIGN.md section 6)
 cudaError_t launch_density_for(const ModelHost &m, const DensityArgs &d, cudaStream_t st) {
-    const HeadArgs a = density_head_args(m);
+    const HeadArgs a = head_field_args(m);
     if (m.mlp_precision == 1 && m.tc.w_hi && m.pos_octs && m.amb_octs) return launch_density_tc(a, m.tc, d, st);
     return launch_density(a, d, st);
 }
@@ -1309,13 +1292,12 @@ extern "C" {
 
 int gfpp_density_query(const gfpp_model *model, const float *xyzs, uint32_t n, const float *cond_feat, float *sigma, float *geo_feat,
                        void *stream) {
-    if (!model || !xyzs || !cond_feat || !sigma) return fail(GFPP_ERR_INVALID, "density_query: null pointer%s");
+    if (!model || !xyzs || !cond_feat || !sigma) return fail(GFPP_ERR_INVALID, "density_query: null pointer");
     ModelHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "density_query: model handle not initialised by gfpp_model_pack%s");
+    if (const int rc = unpack("density_query", model, m); rc != GFPP_OK) return rc;
     if (!aligned16(cond_feat) || (geo_feat && !aligned16(geo_feat)))
-        return fail(GFPP_ERR_INVALID, "density_query: cond_feat and geo_feat must be 16-byte aligned%s");
-    if (n >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "density_query: n must be < 2^31%s");
+        return fail(GFPP_ERR_INVALID, "density_query: cond_feat and geo_feat must be 16-byte aligned");
+    if (n >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "density_query: n must be < 2^31");
     DensityArgs d;
     memset(&d, 0, sizeof(d));
     d.n = n; d.xyzs = xyzs; d.cond = cond_feat; d.bound = m.bound;
@@ -1332,17 +1314,16 @@ size_t gfpp_density_grid_workspace_bytes(uint32_t cascade, uint32_t grid_size) {
 int gfpp_density_grid_update(const gfpp_model *model, const float *cond_feat, const float *noise, float decay, float density_thresh,
                              float *density_grid, float *mean_out, float *tmp_grid, void *workspace, size_t workspace_bytes, void *stream) {
     if (!model || !cond_feat || !noise || !density_grid || !mean_out || !workspace)
-        return fail(GFPP_ERR_INVALID, "density_grid_update: null pointer%s");
+        return fail(GFPP_ERR_INVALID, "density_grid_update: null pointer");
     ModelHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "density_grid_update: model handle not initialised by gfpp_model_pack%s");
+    if (const int rc = unpack("density_grid_update", model, m); rc != GFPP_OK) return rc;
     const uint32_t C = m.cascade, H = m.grid_size;
     if (!grid_shape_ok(C, H))
-        return fail(GFPP_ERR_UNSUPPORTED, "density_grid_update: needs cascade 1..8, grid_size a power of two in 8..512, C*H^3 <= 2^30%s");
+        return fail(GFPP_ERR_UNSUPPORTED, "density_grid_update: needs cascade 1..8, grid_size a power of two in 8..512, C*H^3 <= 2^30");
     if (!aligned16(cond_feat) || !aligned16(density_grid) || (tmp_grid && !aligned16(tmp_grid)))
-        return fail(GFPP_ERR_INVALID, "density_grid_update: cond_feat, density_grid and tmp_grid must be 16-byte aligned%s");
+        return fail(GFPP_ERR_INVALID, "density_grid_update: cond_feat, density_grid and tmp_grid must be 16-byte aligned");
     const GridWork W = grid_work_layout(C, H);
-    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "density_grid_update: workspace too small%s");
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "density_grid_update: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     float *tmp = tmp_grid ? tmp_grid : (float *)(ws + W.tmp);
@@ -1374,10 +1355,10 @@ int gfpp_density_grid_update(const gfpp_model *model, const float *cond_feat, co
 
 int gfpp_mark_untrained_grid(const float *poses_c2w, uint32_t n_poses, double fx, double fy, double cx, double cy, double bound,
                              uint32_t cascade, uint32_t grid_size, float *density_grid, void *stream) {
-    if (!poses_c2w || !density_grid) return fail(GFPP_ERR_INVALID, "mark_untrained_grid: null pointer%s");
+    if (!poses_c2w || !density_grid) return fail(GFPP_ERR_INVALID, "mark_untrained_grid: null pointer");
     if (!grid_shape_ok(cascade, grid_size))
-        return fail(GFPP_ERR_UNSUPPORTED, "mark_untrained_grid: needs cascade 1..8, grid_size a power of two in 8..512, C*H^3 <= 2^30%s");
-    if (n_poses == 0 || !(fx != 0.0) || !(fy != 0.0)) return fail(GFPP_ERR_INVALID, "mark_untrained_grid: no poses or zero focal length%s");
+        return fail(GFPP_ERR_UNSUPPORTED, "mark_untrained_grid: needs cascade 1..8, grid_size a power of two in 8..512, C*H^3 <= 2^30");
+    if (n_poses == 0 || !(fx != 0.0) || !(fy != 0.0)) return fail(GFPP_ERR_INVALID, "mark_untrained_grid: no poses or zero focal length");
     float scale[8], pad[8];
     cascade_constants(bound, cascade, grid_size, scale, nullptr, pad);
     g_launches = 0;
@@ -1400,14 +1381,13 @@ struct TorsoGridWork {
 
 TorsoGridWork torso_grid_work_layout(uint32_t H) {
     TorsoGridWork W;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
-    W.bias_def = take(64 * 4);
-    W.bias_can = take(32 * 4);
-    W.tmp = take((size_t)H * H * 4);
-    W.partial = take((size_t)torso_dilate_ema_blocks(H) * 8);
-    W.thresh = take(4);
-    W.total = o;
+    Bump b;
+    W.bias_def = b.take(64 * 4);
+    W.bias_can = b.take(32 * 4);
+    W.tmp = b.take((size_t)H * H * 4);
+    W.partial = b.take((size_t)torso_dilate_ema_blocks(H) * 8);
+    W.thresh = b.take(4);
+    W.total = b.end;
     return W;
 }
 
@@ -1462,14 +1442,13 @@ size_t gfpp_torso_query_workspace_bytes(void) { return torso_query_work_bytes();
 
 int gfpp_torso_query(const gfpp_model *model, const float *xy, uint32_t n, const float *pose6, const float *code, float *alpha,
                      float *color, float *deform, void *workspace, size_t workspace_bytes, void *stream) {
-    if (!model || !xy || !pose6 || !alpha || !workspace) return fail(GFPP_ERR_INVALID, "torso_query: null pointer%s");
+    if (!model || !xy || !pose6 || !alpha || !workspace) return fail(GFPP_ERR_INVALID, "torso_query: null pointer");
     ModelHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "torso_query: model handle not initialised by gfpp_model_pack%s");
-    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "torso_query: the model was packed without a torso (has_torso = 0)%s");
-    if ((code == nullptr) != (m.torso_code_dim == 0)) return fail(GFPP_ERR_INVALID, "torso_query: code must be given iff torso_code_dim > 0%s");
-    if (n >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_query: n must be < 2^31%s");
-    if (workspace_bytes < torso_query_work_bytes()) return fail(GFPP_ERR_WORKSPACE, "torso_query: workspace too small%s");
+    if (const int rc = unpack("torso_query", model, m); rc != GFPP_OK) return rc;
+    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "torso_query: the model was packed without a torso (has_torso = 0)");
+    if ((code == nullptr) != (m.torso_code_dim == 0)) return fail(GFPP_ERR_INVALID, "torso_query: code must be given iff torso_code_dim > 0");
+    if (n >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_query: n must be < 2^31");
+    if (workspace_bytes < torso_query_work_bytes()) return fail(GFPP_ERR_WORKSPACE, "torso_query: workspace too small");
     const TorsoGridWork W = torso_grid_work_layout(2);   // only its bias block is used
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
@@ -1487,17 +1466,16 @@ int gfpp_torso_grid_update(const gfpp_model *model, const float *pose6, const fl
                            float *density_grid_torso, float *mean_out, float *tmp_grid, void *workspace, size_t workspace_bytes,
                            void *stream) {
     if (!model || !pose6 || !noise || !density_grid_torso || !mean_out || !workspace)
-        return fail(GFPP_ERR_INVALID, "torso_grid_update: null pointer%s");
+        return fail(GFPP_ERR_INVALID, "torso_grid_update: null pointer");
     ModelHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "torso_grid_update: model handle not initialised by gfpp_model_pack%s");
-    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "torso_grid_update: the model was packed without a torso (has_torso = 0)%s");
+    if (const int rc = unpack("torso_grid_update", model, m); rc != GFPP_OK) return rc;
+    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "torso_grid_update: the model was packed without a torso (has_torso = 0)");
     if ((code == nullptr) != (m.torso_code_dim == 0))
-        return fail(GFPP_ERR_INVALID, "torso_grid_update: code must be given iff torso_code_dim > 0%s");
+        return fail(GFPP_ERR_INVALID, "torso_grid_update: code must be given iff torso_code_dim > 0");
     const uint32_t H = m.grid_size;
-    if (!torso_grid_ok(H)) return fail(GFPP_ERR_UNSUPPORTED, "torso_grid_update: grid_size must be in 2..4096%s");
+    if (!torso_grid_ok(H)) return fail(GFPP_ERR_UNSUPPORTED, "torso_grid_update: grid_size must be in 2..4096");
     const TorsoGridWork W = torso_grid_work_layout(H);
-    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "torso_grid_update: workspace too small%s");
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "torso_grid_update: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     g_launches = 0;
@@ -1509,16 +1487,15 @@ int gfpp_torso_sr_grid_update(const gfpp_torso_sr_model *model, const float *lm6
                               float *density_grid_torso, float *mean_out, float *tmp_grid, void *workspace, size_t workspace_bytes,
                               void *stream) {
     if (!model || !lm68 || !noise || !density_grid_torso || !mean_out || !workspace)
-        return fail(GFPP_ERR_INVALID, "torso_sr_grid_update: null pointer%s");
+        return fail(GFPP_ERR_INVALID, "torso_sr_grid_update: null pointer");
     TorsoSrHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kTorsoSrMagic) return fail(GFPP_ERR_INVALID, "torso_sr_grid_update: model handle not initialised by gfpp_torso_sr_pack%s");
+    if (const int rc = unpack("torso_sr_grid_update", model, m); rc != GFPP_OK) return rc;
     if ((code == nullptr) != (m.code_dim == 0))
-        return fail(GFPP_ERR_INVALID, "torso_sr_grid_update: code must be given iff torso_code_dim > 0%s");
+        return fail(GFPP_ERR_INVALID, "torso_sr_grid_update: code must be given iff torso_code_dim > 0");
     const uint32_t H = m.grid_size;
-    if (!torso_grid_ok(H)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_grid_update: grid_size must be in 2..4096%s");
+    if (!torso_grid_ok(H)) return fail(GFPP_ERR_UNSUPPORTED, "torso_sr_grid_update: grid_size must be in 2..4096");
     const TorsoGridWork W = torso_grid_work_layout(H);
-    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "torso_sr_grid_update: workspace too small%s");
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "torso_sr_grid_update: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     g_launches = 0;
@@ -1534,21 +1511,19 @@ int gfpp_torso_sr_grid_update(const gfpp_torso_sr_model *model, const float *lm6
 }
 
 int gfpp_model_set_torso_threshold(gfpp_model *model, float density_thresh_torso) {
-    if (!model) return fail(GFPP_ERR_INVALID, "model_set_torso_threshold: null pointer%s");
+    if (!model) return fail(GFPP_ERR_INVALID, "model_set_torso_threshold: null pointer");
     ModelHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "model_set_torso_threshold: model handle not initialised by gfpp_model_pack%s");
-    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "model_set_torso_threshold: the model was packed without a torso (has_torso = 0)%s");
+    if (const int rc = unpack("model_set_torso_threshold", model, m); rc != GFPP_OK) return rc;
+    if (!m.has_torso) return fail(GFPP_ERR_INVALID, "model_set_torso_threshold: the model was packed without a torso (has_torso = 0)");
     m.density_thresh_torso = density_thresh_torso;
     memcpy(model, &m, sizeof(m));
     return GFPP_OK;
 }
 
 int gfpp_torso_sr_set_threshold(gfpp_torso_sr_model *model, float density_thresh_torso) {
-    if (!model) return fail(GFPP_ERR_INVALID, "torso_sr_set_threshold: null pointer%s");
+    if (!model) return fail(GFPP_ERR_INVALID, "torso_sr_set_threshold: null pointer");
     TorsoSrHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kTorsoSrMagic) return fail(GFPP_ERR_INVALID, "torso_sr_set_threshold: model handle not initialised by gfpp_torso_sr_pack%s");
+    if (const int rc = unpack("torso_sr_set_threshold", model, m); rc != GFPP_OK) return rc;
     m.density_thresh_torso = density_thresh_torso;
     memcpy(model, &m, sizeof(m));
     return GFPP_OK;
@@ -1595,6 +1570,49 @@ static int field_setup(const char *who, const gfpp_model_desc *d, FieldArgs &a) 
     return GFPP_OK;
 }
 
+// The checks and FieldArgs of a forward (gfpp_field_forward, gfpp_field_tc_forward) but the workspace's layout; M = 0 returns GFPP_OK
+// before the per-call checks.
+static int field_forward_setup(const char *who, const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M,
+                               const float *cond_feat, float *sigma, float *color, float *ambient_pos, void *workspace,
+                               size_t workspace_bytes, size_t need, FieldArgs &a) {
+    const int rc = field_setup(who, desc, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xyzs || !dirs || !cond_feat || !sigma || !color || !ambient_pos || !workspace) return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
+    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "%s: M must be < 2^30", who);
+    if (const int rw = check_workspace(who, workspace, workspace_bytes, need); rw != GFPP_OK) return rw;
+    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    a.sigma = sigma; a.color = color; a.ambient = ambient_pos;
+    return GFPP_OK;
+}
+
+// The same for a backward (gfpp_field_backward, gfpp_field_tc_backward).
+static int field_backward_setup(const char *who, const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M,
+                                const float *cond_feat, const float *grad_sigma, const float *grad_color, const float *grad_ambient_pos,
+                                float *const grad_w[8], float *grad_cond, float *grad_code, float *grad_position_table,
+                                float *grad_ambient_table, void *workspace, size_t workspace_bytes, size_t need, FieldArgs &a) {
+    const int rc = field_setup(who, desc, a);
+    if (rc != GFPP_OK) return rc;
+    g_launches = 0;
+    if (M == 0) return GFPP_OK;
+    if (!xyzs || !dirs || !cond_feat || !grad_sigma || !grad_color || !grad_ambient_pos || !grad_w || !grad_cond || !grad_position_table ||
+        !grad_ambient_table || !workspace || (a.ind_dim > 0 && !grad_code))
+        return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
+    for (int i = 0; i < 8; ++i)
+        if (!grad_w[i]) return fail(GFPP_ERR_INVALID, "%s: null weight gradient", who);
+    if (((uintptr_t)grad_position_table & 7u) || ((uintptr_t)grad_ambient_table & 7u))
+        return fail(GFPP_ERR_INVALID, "%s: table gradients must be 8-byte aligned", who);
+    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "%s: M must be < 2^30", who);
+    if (const int rw = check_workspace(who, workspace, workspace_bytes, need); rw != GFPP_OK) return rw;
+    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    a.g_sigma = grad_sigma; a.g_color = grad_color; a.g_ambient = grad_ambient_pos;
+    a.g_pos_tab = (float2 *)grad_position_table; a.g_amb_tab = (float2 *)grad_ambient_table;
+    for (int i = 0; i < 8; ++i) a.g_w[i] = grad_w[i];
+    a.g_cond = grad_cond; a.g_code = grad_code;
+    return GFPP_OK;
+}
+
 size_t gfpp_field_backward_workspace_bytes(uint32_t M) {
     if (M >= (1u << 30)) return 0;
     return field_wt_bytes() + (size_t)field_ctas(M) * FieldPart::total * 4;
@@ -1603,17 +1621,10 @@ size_t gfpp_field_backward_workspace_bytes(uint32_t M) {
 int gfpp_field_forward(const gfpp_model_desc *desc, const float *xyzs, const float *dirs, uint32_t M, const float *cond_feat, float *sigma,
                        float *color, float *ambient_pos, void *workspace, size_t workspace_bytes, void *stream) {
     FieldArgs a;
-    const int rc = field_setup("field_forward", desc, a);
-    if (rc != GFPP_OK) return rc;
-    g_launches = 0;
-    if (M == 0) return GFPP_OK;
-    if (!xyzs || !dirs || !cond_feat || !sigma || !color || !ambient_pos || !workspace) return fail(GFPP_ERR_INVALID, "field_forward: null pointer%s");
-    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "field_forward: M must be < 2^30%s");
-    if (workspace_bytes < field_wt_bytes()) return fail(GFPP_ERR_WORKSPACE, "field_forward: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "field_forward: workspace must be 256-byte aligned%s");
-    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    const int rc = field_forward_setup("field_forward", desc, xyzs, dirs, M, cond_feat, sigma, color, ambient_pos, workspace, workspace_bytes,
+                                       field_wt_bytes(), a);
+    if (rc != GFPP_OK || M == 0) return rc;
     a.wt = (float *)workspace;
-    a.sigma = sigma; a.color = color; a.ambient = ambient_pos;
     cudaStream_t st = (cudaStream_t)stream;
     CK(launch_field_relayout(a, st));
     CK(launch_field_fwd(a, st));
@@ -1625,28 +1636,13 @@ int gfpp_field_backward(const gfpp_model_desc *desc, const float *xyzs, const fl
                         float *grad_code, float *grad_position_table, float *grad_ambient_table, void *workspace, size_t workspace_bytes,
                         void *stream) {
     FieldArgs a;
-    const int rc = field_setup("field_backward", desc, a);
-    if (rc != GFPP_OK) return rc;
-    g_launches = 0;
-    if (M == 0) return GFPP_OK;
-    if (!xyzs || !dirs || !cond_feat || !grad_sigma || !grad_color || !grad_ambient_pos || !grad_w || !grad_cond || !grad_position_table ||
-        !grad_ambient_table || !workspace || (a.ind_dim > 0 && !grad_code))
-        return fail(GFPP_ERR_INVALID, "field_backward: null pointer%s");
-    for (int i = 0; i < 8; ++i)
-        if (!grad_w[i]) return fail(GFPP_ERR_INVALID, "field_backward: null weight gradient%s");
-    if (((uintptr_t)grad_position_table & 7u) || ((uintptr_t)grad_ambient_table & 7u))
-        return fail(GFPP_ERR_INVALID, "field_backward: table gradients must be 8-byte aligned%s");
-    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "field_backward: M must be < 2^30%s");
-    if (workspace_bytes < gfpp_field_backward_workspace_bytes(M)) return fail(GFPP_ERR_WORKSPACE, "field_backward: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "field_backward: workspace must be 256-byte aligned%s");
-    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    const int rc = field_backward_setup("field_backward", desc, xyzs, dirs, M, cond_feat, grad_sigma, grad_color, grad_ambient_pos, grad_w,
+                                        grad_cond, grad_code, grad_position_table, grad_ambient_table, workspace, workspace_bytes,
+                                        gfpp_field_backward_workspace_bytes(M), a);
+    if (rc != GFPP_OK || M == 0) return rc;
     a.wt = (float *)workspace;
     a.part = (float *)((char *)workspace + field_wt_bytes());
     a.n_cta = field_ctas(M);
-    a.g_sigma = grad_sigma; a.g_color = grad_color; a.g_ambient = grad_ambient_pos;
-    a.g_pos_tab = (float2 *)grad_position_table; a.g_amb_tab = (float2 *)grad_ambient_table;
-    for (int i = 0; i < 8; ++i) a.g_w[i] = grad_w[i];
-    a.g_cond = grad_cond; a.g_code = grad_code;
     cudaStream_t st = (cudaStream_t)stream;
     CK(launch_field_relayout(a, st));
     CK(launch_field_bwd(a, st));
@@ -1722,8 +1718,7 @@ static int torso_field_relayout(const char *who, TorsoTrainArgs &a, const float 
                                 const float *deform, void *workspace, size_t workspace_bytes, cudaStream_t st) {
     if (!xy || !alpha || !color || !deform || !workspace) return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
     if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: M must be < 2^31", who);
-    if (workspace_bytes < torso_wt_bytes<SR>()) return fail(GFPP_ERR_WORKSPACE, "%s: workspace too small", who);
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
+    if (const int rc = check_workspace(who, workspace, workspace_bytes, torso_wt_bytes<SR>()); rc != GFPP_OK) return rc;
     a.wt = (float *)workspace;
     CK(launch_torso_field_relayout<SR>(a, st));
     return GFPP_OK;
@@ -1744,8 +1739,7 @@ static int torso_field_backward(const char *who, TorsoTrainArgs &a, const float 
         if (!grad_deform_w[i] || !grad_canon_w[i]) return fail(GFPP_ERR_INVALID, "%s: null weight gradient", who);
     if (((uintptr_t)grad_torso_table & 7u) != 0) return fail(GFPP_ERR_INVALID, "%s: the table gradient must be 8-byte aligned", who);
     if (M >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: M must be < 2^31", who);
-    if (workspace_bytes < torso_field_ws_bytes<SR>(M)) return fail(GFPP_ERR_WORKSPACE, "%s: workspace too small", who);
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "%s: workspace must be 256-byte aligned", who);
+    if (const int rc = check_workspace(who, workspace, workspace_bytes, torso_field_ws_bytes<SR>(M)); rc != GFPP_OK) return rc;
     a.M = M; a.xy = xy;
     a.wt = (float *)workspace;
     a.part = (float *)((char *)workspace + torso_wt_bytes<SR>());
@@ -1770,7 +1764,7 @@ int gfpp_torso_field_forward(const gfpp_model_desc *desc, const float *xy, uint3
     TorsoTrainArgs a;
     int rc = torso_field_setup("torso_field_forward", desc, code, a);
     if (rc != GFPP_OK) return rc;
-    if (!pose6) return fail(GFPP_ERR_INVALID, "torso_field_forward: null pose6%s");
+    if (!pose6) return fail(GFPP_ERR_INVALID, "torso_field_forward: null pose6");
     a.cond = pose6;
     g_launches = 0;
     if (M == 0) return GFPP_OK;
@@ -1799,7 +1793,7 @@ int gfpp_torso_field_backward(const gfpp_model_desc *desc, const float *xy, uint
     TorsoTrainArgs a;
     const int rc = torso_field_setup("torso_field_backward", desc, code, a);
     if (rc != GFPP_OK) return rc;
-    if (!pose6) return fail(GFPP_ERR_INVALID, "torso_field_backward: null pose6%s");
+    if (!pose6) return fail(GFPP_ERR_INVALID, "torso_field_backward: null pose6");
     a.cond = pose6;
     return torso_field_backward<false>("torso_field_backward", a, xy, M, grad_alpha, grad_color, grad_deform, grad_deform_w, grad_canon_w,
                                        grad_code, grad_torso_table, workspace, workspace_bytes, stream);
@@ -1845,10 +1839,10 @@ int gfpp_torso_sr_field_backward(const gfpp_torso_sr_desc *desc, const float *xy
     const int rc = torso_sr_field_setup("torso_sr_field_backward", desc, lm68, code, image, weights_sum, a);
     if (rc != GFPP_OK) return rc;
     if ((grad_ha_w == nullptr) != (a.head_aware == 0) || (grad_ha_b == nullptr) != (a.head_aware == 0))
-        return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: grad_ha_w / grad_ha_b must be given iff head_aware%s");
+        return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: grad_ha_w / grad_ha_b must be given iff head_aware");
     if (a.head_aware)
         for (int i = 0; i < 3; ++i) {
-            if (!grad_ha_w[i] || !grad_ha_b[i]) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: null head-aware gradient%s");
+            if (!grad_ha_w[i] || !grad_ha_b[i]) return fail(GFPP_ERR_INVALID, "torso_sr_field_backward: null head-aware gradient");
             a.g_ha_w[i] = grad_ha_w[i];
             a.g_ha_b[i] = grad_ha_b[i];
         }
@@ -1871,18 +1865,11 @@ int gfpp_field_tc_forward(const gfpp_model_desc *desc, const float *xyzs, const 
                           float *color, float *ambient_pos, void *workspace, size_t workspace_bytes, void *stream) {
     FieldTcArgs t;
     FieldArgs &a = t.f;
-    const int rc = field_setup("field_tc_forward", desc, a);
-    if (rc != GFPP_OK) return rc;
-    g_launches = 0;
-    if (M == 0) return GFPP_OK;
-    if (!xyzs || !dirs || !cond_feat || !sigma || !color || !ambient_pos || !workspace) return fail(GFPP_ERR_INVALID, "field_tc_forward: null pointer%s");
-    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "field_tc_forward: M must be < 2^30%s");
-    if (workspace_bytes < FieldTcImg::total) return fail(GFPP_ERR_WORKSPACE, "field_tc_forward: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "field_tc_forward: workspace must be 256-byte aligned%s");
-    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    const int rc = field_forward_setup("field_tc_forward", desc, xyzs, dirs, M, cond_feat, sigma, color, ambient_pos, workspace,
+                                       workspace_bytes, FieldTcImg::total, a);
+    if (rc != GFPP_OK || M == 0) return rc;
     t.img = (unsigned char *)workspace;
     a.wt = (float *)(t.img + FieldTcImg::bias);
-    a.sigma = sigma; a.color = color; a.ambient = ambient_pos;
     cudaStream_t st = (cudaStream_t)stream;
     CK(launch_field_tc_relayout(t, st));
     CK(launch_field_tc_fwd(t, st));
@@ -1895,29 +1882,14 @@ int gfpp_field_tc_backward(const gfpp_model_desc *desc, const float *xyzs, const
                            void *stream) {
     FieldTcArgs t;
     FieldArgs &a = t.f;
-    const int rc = field_setup("field_tc_backward", desc, a);
-    if (rc != GFPP_OK) return rc;
-    g_launches = 0;
-    if (M == 0) return GFPP_OK;
-    if (!xyzs || !dirs || !cond_feat || !grad_sigma || !grad_color || !grad_ambient_pos || !grad_w || !grad_cond || !grad_position_table ||
-        !grad_ambient_table || !workspace || (a.ind_dim > 0 && !grad_code))
-        return fail(GFPP_ERR_INVALID, "field_tc_backward: null pointer%s");
-    for (int i = 0; i < 8; ++i)
-        if (!grad_w[i]) return fail(GFPP_ERR_INVALID, "field_tc_backward: null weight gradient%s");
-    if (((uintptr_t)grad_position_table & 7u) || ((uintptr_t)grad_ambient_table & 7u))
-        return fail(GFPP_ERR_INVALID, "field_tc_backward: table gradients must be 8-byte aligned%s");
-    if (M >= (1u << 30)) return fail(GFPP_ERR_UNSUPPORTED, "field_tc_backward: M must be < 2^30%s");
-    if (workspace_bytes < gfpp_field_tc_workspace_bytes(M)) return fail(GFPP_ERR_WORKSPACE, "field_tc_backward: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "field_tc_backward: workspace must be 256-byte aligned%s");
-    a.M = M; a.xyzs = xyzs; a.dirs = dirs; a.cond = cond_feat;
+    const int rc = field_backward_setup("field_tc_backward", desc, xyzs, dirs, M, cond_feat, grad_sigma, grad_color, grad_ambient_pos, grad_w,
+                                        grad_cond, grad_code, grad_position_table, grad_ambient_table, workspace, workspace_bytes,
+                                        gfpp_field_tc_workspace_bytes(M), a);
+    if (rc != GFPP_OK || M == 0) return rc;
     t.img = (unsigned char *)workspace;
     a.wt = (float *)(t.img + FieldTcImg::bias);
     a.part = (float *)(t.img + FieldTcImg::total);
     a.n_cta = field_tc_ctas(M);
-    a.g_sigma = grad_sigma; a.g_color = grad_color; a.g_ambient = grad_ambient_pos;
-    a.g_pos_tab = (float2 *)grad_position_table; a.g_amb_tab = (float2 *)grad_ambient_table;
-    for (int i = 0; i < 8; ++i) a.g_w[i] = grad_w[i];
-    a.g_cond = grad_cond; a.g_code = grad_code;
     cudaStream_t st = (cudaStream_t)stream;
     CK(launch_field_tc_relayout(t, st));
     CK(launch_field_tc_bwd(t, st));
@@ -1932,19 +1904,18 @@ namespace {
 struct FrozenWork { size_t narrow, depth, rays_t, survivors, hits, zero_begin, hist, counters, zero_end, cond, total; };
 FrozenWork frozen_work_layout(uint32_t N, uint32_t max_steps) {
     FrozenWork W;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) / 256 * 256; return r; };
-    W.narrow = take(8 * 128 * 4);          // the packed narrow rows with this call's individual code folded into row 7
-    W.depth = take((size_t)N * 4);
-    W.rays_t = take((size_t)N * 4);
-    W.survivors = take((size_t)N * 4);
-    W.hits = take((size_t)N * 64);         // HitRecord (head_common.cuh)
-    W.zero_begin = o;
-    W.hist = take((size_t)(max_steps + 2) * 4);
-    W.counters = take(16 * 4);
-    W.zero_end = o;
-    W.cond = take(64 * 2 * 2);             // fp16 hi + lo images of cond_feat (v2 head kernel)
-    W.total = o;
+    Bump b;
+    W.narrow = b.take(8 * 128 * 4);          // the packed narrow rows with this call's individual code folded into row 7
+    W.depth = b.take((size_t)N * 4);
+    W.rays_t = b.take((size_t)N * 4);
+    W.survivors = b.take((size_t)N * 4);
+    W.hits = b.take((size_t)N * 64);         // HitRecord (head_common.cuh)
+    W.zero_begin = b.end;
+    W.hist = b.take((size_t)(max_steps + 2) * 4);
+    W.counters = b.take(16 * 4);
+    W.zero_end = b.end;
+    W.cond = b.take(64 * 2 * 2);             // fp16 hi + lo images of cond_feat (v2 head kernel)
+    W.total = b.end;
     return W;
 }
 }  // namespace
@@ -1960,21 +1931,19 @@ int gfpp_frozen_head(const gfpp_model *model, const float *rays_o, const float *
                      const float *code, const float *noises, float dt_gamma, uint32_t max_steps, float T_thresh, float *weights_sum, float *image,
                      void *workspace, size_t workspace_bytes, void *stream) {
     if (!model || !rays_o || !rays_d || !aabb || !cond_feat || !weights_sum || !image || !workspace)
-        return fail(GFPP_ERR_INVALID, "frozen_head: null pointer%s");
+        return fail(GFPP_ERR_INVALID, "frozen_head: null pointer");
     ModelHost m;
-    memcpy(&m, model, sizeof(m));
-    if (m.magic != kMagic) return fail(GFPP_ERR_INVALID, "frozen_head: model handle not initialised by gfpp_model_pack%s");
-    if (N == 0) return fail(GFPP_ERR_INVALID, "frozen_head: no rays%s");
-    if (N >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "frozen_head: N must be < 2^31%s");
-    if (max_steps < 1 || max_steps > 4096) return fail(GFPP_ERR_UNSUPPORTED, "frozen_head: max_steps must be in 1..4096%s");
-    if ((m.ind_dim > 0) != (code != nullptr)) return fail(GFPP_ERR_INVALID, "frozen_head: code must be given iff the model has individual codes%s");
+    if (const int rc = unpack("frozen_head", model, m); rc != GFPP_OK) return rc;
+    if (N == 0) return fail(GFPP_ERR_INVALID, "frozen_head: no rays");
+    if (N >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "frozen_head: N must be < 2^31");
+    if (max_steps < 1 || max_steps > 4096) return fail(GFPP_ERR_UNSUPPORTED, "frozen_head: max_steps must be in 1..4096");
+    if ((m.ind_dim > 0) != (code != nullptr)) return fail(GFPP_ERR_INVALID, "frozen_head: code must be given iff the model has individual codes");
     for (int k = 0; k < 3; ++k)
-        if (!(aabb[k] <= aabb[3 + k])) return fail(GFPP_ERR_INVALID, "frozen_head: aabb must be (xmin, ymin, zmin, xmax, ymax, zmax)%s");
-    const bool use_v2 = m.v2_ok && (m.mlp_precision == 4 || (m.mlp_precision == 1 && getenv("GFPP_HEAD_V1") == nullptr));
-    if (m.mlp_precision == 4 && !use_v2) return fail(GFPP_ERR_UNSUPPORTED, "frozen_head: robust mode unavailable for this model%s");
+        if (!(aabb[k] <= aabb[3 + k])) return fail(GFPP_ERR_INVALID, "frozen_head: aabb must be (xmin, ymin, zmin, xmax, ymax, zmax)");
+    HeadKernel hk;
+    if (const int rc = choose_head_kernel("frozen_head", m, hk); rc != GFPP_OK) return rc;
     const FrozenWork W = frozen_work_layout(N, max_steps);
-    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "frozen_head: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "frozen_head: workspace must be 256-byte aligned%s");
+    if (const int rc = check_workspace("frozen_head", workspace, workspace_bytes, W.total); rc != GFPP_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     g_launches = 0;
@@ -1985,24 +1954,15 @@ int gfpp_frozen_head(const gfpp_model *model, const float *rays_o, const float *
     CKN(cudaMemcpyAsync(narrow, m.narrow, (code ? 7 : 8) * 128 * 4, cudaMemcpyDeviceToDevice, st));
     if (code) CK(launch_fold_bias(m.color0_src, 16 + 128 + m.ind_dim, 144, m.ind_dim, code, 128, narrow + 7 * 128, st));
 
-    HeadArgs a;
-    memset(&a, 0, sizeof(a));
-    a.pos_gm = m.pos_gm; a.amb_gm = m.amb_gm;
-    a.pos_tab = m.pos_tab; a.amb_tab = m.amb_tab;
-    a.pos_quads = m.pos_quads; a.amb_quads = m.amb_quads;
-    a.pos_octs = m.pos_octs; a.amb_octs = m.amb_octs;
-    a.wide = m.wide; a.narrow = narrow;
-    for (int c = 0; c < HEAD_NCHUNK; ++c) { a.chunk_off[c] = m.chunk_off[c]; a.chunk_k[c] = kChunkK[c]; }
+    HeadArgs a = head_field_args(m);
+    a.narrow = narrow;
     march_const_init(a.mc, m.bound, dt_gamma, max_steps, m.cascade, m.grid_size, m.bitfield);
     a.occ_bounds = m.occ_bounds;
     a.coarse_bits = m.coarse_bits;
     a.coarse_words = m.coarse_words;
     memcpy(a.aabb, aabb, sizeof(a.aabb));
     a.min_near = m.min_near; a.density_scale = m.density_scale;
-    // the occupied-box shortcut assumes no sample position is clamped to the cube: it holds for this call's aabb only if it lies inside
-    const float cube = m.bound;
-    a.use_occ_box = (m.cascade == 1 && aabb[0] >= -cube && aabb[1] >= -cube && aabb[2] >= -cube && aabb[3] <= cube && aabb[4] <= cube &&
-                     aabb[5] <= cube) ? 1 : 0;
+    a.use_occ_box = occ_box_ok(aabb, m.bound, m.cascade);
     a.n_frames = 1; a.n_rays = (int)N;
     a.rays_o = rays_o; a.rays_d = rays_d;
     a.cond_feat = cond_feat;
@@ -2023,16 +1983,9 @@ int gfpp_frozen_head(const gfpp_model *model, const float *rays_o, const float *
     // pass 1 only: a ray that reaches max_steps samples is final (march_rays_train gives it no more), so there is no schedule,
     // no pass 2 and no epilogue
     CK(launch_ray_setup(a, st));
-    if (m.mlp_precision == 0) CK(launch_head(a, -1, st, true));
-    else if (use_v2) {
-        HeadV2Args v2;
-        v2.w_stream = m.v2_stream; v2.w_res = m.v2_res; v2.pos_step = m.v2_pos_step;
-        v2.cond_hi = (const unsigned char *)(ws + W.cond);
-        v2.cond_lo = v2.cond_hi + 128;
-        CK(launch_cond_images(cond_feat, 1, ws + W.cond, ws + W.cond + 128, st));
-        CK(launch_head_v2(a, v2, m.mlp_precision, st, true));
-    } else CK(launch_head_tc(a, m.tc, m.mlp_precision, -1, st, true));
-    return GFPP_OK;
+    const HeadV2Args v2 = head_v2_args(m, ws + W.cond, 1);
+    if (hk == HEAD_V2) CK(launch_cond_images(cond_feat, 1, ws + W.cond, ws + W.cond + 128, st));
+    return launch_head_pass(hk, m, a, v2, st, true);
 }
 
 }  // extern "C"
@@ -2048,15 +2001,14 @@ size_t gfpp_torso_pass_workspace_bytes(uint32_t N) {
 int gfpp_torso_mask(const float *density_grid_torso, uint32_t G, float thr, const float *bg_coords, uint32_t N, const float *image,
                     const float *weights_sum, int32_t *idx, int32_t *slot, float *xy, float *image_m, float *weights_sum_m, int32_t *count,
                     void *workspace, size_t workspace_bytes, void *stream) {
-    if (!density_grid_torso || !bg_coords || !idx || !slot || !xy || !count || !workspace) return fail(GFPP_ERR_INVALID, "torso_mask: null pointer%s");
+    if (!density_grid_torso || !bg_coords || !idx || !slot || !xy || !count || !workspace) return fail(GFPP_ERR_INVALID, "torso_mask: null pointer");
     if ((image == nullptr) != (weights_sum == nullptr) || (image == nullptr) != (image_m == nullptr) || (image == nullptr) != (weights_sum_m == nullptr))
-        return fail(GFPP_ERR_INVALID, "torso_mask: image, weights_sum and their gathers must all be given or all be NULL%s");
-    if (N == 0) return fail(GFPP_ERR_INVALID, "torso_mask: no pixels%s");
-    if (N >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_mask: N must be < 2^31%s");
-    if (G < 2 || G > 4096) return fail(GFPP_ERR_UNSUPPORTED, "torso_mask: grid_size must be in 2..4096%s");
-    if ((((uintptr_t)bg_coords | (uintptr_t)xy) & 7u) != 0) return fail(GFPP_ERR_INVALID, "torso_mask: bg_coords and xy must be 8-byte aligned%s");
-    if (workspace_bytes < gfpp_torso_pass_workspace_bytes(N)) return fail(GFPP_ERR_WORKSPACE, "torso_mask: workspace too small%s");
-    if (((uintptr_t)workspace & 255u) != 0) return fail(GFPP_ERR_INVALID, "torso_mask: workspace must be 256-byte aligned%s");
+        return fail(GFPP_ERR_INVALID, "torso_mask: image, weights_sum and their gathers must all be given or all be NULL");
+    if (N == 0) return fail(GFPP_ERR_INVALID, "torso_mask: no pixels");
+    if (N >= (1u << 31)) return fail(GFPP_ERR_UNSUPPORTED, "torso_mask: N must be < 2^31");
+    if (G < 2 || G > 4096) return fail(GFPP_ERR_UNSUPPORTED, "torso_mask: grid_size must be in 2..4096");
+    if ((((uintptr_t)bg_coords | (uintptr_t)xy) & 7u) != 0) return fail(GFPP_ERR_INVALID, "torso_mask: bg_coords and xy must be 8-byte aligned");
+    if (const int rc = check_workspace("torso_mask", workspace, workspace_bytes, gfpp_torso_pass_workspace_bytes(N)); rc != GFPP_OK) return rc;
     g_launches = 0;
     CK(launch_torso_mask(density_grid_torso, G, thr, bg_coords, image, weights_sum, N, idx, slot, xy, image_m, weights_sum_m, count,
                          (int *)workspace, (cudaStream_t)stream));
@@ -2080,7 +2032,7 @@ static int torso_composite_check(const char *who, uint32_t N, uint32_t M, const 
 int gfpp_torso_composite_forward(const int32_t *slot, uint32_t N, uint32_t M, const float *alpha, const float *color, const float *image,
                                  const float *weights_sum, const float *bg_color, uint32_t bg_mode, float *torso_alpha_map,
                                  float *torso_rgb_map, float *rgb_map, void *stream) {
-    if (!slot || !torso_alpha_map || !torso_rgb_map || !rgb_map) return fail(GFPP_ERR_INVALID, "torso_composite_forward: null pointer%s");
+    if (!slot || !torso_alpha_map || !torso_rgb_map || !rgb_map) return fail(GFPP_ERR_INVALID, "torso_composite_forward: null pointer");
     const int rc = torso_composite_check("torso_composite_forward", N, M, alpha, color, image, weights_sum, bg_color, bg_mode);
     if (rc != GFPP_OK) return rc;
     g_launches = 0;
@@ -2095,7 +2047,7 @@ int gfpp_torso_composite_backward(const int32_t *idx, uint32_t N, uint32_t M, co
                                   void *stream) {
     const int rc = torso_composite_check("torso_composite_backward", N, M, alpha, color, image, weights_sum, bg_color, bg_mode);
     if (rc != GFPP_OK) return rc;
-    if (M > 0 && (!idx || !grad_alpha || !grad_color)) return fail(GFPP_ERR_INVALID, "torso_composite_backward: null pointer%s");
+    if (M > 0 && (!idx || !grad_alpha || !grad_color)) return fail(GFPP_ERR_INVALID, "torso_composite_backward: null pointer");
     g_launches = 0;
     if (M == 0) return GFPP_OK;
     CK(launch_torso_composite_bwd(idx, M, alpha, color, image, weights_sum, bg_color, bg_mode, grad_torso_alpha_map, grad_torso_rgb_map,
@@ -2109,10 +2061,10 @@ int gfpp_torso_composite_backward(const int32_t *idx, uint32_t N, uint32_t M, co
 extern "C" {
 
 int gfpp_rgb_u8_to_i420(const uint8_t *rgb, uint32_t F, uint32_t H, uint32_t W, uint8_t *out, void *stream) {
-    if (!rgb || !out) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: null pointer%s");
-    if (F == 0) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: no frames%s");
-    if (H == 0 || W == 0 || (H | W) & 1u) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: H and W must be even and non-zero (4:2:0 subsampling)%s");
-    if ((uint64_t)H * W > SIZE_MAX / 3 / F) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: F*H*W*3 bytes overflow size_t%s");
+    if (!rgb || !out) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: null pointer");
+    if (F == 0) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: no frames");
+    if (H == 0 || W == 0 || (H | W) & 1u) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: H and W must be even and non-zero (4:2:0 subsampling)");
+    if ((uint64_t)H * W > SIZE_MAX / 3 / F) return fail(GFPP_ERR_INVALID, "rgb_u8_to_i420: F*H*W*3 bytes overflow size_t");
     g_launches = 0;
     CK(launch_rgb_u8_to_i420(rgb, F, H, W, out, (cudaStream_t)stream));
     return GFPP_OK;

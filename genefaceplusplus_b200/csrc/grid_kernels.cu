@@ -4,6 +4,7 @@
 // torso_grid_kernel.cu).  Everything is stream-ordered and deterministic: fixed work per block, fixed reduction trees, no atomics.
 #include "common.cuh"
 #include "launch.cuh"
+#include "ops.cuh"
 
 namespace gfpp {
 

@@ -7,6 +7,7 @@
 // sized in multiples of the SM count.
 #include "common.cuh"
 #include "launch.cuh"
+#include "ops.cuh"
 
 namespace gfpp {
 

@@ -1,5 +1,6 @@
 // tc_pack.cu -- weight repacking for the wgmma path + a one-tile GEMM self-test of the wgmma plumbing.
 #include "launch.cuh"
+#include "ops.cuh"
 #include "tc.cuh"
 
 namespace gfpp {

@@ -12,6 +12,7 @@
 // The kernels take plain arrays only (no model descriptor): one set serves both torso models.
 #include "common.cuh"
 #include "launch.cuh"
+#include "ops.cuh"
 #include "torso_common.cuh"
 
 namespace gfpp {

@@ -19,6 +19,7 @@
 // Marching reuses the bit-exact device marcher of the inference path (common.cuh).
 #include "common.cuh"
 #include "launch.cuh"
+#include "ops.cuh"
 
 namespace gfpp {
 

@@ -8,6 +8,7 @@
 //   * BX = 2 (bytes): any even W and any alignment.
 // Integer arithmetic only (BT.601 limited range, gfpp.h (N)), so every byte is reproducible on the host.
 #include "launch.cuh"
+#include "ops.cuh"
 
 namespace gfpp {
 
