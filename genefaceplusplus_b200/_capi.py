@@ -67,6 +67,11 @@ class SrModel(ctypes.Structure):
     _fields_ = [("opaque", ctypes.c_uint64 * 32)]
 
 
+class SrGrad(ctypes.Structure):
+    _fields_ = [("conv_in_w", c_void_p), ("conv0_w", c_void_p), ("up_w", c_void_p), ("conv1_w", c_void_p),
+                ("bias", c_void_p * 4), ("noise_strength", c_void_p), ("rgb_w", c_void_p * 2), ("rgb_b", c_void_p * 2)]
+
+
 class TorsoSrDesc(ctypes.Structure):
     _fields_ = [("torso_grid", GridDesc), ("torso_deform_w", c_void_p * 3), ("torso_canon_w", c_void_p * 3), ("torso_code", c_void_p),
                 ("torso_code_dim", c_u32), ("head_aware", c_int), ("ha_w", c_void_p * 3), ("ha_b", c_void_p * 3),
@@ -109,6 +114,7 @@ EXPORTS = [
     "gfpp_grid_encode_forward_half", "gfpp_grid_encode_backward_half",
     "gfpp_torso_pass_workspace_bytes", "gfpp_torso_mask", "gfpp_torso_composite_forward", "gfpp_torso_composite_backward",
     "gfpp_rgb_u8_to_i420",
+    "gfpp_sr_train_workspace_bytes", "gfpp_sr_backward_workspace_bytes", "gfpp_sr_forward_train", "gfpp_sr_backward",
 ]
 
 
@@ -149,6 +155,14 @@ def lib():
                                       c_int, c_void_p, c_size_t, c_void_p]
         L.gfpp_sr_forward_video.argtypes = [ctypes.POINTER(SrModel), c_u32, c_u32, c_void_p, ctypes.POINTER(c_void_p * 4), c_u32,
                                             c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
+        L.gfpp_sr_train_workspace_bytes.restype = c_size_t
+        L.gfpp_sr_train_workspace_bytes.argtypes = [c_u32, c_u32]
+        L.gfpp_sr_backward_workspace_bytes.restype = c_size_t
+        L.gfpp_sr_backward_workspace_bytes.argtypes = [c_u32, c_u32]
+        L.gfpp_sr_forward_train.argtypes = [ctypes.POINTER(SrModel), c_u32, c_u32, c_void_p, ctypes.POINTER(c_void_p * 4), c_u32,
+                                            c_void_p, c_void_p, c_size_t, c_void_p]
+        L.gfpp_sr_backward.argtypes = [ctypes.POINTER(SrModel), c_u32, c_u32, c_void_p, c_void_p, c_size_t, ctypes.POINTER(c_void_p * 4),
+                                       c_u32, c_void_p, c_void_p, ctypes.POINTER(SrGrad), c_void_p, c_size_t, c_void_p]
         L.gfpp_torso_sr_packed_bytes.restype = c_size_t
         L.gfpp_torso_sr_packed_bytes.argtypes = []
         L.gfpp_torso_sr_pack.argtypes = [ctypes.POINTER(TorsoSrDesc), c_void_p, c_size_t, ctypes.POINTER(TorsoSrModel), c_void_p]

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libgfpp.so")
-SOURCES = ["capi.cu", "ops_kernels.cu", "head_kernel.cu", "torso_kernel.cu", "tc_pack.cu", "head_tc_kernel.cu", "head_v2_kernel.cu", "sr_kernel.cu", "torso_sr_kernel.cu", "train_kernels.cu", "grid_kernels.cu", "torso_grid_kernel.cu", "field_train_kernel.cu", "field_train_tc_kernel.cu", "torso_train_kernel.cu", "torso_sr_points_kernel.cu", "grid_half_kernels.cu", "torso_pass_kernels.cu", "video_kernels.cu"]
+SOURCES = ["capi.cu", "ops_kernels.cu", "head_kernel.cu", "torso_kernel.cu", "tc_pack.cu", "head_tc_kernel.cu", "head_v2_kernel.cu", "sr_kernel.cu", "sr_train_kernel.cu", "torso_sr_kernel.cu", "train_kernels.cu", "grid_kernels.cu", "torso_grid_kernel.cu", "field_train_kernel.cu", "field_train_tc_kernel.cu", "torso_train_kernel.cu", "torso_sr_points_kernel.cu", "grid_half_kernels.cu", "torso_pass_kernels.cu", "video_kernels.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]

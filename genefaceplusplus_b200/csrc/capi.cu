@@ -16,6 +16,7 @@
 #include "launch.cuh"
 #include "ops.cuh"
 #include "sr_kernel.cuh"
+#include "sr_train_kernel.cuh"
 #include "torso_grid_kernel.cuh"
 #include "torso_kernel.cuh"
 #include "torso_sr_kernel.cuh"
@@ -787,8 +788,9 @@ SrPacked sr_packed_layout() {
     L.total = b.end;
     return L;
 }
-struct SrWork { size_t x0a, x0b, img0, x1a, total; };
-SrWork sr_work_layout(uint32_t F, uint32_t R) {
+// `train`: gfpp_sr_forward_train's layout, which also keeps block1.conv1's activation x1b for the backward
+struct SrWork { size_t x0a, x0b, img0, x1a, x1b, total; };
+SrWork sr_work_layout(uint32_t F, uint32_t R, bool train = false) {
     SrWork W;
     Bump b;
     const size_t px = (size_t)F * R * R;
@@ -796,6 +798,30 @@ SrWork sr_work_layout(uint32_t F, uint32_t R) {
     W.x0b = b.take(px * 128 * 2);
     W.img0 = b.take(px * 3 * 4);
     W.x1a = b.take(px * 4 * 64 * 2);
+    W.x1b = train ? b.take(px * 4 * 64 * 2) : 0;
+    W.total = b.end;
+    return W;
+}
+// gfpp_sr_backward's workspace: the dgrad weight images, the fp32 gradients of the layers' pre-activations, g_img0 / g_r0 and
+// the partials of every reduction (slice counts fixed by sr_train_kernel.cuh, independent of the device)
+struct SrBwdWork { size_t wt[3], g1, gup, g0, gin, gimg0, gr0, pw[3], pin, prgb[2], pchan[4], total; };
+constexpr int kSrChanC[4] = {128, 128, 64, 64};
+SrBwdWork sr_bwd_layout(uint32_t F, uint32_t R) {
+    SrBwdWork W;
+    Bump b;
+    const size_t px = (size_t)F * R * R;
+    for (int m = 0; m < 3; ++m) W.wt[m] = b.take(sr_dgrad_weight_bytes(m), 1024);
+    W.g1 = b.take(px * 4 * 64 * 4);
+    W.gup = b.take(px * 4 * 64 * 4);
+    W.g0 = b.take(px * 128 * 4);
+    W.gin = b.take(px * 128 * 4);
+    W.gimg0 = b.take(px * 3 * 4);
+    W.gr0 = b.take(px * 3 * 4);
+    for (int m = 0; m < 3; ++m) W.pw[m] = b.take((size_t)sr_wgrad_slices(m) * sr_wgrad_m(m) * 9 * sr_wgrad_ci(m) * 4);
+    W.pin = b.take((size_t)SR_SIMT_SLICES * 27 * 128 * 4);
+    W.prgb[0] = b.take((size_t)SR_SIMT_SLICES * (3 * 128 + 3) * 4);
+    W.prgb[1] = b.take((size_t)SR_SIMT_SLICES * (3 * 64 + 3) * 4);
+    for (int i = 0; i < 4; ++i) W.pchan[i] = b.take((size_t)SR_SIMT_SLICES * (kSrChanC[i] + 1) * 4);
     W.total = b.end;
     return W;
 }
@@ -852,16 +878,17 @@ size_t gfpp_sr_workspace_bytes(uint32_t n_frames, uint32_t in_res) { return sr_w
 }  // extern "C"
 
 // gfpp_sr_forward (out, clamp01) and gfpp_sr_forward_video (out and/or out_u8, always clamped): `who` names the entry point in errors
+// gfpp_sr_forward_train (train: keep x1b in the workspace) shares it too
 static int sr_forward_impl(const char *who, const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in,
                            const float *const noise[4], uint32_t noise_per_frame, float *out, uint8_t *out_u8, int clamp01, void *workspace,
-                           size_t workspace_bytes, void *stream) {
+                           size_t workspace_bytes, void *stream, bool train = false) {
     if (!model || !rgb_in || (!out && !out_u8) || !workspace) return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
     if (((uintptr_t)out_u8 & 3u) != 0) return fail(GFPP_ERR_INVALID, "%s: out_u8 must be 4-byte aligned", who);
     SrHost m;
     if (const int rc = unpack(who, model, m); rc != GFPP_OK) return rc;
     if (n_frames == 0 || in_res == 0 || in_res % 128 != 0 || in_res > 1024) return fail(GFPP_ERR_UNSUPPORTED, "%s: in_res must be a multiple of 128 (256 in the reference)", who);
     if ((uint64_t)n_frames * in_res * in_res * 4 >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: too many frames per call", who);
-    const SrWork W = sr_work_layout(n_frames, in_res);
+    const SrWork W = sr_work_layout(n_frames, in_res, train);
     if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "%s: workspace too small", who);
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
@@ -888,6 +915,7 @@ static int sr_forward_impl(const char *who, const gfpp_sr_model *model, uint32_t
     a.noise = noise ? noise[3] : nullptr; a.noise_fstride = hi;
     a.rgb_w = m.rgb_w[1]; a.rgb_b = m.rgb_b[1]; a.img_in = (const float *)(ws + W.img0); a.img_out = out; a.clamp01 = clamp01;
     a.img_u8 = out_u8;
+    if (train) a.out = (__half *)(ws + W.x1b);
     CK(launch_sr_conv(2, a, st));
     return GFPP_OK;
 }
@@ -905,6 +933,99 @@ int gfpp_sr_forward_video(const gfpp_sr_model *model, uint32_t n_frames, uint32_
                           uint32_t noise_per_frame, float *out, uint8_t *out_u8, void *workspace, size_t workspace_bytes, void *stream) {
     return sr_forward_impl("sr_forward_video", model, n_frames, in_res, rgb_in, noise, noise_per_frame, out, out_u8, 1, workspace,
                            workspace_bytes, stream);
+}
+
+// ------------------------------------------------------------------ (O) gradients of the SR head (sr_train_kernel.cu)
+size_t gfpp_sr_train_workspace_bytes(uint32_t n_frames, uint32_t in_res) { return sr_work_layout(n_frames, in_res, true).total; }
+size_t gfpp_sr_backward_workspace_bytes(uint32_t n_frames, uint32_t in_res) { return sr_bwd_layout(n_frames, in_res).total; }
+
+int gfpp_sr_forward_train(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in, const float *const noise[4],
+                          uint32_t noise_per_frame, float *out, void *saved, size_t saved_bytes, void *stream) {
+    if (!out) return fail(GFPP_ERR_INVALID, "sr_forward_train: null pointer");
+    // the frames its backward takes (fp32 gradients of the 2R grid's 64 channels)
+    if ((uint64_t)n_frames * in_res * in_res * 4 * 64 >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "sr_forward_train: too many frames per call");
+    return sr_forward_impl("sr_forward_train", model, n_frames, in_res, rgb_in, noise, noise_per_frame, out, nullptr, 0, saved, saved_bytes,
+                           stream, true);
+}
+
+int gfpp_sr_backward(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in, const void *saved,
+                     size_t saved_bytes, const float *const noise_raw[4], uint32_t noise_per_frame, const float *grad_out, float *grad_in,
+                     const gfpp_sr_grad *grad, void *workspace, size_t workspace_bytes, void *stream) {
+    const char *who = "sr_backward";
+    if (!model || !rgb_in || !saved || !grad_out || !workspace) return fail(GFPP_ERR_INVALID, "%s: null pointer", who);
+    if (!grad_in && !grad) return fail(GFPP_ERR_INVALID, "%s: neither grad_in nor grad requested", who);
+    if (grad) {
+        if (!grad->conv_in_w || !grad->conv0_w || !grad->up_w || !grad->conv1_w || !grad->noise_strength)
+            return fail(GFPP_ERR_INVALID, "%s: null gradient pointer", who);
+        for (int i = 0; i < 4; ++i) if (!grad->bias[i]) return fail(GFPP_ERR_INVALID, "%s: null gradient pointer", who);
+        for (int i = 0; i < 2; ++i) if (!grad->rgb_w[i] || !grad->rgb_b[i]) return fail(GFPP_ERR_INVALID, "%s: null gradient pointer", who);
+    }
+    if (n_frames == 0 || in_res == 0 || in_res % 128 != 0 || in_res > 1024) return fail(GFPP_ERR_UNSUPPORTED, "%s: in_res must be a multiple of 128 (256 in the reference)", who);
+    if ((uint64_t)n_frames * in_res * in_res * 4 * 64 >= (1ull << 31)) return fail(GFPP_ERR_UNSUPPORTED, "%s: too many frames per call", who);
+    const SrWork S = sr_work_layout(n_frames, in_res, true);
+    if (saved_bytes < S.total) return fail(GFPP_ERR_WORKSPACE, "%s: saved buffer smaller than gfpp_sr_train_workspace_bytes", who);
+    const SrBwdWork W = sr_bwd_layout(n_frames, in_res);
+    if (workspace_bytes < W.total) return fail(GFPP_ERR_WORKSPACE, "%s: workspace too small", who);
+    if (((uintptr_t)workspace & 255u) != 0 || ((uintptr_t)saved & 255u) != 0) return fail(GFPP_ERR_INVALID, "%s: saved and workspace must be 256-byte aligned", who);
+    SrHost m;
+    if (const int rc = unpack(who, model, m); rc != GFPP_OK) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const char *sv = (const char *)saved;
+    char *ws = (char *)workspace;
+    const int F = (int)n_frames, R = (int)in_res;
+    const __half *x0a = (const __half *)(sv + S.x0a), *x0b = (const __half *)(sv + S.x0b), *x1a = (const __half *)(sv + S.x1a),
+                 *x1b = (const __half *)(sv + S.x1b);
+    float *g1 = (float *)(ws + W.g1), *gup = (float *)(ws + W.gup), *g0 = (float *)(ws + W.g0), *gin = (float *)(ws + W.gin);
+    float *gimg0 = (float *)(ws + W.gimg0), *gr0 = (float *)(ws + W.gr0);
+    g_launches = 0;
+    unsigned char *wt[3];
+    for (int i = 0; i < 3; ++i) wt[i] = (unsigned char *)(ws + W.wt[i]);
+    CK(launch_sr_pack_dgrad(m.tiles, wt, st));
+    // toRGB stages, then dgrad from the output back to block0.conv1's pre-activation
+    CK(launch_sr_bwd_out(grad_out, x1b, m.rgb_w[1], m.rgb_b[1], F, 2 * R, g1, grad ? (float *)(ws + W.prgb[1]) : nullptr, st));
+    CK(launch_sr_bwd_img0(grad_out, x0b, m.rgb_w[0], m.rgb_b[0], F, R, gimg0, gr0, grad ? (float *)(ws + W.prgb[0]) : nullptr, st));
+    SrDgradArgs d;
+    memset(&d, 0, sizeof(d));
+    d.g = g1; d.F = F; d.H = 2 * R; d.W = 2 * R; d.wt = wt[0]; d.act = x1a; d.out = gup;
+    CK(launch_sr_dgrad(0, d, st));
+    memset(&d, 0, sizeof(d));
+    d.g = gup; d.F = F; d.H = R; d.W = R; d.wt = wt[1]; d.act = x0b; d.rgb_w = m.rgb_w[0]; d.g_rgb = gr0; d.out = g0;
+    CK(launch_sr_dgrad(1, d, st));
+    memset(&d, 0, sizeof(d));
+    d.g = g0; d.F = F; d.H = R; d.W = R; d.wt = wt[2]; d.act = x0a; d.out = gin;
+    CK(launch_sr_dgrad(2, d, st));
+    if (grad_in) CK(launch_sr_in_dgrad(gin, m.conv_in_w, gimg0, F, R, grad_in, st));
+    if (!grad) return GFPP_OK;
+    // weight gradients: per-CTA partials, then one fixed-order sum per tensor
+    const __half *wx[3] = {x1a, x0b, x0a};
+    const float *wg[3] = {g1, gup, g0};
+    float *wout[3] = {grad->conv1_w, grad->up_w, grad->conv0_w};
+    for (int mode = 0; mode < 3; ++mode) {
+        SrWgradArgs w;
+        w.g = wg[mode]; w.x = wx[mode]; w.F = F; w.H = mode == 0 ? 2 * R : R; w.W = w.H; w.slices = sr_wgrad_slices(mode);
+        w.partial = (float *)(ws + W.pw[mode]);
+        CK(launch_sr_wgrad(mode, w, st));
+        CK(launch_sr_sum_cols(w.partial, w.slices, sr_wgrad_m(mode) * 9 * sr_wgrad_ci(mode), 0, sr_wgrad_m(mode) * 9 * sr_wgrad_ci(mode), wout[mode], st));
+    }
+    CK(launch_sr_in_wgrad(gin, rgb_in, F, R, (float *)(ws + W.pin), st));
+    CK(launch_sr_sum_cols((float *)(ws + W.pin), SR_SIMT_SLICES, 27 * 128, 0, 27 * 128, grad->conv_in_w, st));
+    const float *cg[4] = {gin, g0, gup, g1};
+    for (int i = 0; i < 4; ++i) {
+        const long long P = (long long)R * R * (i < 2 ? 1 : 4);
+        const float *raw = noise_raw ? noise_raw[i] : nullptr;
+        float *part = (float *)(ws + W.pchan[i]);
+        CK(launch_sr_chan_sums(cg[i], kSrChanC[i], F, P, raw, noise_per_frame ? 1 : 0, part, st));
+        // [slices][C + 1]: the bias gradient is columns 0..C-1, the noise strength's column C
+        CK(launch_sr_sum_cols(part, SR_SIMT_SLICES, kSrChanC[i] + 1, 0, kSrChanC[i], grad->bias[i], st));
+        CK(launch_sr_sum_cols(part, SR_SIMT_SLICES, kSrChanC[i] + 1, kSrChanC[i], 1, grad->noise_strength + i, st));
+    }
+    for (int i = 0; i < 2; ++i) {
+        const int C = i == 0 ? 128 : 64;
+        float *part = (float *)(ws + W.prgb[i]);
+        CK(launch_sr_sum_cols(part, SR_SIMT_SLICES, 3 * C + 3, 0, 3 * C, grad->rgb_w[i], st));
+        CK(launch_sr_sum_cols(part, SR_SIMT_SLICES, 3 * C + 3, 3 * C, 3, grad->rgb_b[i], st));
+    }
+    return GFPP_OK;
 }
 
 }  // extern "C"

@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(NT, LAYER == 1 ? 1 : 2) k_sr_conv(const __grid
                 const float t0 = lrelu_clamp(d[0][i] + nz[h] + s.bias[col]), t1 = lrelu_clamp(d[0][i + 1] + nz[h] + s.bias[col + 1]);
 #pragma unroll
                 for (int o = 0; o < 3; ++o) dot[h][o] = fmaf(t1, s.rgbw[o * COUT + col + 1], fmaf(t0, s.rgbw[o * COUT + col], dot[h][o]));
-                if (LAYER == 0) {
+                if (LAYER == 0 || a.out) {   // LAYER 2 keeps its activation only for the backward (gfpp_sr_forward_train)
                     const size_t pix = ((size_t)f * a.H + y) * a.W + x0 + 64 * wg + frag_row(i, lane, wwarp);
                     *reinterpret_cast<uint32_t *>(a.out + pix * COUT + col) = pack2<false>(t0, t1);
                 }

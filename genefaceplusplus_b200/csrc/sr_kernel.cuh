@@ -17,7 +17,7 @@ struct SrConvArgs {
     const float *bias;         // [COUT]
     const float *noise;        // [H_out * W_out] (+ f * noise_fstride), already multiplied by noise_strength; or nullptr
     long long noise_fstride;   // 0: one plane for every frame (noise_mode 'const'); H_out*W_out: one per frame ('random')
-    __half *out;               // LAYER 0: [F,H,W,128]; LAYER 1: [F,2H,2W,64]; LAYER 2: unused
+    __half *out;               // LAYER 0: [F,H,W,128]; LAYER 1: [F,2H,2W,64]; LAYER 2: [F,H,W,64] for the backward, or nullptr
     const float *rgb_w;        // [3][COUT] effective toRGB weights (layers 0 and 2)
     const float *rgb_b;        // [3]
     const float *img_in;       // LAYER 0: the NeRF image [F,H,W,3]; LAYER 2: img0 [F,H/2,W/2,3]

@@ -25,6 +25,8 @@ Two implementations live behind `Superresolution.forward`:
     (the reference switches these blocks to fp16 on CUDA), toRGB and the skip path fp32.  `folded_weights()` is the host
     half of that path: it folds modulation, demodulation and -- for the up-sampling layer -- the transposed stride-2
     convolution together with its FIR filter into plain GEMM matrices.  A missing libgfpp raises (no silent eager path).
+    Under grad, when the input or a parameter requires it, the same kernels run through train_ops.sr_head, whose backward is
+    csrc/sr_train_kernel.cu (gfpp_sr_forward_train / gfpp_sr_backward).
   * `backend == "torch"` or CPU tensors: the plain fp32 convolutions below -- the math the goldens pin
     (tests/golden/sr_head.npz) and the checker of the native path (tests/test_gpu_sr_native.py).
 """
@@ -161,7 +163,6 @@ class Superresolution(nn.Module):
         self.register_buffer("resample_filter", _binomial_filter())
 
     # ------------------------------------------------------------------ host half of the native path
-    @torch.no_grad()
     def folded_weights(self, dtype=torch.float32):
         """The six layers as plain convolutions / GEMM matrices (fp32, or `dtype`, on the parameters' device), given the constant
         latent w = 1 (radnerf_sr.py:33-34); layouts as gfpp_sr_desc (include/gfpp.h) wants them:
@@ -175,6 +176,9 @@ class Superresolution(nn.Module):
                                 zero-extending x reproduces the padding of the reference's conv2d_resample exactly.
           conv1_w   [64,576]    block1.conv1, k = (ky*3+kx)*64 + ci
           bias[4], rgb_w[2] ([3,C]: toRGB weight * style / sqrt(C)), rgb_b[2]
+
+        Differentiable when called with grad enabled: the native backward's gradients w.r.t. these matrices reach the conv and
+        affine weights, the biases and the toRGB weights through autograd on this fold (train_ops.sr_head).
         """
         # computed on the host from CPU copies of the (small) parameters -- a few hundred tiny tensor ops that would otherwise be a
         # few hundred kernel launches per (re)pack -- and moved to the parameters' device at the end
@@ -182,8 +186,9 @@ class Superresolution(nn.Module):
         w = torch.ones(self.w_dim, dtype=dtype)
         b0, b1 = self.block0, self.block1
 
-        def c(t):
-            return t.detach().to(dtype).cpu()
+        def c(t):   # a tensor of its own, never the parameter itself (the model may move to another device afterwards)
+            t = t.to(dtype).cpu()
+            return t.clone() if torch.is_grad_enabled() else t.detach()
 
         def mod_w(layer):     # _ModConv.modulated_weight on the CPU copies
             s_ = torch.addmv(c(layer.affine.bias), c(layer.affine.weight) * layer.affine.weight_gain, w)
@@ -195,20 +200,15 @@ class Superresolution(nn.Module):
         f1 = c(b1.conv0.resample_filter).double().sum(dim=0)     # separable: rows of outer(f,f)/64 sum to f/8
         f1 = f1 / f1.sum() * 2.0                                 # [1,3,3,1]/8 * 2
         O, I = k10.shape[:2]
-        K = torch.zeros(2, 2, O, I, 3, 3, dtype=torch.float64)
+        # per axis, M[p, o, a] = sum of the filter taps f1[t] with t - 1 - a = 2o - p (o shifted to 0..2); the phase kernels are the
+        # separable product, one differentiable contraction (no in-place accumulation for autograd to replay)
+        M = torch.zeros(2, 3, 3, dtype=torch.float64)
         for p in range(2):
-            for ty in range(4):
-                for ay in range(3):
-                    if (p + ty - 1 - ay) % 2:
-                        continue
-                    oy = (p + ty - 1 - ay) // 2 + 1
-                    for q in range(2):
-                        for tx in range(4):
-                            for ax in range(3):
-                                if (q + tx - 1 - ax) % 2:
-                                    continue
-                                ox = (q + tx - 1 - ax) // 2 + 1
-                                K[p, q, :, :, oy, ox] += f1[ty] * f1[tx] * k10[:, :, ay, ax]
+            for t in range(4):
+                for a in range(3):
+                    if (p + t - 1 - a) % 2 == 0:
+                        M[p, (p + t - 1 - a) // 2 + 1, a] += f1[t]
+        K = torch.einsum("poa,qxb,ijab->pqijox", M, M, k10)          # [py, px, O, I, oy, ox]
 
         def rgb(t):
             s_ = torch.addmv(c(t.affine.bias), c(t.affine.weight) * t.affine.weight_gain, w) * t.weight_gain
@@ -239,7 +239,8 @@ class Superresolution(nn.Module):
         if st is None or st["key"] != key:
             dev = self.block0.conv0.weight.device
             L = _capi.lib()
-            fw = self.folded_weights()
+            with torch.no_grad():
+                fw = self.folded_weights()
             d = _capi.SrDesc()
             keep = []
             for name in ("conv_in_w", "conv0_w", "up_w", "conv1_w"):
@@ -332,7 +333,11 @@ class Superresolution(nn.Module):
 
     def forward(self, rgb, noise_mode="random"):
         if rgb.is_cuda and self.backend == "native" and rgb.shape[-2:] == (self.input_resolution, self.input_resolution):
-            return self.forward_native(rgb.float().permute(0, 2, 3, 1).reshape(rgb.shape[0], -1, 3), noise_mode=noise_mode)
+            x = rgb.float().permute(0, 2, 3, 1).reshape(rgb.shape[0], -1, 3)
+            if torch.is_grad_enabled() and (rgb.requires_grad or any(p.requires_grad for p in self.parameters())):
+                from . import train_ops
+                return train_ops.sr_head(self, x, noise_mode)
+            return self.forward_native(x, noise_mode=noise_mode)
         x = rgb.float()
         if x.shape[-1] < self.input_resolution:
             x = F.interpolate(x, size=(self.input_resolution, self.input_resolution), mode="bilinear", align_corners=False,

@@ -12,6 +12,8 @@ train_precision = "fp16" section J, csrc/field_train_tc_kernel.cu); RADNeRF.forw
 `torso_field` is RADNeRFTorso.forward_torso with its gradient (section H); forward_torso calls it in training mode.
 `torso_sr_field` is the same for RADNeRFTorsowithSR.forward_torso (section I).  Both run csrc/torso_train_kernel.cu, one source
 instantiated for each field.
+`sr_head` is Superresolution.forward with its gradient (section O, csrc/sr_train_kernel.cu); Superresolution.forward calls it under
+grad.
 
 fp32 only (the reference casts with custom_fwd(cast_inputs=float32) as well); CUDA tensors only -- there is no CPU path.
 Differences from the reference, both deliberate: march_rays_train lays the samples out in ray order (deterministic; the
@@ -544,6 +546,97 @@ class _torso_sr_field(Function):
 
 
 torso_sr_field = _torso_sr_field.apply
+
+
+# ------------------------------------------------------------------------------------------------ the SR head
+_SR_GRAD_SHAPES = ((27, 128), (128, 1152), (256, 1152), (64, 576), (128,), (128,), (64,), (64,), (3, 128), (3, 64), (3,), (3,))
+
+
+class _sr_head(Function):
+    """Superresolution.forward on libgfpp with its gradient (include/gfpp.h section O): rgb_flat [F, R*R, 3] -> [F, 3, 2R, 2R], not
+    clamped.  `tensors` are the folded matrices of Superresolution.folded_weights (conv_in_w, conv0_w, up_w, conv1_w, bias[4],
+    rgb_w[2], rgb_b[2]) followed by the four layers' noise_strength: autograd takes their gradients on to the checkpoint's
+    parameters through the fold.  The kernels read the packed copy of the same weights.  The raw noise planes of the forward
+    (noise_const, or the draws of 'random') are kept for the noise strengths' gradient."""
+
+    @staticmethod
+    def forward(ctx, sr, noise_mode, x, *tensors):
+        R = sr.input_resolution
+        x = _cuda_f32(x).reshape(-1, R * R, 3).contiguous()
+        F_, dev = x.shape[0], x.device
+        if F_ * R * R * 256 >= 2 ** 31:
+            raise ValueError(f"the SR head's backward takes at most {(2 ** 31 - 1) // (R * R * 256)} frames of {R}x{R} per call")
+        if noise_mode not in ("random", "const", "none"):
+            raise ValueError(f"noise_mode must be random / const / none, not {noise_mode!r}")
+        st = sr._native_state()
+        L = _capi.lib()
+        per_frame = noise_mode == "random"
+        planes, raws = [], []
+        arr, rarr = (ctypes.c_void_p * 4)(), (ctypes.c_void_p * 4)()
+        for i, lay in enumerate(sr._layers()):
+            raw = p = None
+            if noise_mode == "const":
+                raw = lay.noise_const.float().contiguous()
+                if st["strengths"][i] != 0.0:
+                    p = (lay.noise_const * lay.noise_strength).float().contiguous()
+            elif noise_mode == "random":
+                raw = torch.randn(F_, lay.resolution, lay.resolution, device=dev)
+                if st["strengths"][i] != 0.0:
+                    p = (raw * lay.noise_strength).float().contiguous()
+            planes.append(p)
+            raws.append(raw)
+            arr[i] = p.data_ptr() if p is not None else None
+            rarr[i] = raw.data_ptr() if raw is not None else None
+        out = torch.empty(F_, 3, 2 * R, 2 * R, device=dev, dtype=torch.float32)
+        saved = torch.empty(L.gfpp_sr_train_workspace_bytes(F_, R), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            _capi.check(L.gfpp_sr_forward_train(ctypes.byref(st["model"]), F_, R, x.data_ptr(), ctypes.byref(arr), 1 if per_frame else 0,
+                                                out.data_ptr(), saved.data_ptr(), saved.numel(), _capi.stream_ptr(dev)),
+                        "gfpp_sr_forward_train")
+        ctx.st, ctx.saved_buf, ctx.raws, ctx.rarr, ctx.per_frame, ctx.R = st, saved, raws, rarr, per_frame, R
+        ctx.save_for_backward(x)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        (x,) = ctx.saved_tensors
+        F_, dev, R = x.shape[0], x.device, ctx.R
+        need_in, need_w = ctx.needs_input_grad[2], any(ctx.needs_input_grad[3:])
+        if not (need_in or need_w):
+            return (None,) * (3 + 12 + 4)
+        L = _capi.lib()
+        g = _cuda_f32(g).contiguous()
+        grad_in = torch.empty_like(x) if need_in else None
+        grads, gd = None, None
+        if need_w:
+            sizes = [int(np.prod(s)) for s in _SR_GRAD_SHAPES] + [4]
+            flat = torch.empty(sum(sizes), device=dev, dtype=torch.float32)
+            parts = list(torch.split(flat, sizes))
+            grads = [t.view(s) for t, s in zip(parts[:12], _SR_GRAD_SHAPES)]
+            gd = _capi.SrGrad()
+            gd.conv_in_w, gd.conv0_w, gd.up_w, gd.conv1_w = (t.data_ptr() for t in grads[:4])
+            for i in range(4):
+                gd.bias[i] = grads[4 + i].data_ptr()
+            for i in range(2):
+                gd.rgb_w[i], gd.rgb_b[i] = grads[8 + i].data_ptr(), grads[10 + i].data_ptr()
+            gd.noise_strength = parts[12].data_ptr()
+            grads += [parts[12][i].reshape(()) for i in range(4)]
+        ws = torch.empty(L.gfpp_sr_backward_workspace_bytes(F_, R), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            _capi.check(L.gfpp_sr_backward(ctypes.byref(ctx.st["model"]), F_, R, x.data_ptr(), ctx.saved_buf.data_ptr(), ctx.saved_buf.numel(),
+                                           ctypes.byref(ctx.rarr), 1 if ctx.per_frame else 0, g.data_ptr(),
+                                           None if grad_in is None else grad_in.data_ptr(), None if gd is None else ctypes.byref(gd),
+                                           ws.data_ptr(), ws.numel(), _capi.stream_ptr(dev)), "gfpp_sr_backward")
+        return (None, None, grad_in, *(grads if grads is not None else [None] * 16))
+
+
+def sr_head(sr, x, noise_mode="random"):
+    """Superresolution.forward of `sr` on x = rgb_flat [F, R*R, 3] (R = 256) with gradients w.r.t. x and every SR parameter that
+    requires one (biases and filters of the buffers get none)."""
+    # the differentiable fold only when a parameter needs its gradient (the fold is host work); else the packed state's copy
+    fw = sr.folded_weights() if any(p.requires_grad for p in sr.parameters()) else sr._native_state()["fw"]
+    tensors = [fw["conv_in_w"], fw["conv0_w"], fw["up_w"], fw["conv1_w"], *fw["bias"], *fw["rgb_w"], *fw["rgb_b"]]
+    return _sr_head.apply(sr, noise_mode, x, *tensors, *[lay.noise_strength for lay in sr._layers()])
 
 
 # ------------------------------------------------------------------------------------------------ the torso pass of the torso steps

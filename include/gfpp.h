@@ -47,6 +47,8 @@
  *  (L) the grid encoder ops of (A) and (D) on half tables, as the reference runs them under autocast.
  *
  *  (M) the torso pass of the torso training steps: mask, compaction and composite between (K) and the fields of (H) / (I).
+ *
+ *  (O) the gradients of the SR head of (C): a training forward that keeps its activations and the backward on TF32 tensor cores.
  */
 #ifndef GFPP_H_
 #define GFPP_H_
@@ -714,6 +716,46 @@ GFPP_API int gfpp_torso_composite_backward(const int32_t *idx, uint32_t N, uint3
  * Validation (before any CUDA call): NULL pointers, F == 0, H or W zero or odd, or F*H*W*3 bytes beyond SIZE_MAX ->
  * GFPP_ERR_INVALID.  One launch, stream-ordered, no host sync, no allocation. */
 GFPP_API int gfpp_rgb_u8_to_i420(const uint8_t *rgb, uint32_t F, uint32_t H, uint32_t W, uint8_t *out, void *stream);
+
+/* ------------------------------------------------------------------ (O) gradients of the SR head
+ *
+ * The SR tasks' losses (sr_mse_loss and LPIPS on sr_net(rgb_map), tasks/radnerfs/radnerf_sr.py, radnerf_torso_sr.py) need the
+ * SR head's gradient w.r.t. its input image and w.r.t. its parameters.  The parameters enter as the folded matrices of
+ * gfpp_sr_desc; the caller carries their gradients on to the checkpoint's parameters through the fold.
+ *
+ * gfpp_sr_forward_train: the four launches of gfpp_sr_forward (same out, clamp01 = 0) that also keep the activations the
+ *   backward needs in `saved` (gfpp_sr_train_workspace_bytes(n_frames, in_res) bytes, 256-byte aligned); `saved` is also the
+ *   forward's workspace.
+ * gfpp_sr_backward: given grad_out [F, 3, 2*in_res, 2*in_res] (the gradient w.r.t. out), the same model, rgb_in and `saved` of
+ *   the training forward, and the RAW noise planes (not multiplied by noise_strength; the layout of gfpp_sr_forward's, NULL
+ *   entries / array: no noise term), writes
+ *     grad_in [F, in_res*in_res, 3]  w.r.t. rgb_in;  NULL: skipped (the input needs no gradient)
+ *     grad    w.r.t. the folded matrices, biases, toRGB weights and biases and the four noise strengths (sum over pixels and
+ *             channels of the layer's pre-activation gradient times the raw plane);  NULL: no weight gradient is computed
+ *   At least one of them must be given.  Gradients are fp32; the three tensor-core layers run dgrad and wgrad on TF32 wgmma with
+ *   fp32 accumulation (the gradient operand rounded to nearest tf32, the other operand fp16 values of the forward).  Reductions
+ *   are per-CTA partials over a fixed slicing summed in a fixed order: repeated calls are bit-identical.
+ *   workspace: gfpp_sr_backward_workspace_bytes(n_frames, in_res) bytes, 256-byte aligned.
+ * in_res a multiple of 128 up to 1024; no host sync, no allocation; gfpp_last_launch_count() gives the launches. */
+typedef struct {
+    float *conv_in_w;          /* [27][128] */
+    float *conv0_w;            /* [128][1152] */
+    float *up_w;               /* [256][1152] */
+    float *conv1_w;            /* [64][576] */
+    float *bias[4];            /* 128, 128, 64, 64 */
+    float *noise_strength;     /* [4] */
+    float *rgb_w[2];           /* [3][128], [3][64] */
+    float *rgb_b[2];           /* [3], [3] */
+} gfpp_sr_grad;
+
+GFPP_API size_t gfpp_sr_train_workspace_bytes(uint32_t n_frames, uint32_t in_res);
+GFPP_API size_t gfpp_sr_backward_workspace_bytes(uint32_t n_frames, uint32_t in_res);
+GFPP_API int gfpp_sr_forward_train(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in,
+                                   const float *const noise[4], uint32_t noise_per_frame, float *out, void *saved,
+                                   size_t saved_bytes, void *stream);
+GFPP_API int gfpp_sr_backward(const gfpp_sr_model *model, uint32_t n_frames, uint32_t in_res, const float *rgb_in, const void *saved,
+                              size_t saved_bytes, const float *const noise_raw[4], uint32_t noise_per_frame, const float *grad_out,
+                              float *grad_in, const gfpp_sr_grad *grad, void *workspace, size_t workspace_bytes, void *stream);
 
 #ifdef __cplusplus
 }
