@@ -554,12 +554,10 @@ int gfpp_model_pack(const gfpp_model_desc *d, void *packed, size_t packed_bytes,
         // the last two: sigma L2's geo rows folded into color L0's geo columns (one fp16 image in both modes, DESIGN §6)
         CK(launch_pack_fold_tile(d->color_w[0], col0_in, 16, d->sigma_w[2], vs + (size_t)ti * V2_TILE_BYTES, V2_TILE_BYTES, st));
         static_assert(V2_NTILE_X1 == 7 + 2 && V2_NTILE_ROBUST == 7 + 4 + 2, "v2 tile table");
-        for (int kt = 0; kt < 2; ++kt) {
-            CK(launch_pack_tc_tile(d->ambient_w[2], 128, 0, kt * 64, amb_dim, 64, 0, 0, 0, vr + V2_RES_AMBN_HI + kt * 2048,
-                                   robust ? vr + V2_RES_AMBN_LO + kt * 2048 : nullptr, st));
-            CK(launch_pack_tc_tile(d->sigma_w[2], 128, 0, kt * 64, 1, 64, 0, 0, 0, vr + V2_RES_SIGROW + kt * 2048, nullptr, st));
-            CK(launch_pack_tc_tile(d->color_w[1], 128, 0, kt * 64, 3, 64, 0, 0, 0, vr + V2_RES_COLN + kt * 2048, nullptr, st));
-        }
+        // the narrow layers as mma.sync B fragments (the kernel is only chosen for amb_dim == 3, v2_ok below)
+        CK(launch_pack_narrow_b(d->ambient_w[2], 128, amb_dim < 8 ? amb_dim : 8, vr + V2_RES_AMBN_HI, robust ? vr + V2_RES_AMBN_LO : nullptr, st));
+        CK(launch_pack_narrow_b(d->sigma_w[2], 128, 1, vr + V2_RES_SIGROW, nullptr, st));
+        CK(launch_pack_narrow_b(d->color_w[1], 128, 3, vr + V2_RES_COLN, nullptr, st));
         CK(launch_pack_tc_tile(d->color_w[0], col0_in, 0, 0, 128, 16, 0, 1, 0, vr + V2_RES_COLSH, nullptr, st));
         m.v2_stream = vs; m.v2_res = vr;
     }

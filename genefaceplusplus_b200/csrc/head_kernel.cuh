@@ -83,8 +83,13 @@ constexpr int V2_TILE_BYTES = 16384;            // one streamed weight tile: 128
 // 32-63) | amb1 a,b | sig0 | sig1 a,b | fold a,b (W_fold = color L0 geo columns x sigma L2 geo rows, K = 128 over sigma L1's output);
 // robust: every ambient tile is followed by its lo image.  Sigma L2 has no streamed tile: its sigma row is resident (V2_RES_SIGROW).
 constexpr int V2_NTILE_X1 = 9, V2_NTILE_ROBUST = 13;
-// Resident small tiles (loaded once per CTA): 16-row N tiles of the narrow layers, 2 KB per 64-wide K tile, and the K16 SH tile
-constexpr int V2_RES_AMBN_HI = 0, V2_RES_AMBN_LO = 4096, V2_RES_SIGROW = 8192, V2_RES_COLSH = 12288, V2_RES_COLN = 16384, V2_RES_BYTES = 20480;
+// Resident block (loaded once per CTA): the K16 SH tile of colour L0, then the narrow layers (K = 128, N <= 3, zero-padded to
+// n = 8) as per-lane B-fragment images of mma.sync m16n8k16 (V2_NARROW_BYTES each, see k_pack_narrow_b): ambient out hi and lo,
+// the sigma row of sigma L2, colour out
+constexpr int V2_NARROW_BYTES = 2048;
+constexpr int V2_RES_COLSH = 0, V2_RES_AMBN_HI = 4096, V2_RES_AMBN_LO = V2_RES_AMBN_HI + V2_NARROW_BYTES,
+              V2_RES_SIGROW = V2_RES_AMBN_LO + V2_NARROW_BYTES, V2_RES_COLN = V2_RES_SIGROW + V2_NARROW_BYTES,
+              V2_RES_BYTES = V2_RES_COLN + V2_NARROW_BYTES;
 struct HeadV2Args {
     const unsigned char *w_stream;   // V2_NTILE_* tiles of V2_TILE_BYTES back to back
     const unsigned char *w_res;      // V2_RES_BYTES

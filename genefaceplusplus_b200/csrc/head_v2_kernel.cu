@@ -11,8 +11,12 @@
 //     the other slots do their gathers and ray work;
 //   * the weight stream is SHARED: the loader warp copies each tile once (NSTAGE-deep ring) for all slots; a stage is refilled
 //     once every owner warp has arrived on `w_free`;
-//   * the 3-wide outputs and the sigma logit are N=16 MMAs against small RESIDENT tiles, handed to the row owners through a
-//     small buffer at the head of the slot's second operand tile (the sigma logit through a per-row buffer of its own);
+//   * the narrow layers (ambient out, colour out; K = 128, N = 3) run in the epilogue of the layer that feeds them: per warp,
+//     eight chained mma.sync m16n8k16 whose A fragments are that layer's accumulator registers after ReLU and fp16 rounding,
+//     against per-lane B-fragment images in the RESIDENT block -- no operand-tile store, no async proxy, no wgmma round trip.
+//     The sigma row of sigma L2 (N = 1) reads sigma L1's stored output back with ldmatrix while color L0's MMAs run.  Their
+//     columns go to the row owners through a small buffer at the head of the slot's second operand tile (ambient out) and a
+//     per-row buffer (sigma logit, colour out);
 //   * the CTA is whole warpgroups: NSLOT owner warpgroups and one producer warpgroup, whose registers (setmaxnreg) go to
 //     the owners;
 //   * fp16: the position-grid features of a row's NEXT sample are looked up by the slot's GATHER WARP (producer warp 1 + s) while
@@ -88,11 +92,11 @@ struct Misc {
     volatile int flag[2][16];            // per batch parity, per owner warp: "I have live rows"
 };
 
-// the sigma logits of a slot's rows, from the sigma row's MMA (issued with color L0) to the row owners (TM floats per slot): the
-// robust mode keeps them at the head of the slot's residual tile l (idle from ambient out to the next batch's operand rows), fp16
-// behind Misc
+// the sigma logits and color out of a slot's rows, from their mma.sync (under / in color L0) to the row owners, [4][TM] floats per
+// slot (sigma, r, g, b): the robust mode keeps them at the head of the slot's residual tile l (idle from ambient L1's MMA to the
+// next batch's operand rows), fp16 behind Misc
 template <bool ROBUST>
-constexpr size_t slogit_bytes() { return ROBUST ? 0 : (size_t)Cfg<ROBUST>::NSLOT * TM * sizeof(float); }
+constexpr size_t slogit_bytes() { return ROBUST ? 0 : (size_t)Cfg<ROBUST>::NSLOT * 4 * TM * sizeof(float); }
 // fp16: the gather warps' staging rows behind the sigma logits, [NSLOT][TM] x 64 bytes: 16 levels as packed fp16 pairs (level j
 // in 32-bit word j) or, from the owner's post to the gather warp's reply, the row's next grid coordinates in chunk 0
 template <bool ROBUST>
@@ -138,6 +142,17 @@ __device__ __forceinline__ void epilogue_half(const float (&d)[64], unsigned cha
     }
 }
 
+// The store of epilogue_half<.., .., false> from an image relu_pack made: the pairs of column blocks cb, cb + 1 are a[2cb .. 2cb + 3]
+__device__ __forceinline__ void store_half(const uint32_t (&a)[32], unsigned char *h, int half, int lane, int wwarp) {
+    const int m = lane >> 3, arow = 64 * half + 16 * wwarp + 8 * (m & 1) + (lane & 7);
+    const uint32_t h_u = smem_u32(h);
+#pragma unroll
+    for (int cb = 0; cb < 16; cb += 2) {
+        const int c = cb + (m >> 1);
+        stmatrix_x4(h_u + (uint32_t)(c >> 3) * V2_TILE_BYTES + sw128_off(arow, c & 7), a[2 * cb], a[2 * cb + 1], a[2 * cb + 2], a[2 * cb + 3]);
+    }
+}
+
 // per-thread register budget of the executing warpgroup (all four warps, converged)
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
@@ -150,20 +165,63 @@ __device__ __forceinline__ float2 unpack_h2(uint32_t h) { return __half22float2(
 // and the gather warp's) fall on distinct banks
 __device__ __forceinline__ uint32_t stage_off(int row, int c) { return (uint32_t)row * 64u + (uint32_t)((c ^ (row >> 1)) & 3) * 16u; }
 
-// N = 16 group over K = 128: operand tiles a | a + one tile against the two 2 KB halves of a resident tile at w
-__device__ __forceinline__ void mma16(float (&d)[8], uint32_t a, uint32_t w, uint32_t acc_first) {
-    wgmma_sw<16, false>(d, a, w, 4, acc_first);
-    wgmma_sw<16, false>(d, a + V2_TILE_BYTES, w + 2048, 4, 1u);
+// The fp16 operand image of a warp's rows of a 128-wide layer, from its accumulator fragment: (+bias) -> ReLU -> a[m] = the
+// rounded pair (d[2m], d[2m + 1]), exactly the values the epilogue stores; a[4kb .. 4kb + 3] is the mma.sync A fragment of
+// k-block kb.  LO: al[m] = the residual pair, x - rn16(x), as store_pair<false, true> writes it.
+template <bool BIAS, bool LO>
+__device__ __forceinline__ void relu_pack(const float (&d)[64], const float *bias, int lane, uint32_t (&a)[32], uint32_t (&al)[LO ? 32 : 1]) {
+#pragma unroll
+    for (int m = 0; m < 32; ++m) {
+        const int col = frag_col(2 * m, lane);
+        float x0 = d[2 * m], x1 = d[2 * m + 1];
+        if (BIAS) { x0 += bias[col]; x1 += bias[col + 1]; }
+        x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f);
+        a[m] = pack2<false>(x0, x1);
+        if constexpr (LO) al[m] = pack2<false>(x0 - round16<false>(x0), x1 - round16<false>(x1));
+    }
 }
 
-// Columns c0 .. c0+NC-1 of an N = 16 accumulator fragment -> out[c][row] (rows of this half), read back by the row owners
-template <int NC>
-__device__ __forceinline__ void put_cols(const float (&d)[8], float *out, int c0, int half, int lane, int wwarp) {
+// A narrow layer (K = 128, N <= 8) on one warp's 16 rows: c (+)= A[16 x 128] * B[128 x 8], eight mma.sync in k order, the A
+// fragments from relu_pack, B from the per-lane fragment image at `img` (k_pack_narrow_b): the sum order of the N = 16 wgmma
+// chain it replaces.  ACC = false starts from zero
+template <bool ACC>
+__device__ __forceinline__ void narrow_mma(float (&c)[4], const uint32_t (&a)[32], const unsigned char *img, int lane) {
+    if (!ACC) c[0] = c[1] = c[2] = c[3] = 0.f;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int col = frag_col(i, lane) - c0;
-        if (col >= 0 && col < NC) out[col * TM + 64 * half + frag_row(i, lane, wwarp)] = d[i];
+    for (int q = 0; q < 4; ++q) {
+        const uint4 b = *reinterpret_cast<const uint4 *>(img + q * 512 + lane * 16);
+        mma_m16n8k16(c, a[8 * q], a[8 * q + 1], a[8 * q + 2], a[8 * q + 3], b.x, b.y);
+        mma_m16n8k16(c, a[8 * q + 4], a[8 * q + 5], a[8 * q + 6], a[8 * q + 7], b.z, b.w);
     }
+}
+
+// The narrow layer of narrow_mma with A read back from the operand tiles h0|h1 that store_half wrote (rows of warp `wwarp`,
+// M-half `half`), one k-block at a time with ldmatrix: the same fp16 values, and no image held in registers
+__device__ __forceinline__ void narrow_mma_smem(float (&c)[4], const unsigned char *h, int half, const unsigned char *img, int lane, int wwarp) {
+    const int m = lane >> 3, arow = 64 * half + 16 * wwarp + 8 * (m & 1) + (lane & 7);
+    const uint32_t h_u = smem_u32(h);
+    c[0] = c[1] = c[2] = c[3] = 0.f;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const uint4 b = *reinterpret_cast<const uint4 *>(img + q * 512 + lane * 16);
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            const int ch = 4 * q + 2 * j + (m >> 1);   // 16-byte chunk of k-block 2q + j this lane addresses
+            uint32_t a0, a1, a2, a3;
+            ldmatrix_x4(h_u + (uint32_t)(ch >> 3) * V2_TILE_BYTES + sw128_off(arow, ch & 7), a0, a1, a2, a3);
+            mma_m16n8k16(c, a0, a1, a2, a3, j ? b.z : b.x, j ? b.w : b.y);
+        }
+    }
+}
+
+// Columns 0 .. NC-1 of a narrow product (m16n8 D fragment of warp `wwarp`, M-half `half`) -> out[c][row], read back by the row
+// owners: lane 4g + t holds rows g and g + 8 at columns 2t and 2t + 1
+template <int NC>
+__device__ __forceinline__ void put_cols(const float (&c)[4], float *out, int half, int lane, int wwarp) {
+    const int col = 2 * (lane & 3), row = 64 * half + 16 * wwarp + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+        if (col + j < NC) { out[(col + j) * TM + row] = c[j]; out[(col + j) * TM + row + 8] = c[2 + j]; }
 }
 
 // warp-level feed of hit-list / survivor-list indices: a chunk of 32 consecutive entries is claimed with ONE global atomic and

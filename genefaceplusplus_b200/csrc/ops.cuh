@@ -31,6 +31,7 @@ cudaError_t launch_pack_octs_i16(const GridMeta &gm, const float *table, void *o
 cudaError_t launch_pack_tc_tile(const float *W, int ld, int row0, int col0, int N, int kc, int dst_row0, int k16, int bf16,
                                 unsigned char *hi, unsigned char *lo, cudaStream_t st);
 cudaError_t launch_pack_fold_tile(const float *Wc, int ldc, int c0, const float *Ws, unsigned char *tiles, int tile_bytes, cudaStream_t st);
+cudaError_t launch_pack_narrow_b(const float *W, int ld, int N, unsigned char *hi, unsigned char *lo, cudaStream_t st);
 cudaError_t launch_tc_selftest(const float *A, int K, const unsigned char *wt_hi, const unsigned char *wt_lo, int N, int nt64,
                                int k16_tail, int precision, float *out, cudaStream_t st);
 

@@ -130,6 +130,17 @@ template <> __device__ __forceinline__ void wgmma<144, false>(float (&d)[72], ui
 template <> __device__ __forceinline__ void wgmma<144, true>(float (&d)[72], uint64_t da, uint64_t db, uint32_t acc) { GFPP_WGMMA_N144("bf16"); }
 #undef GFPP_WGMMA_N144
 #undef GFPP_ACC8
+// ---- warp-level mma.sync (one warp, operands in registers) ----
+// D[16 x 8] += A[16 x 16] * B[16 x 8], fp16 operands, fp32 accumulation.  Lane l = 4g + t holds A rows g (a0, a2) and g + 8
+// (a1, a3) at K columns 2t, 2t + 1 (a0, a1) and 2t + 8, 2t + 9 (a2, a3); B K rows 2t, 2t + 1 (b0) and 2t + 8, 2t + 9 (b1) of
+// column g; C/D rows g (c0, c1) and g + 8 (c2, c3) at columns 2t, 2t + 1.  The 16 columns 16kb .. 16kb + 15 of a warp's m64
+// accumulator fragment are this A fragment as they stand: a_j = the pair (d[8kb + 2j], d[8kb + 2j + 1]).
+__device__ __forceinline__ void mma_m16n8k16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
 // all k-steps of one SW128 K-tile (ksteps x 16 elements); `acc_first` = 0 starts a new accumulation
 template <int N, bool BF16>
 __device__ __forceinline__ void wgmma_sw(float (&d)[N / 2], uint32_t a, uint32_t w, int ksteps, uint32_t acc_first) {
@@ -189,6 +200,13 @@ __device__ __forceinline__ void store_pair(unsigned char *hi_tile, unsigned char
 // register j holds the pair at row l/4, columns 2*(l%4) .. +1 of matrix j -- the layout of an accumulator fragment's pairs
 __device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
     asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
+
+// the inverse of stmatrix_x4: register j of lane l <- the pair at row l/4, columns 2*(l%4) .. +1 of matrix j (lane l addresses row
+// l%8 of matrix l/8)
+__device__ __forceinline__ void ldmatrix_x4(uint32_t saddr, uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(saddr)
                  : "memory");
 }
 

@@ -55,6 +55,28 @@ cudaError_t launch_pack_fold_tile(const float *Wc, int ldc, int c0, const float 
     return cudaGetLastError();
 }
 
+// A narrow layer W[N][ld] (N <= 8 outputs, K = 128 inputs, fp32) as the B operand of eight chained mma.sync m16n8k16, one per
+// 16-wide k-block kb: lane l = 4n + t holds, for kb, the pair W[n][16kb + 2t .. +1] (b0) and W[n][16kb + 8 + 2t .. +1] (b1).
+// Fragment word w = 2kb + (b1 ? 1 : 0) of lane l sits at (w / 4) * 512 + 16 l + 4 (w % 4): one conflict-free 16-byte load per lane
+// gives two k-blocks.  Outputs n >= N are zero; every byte of the 2 KB image is written.  lo (when given) = rn16(W - rn16(W)).
+__global__ void k_pack_narrow_b(const float *__restrict__ W, int ld, int N, unsigned char *__restrict__ hi, unsigned char *__restrict__ lo) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;   // (n, k), n < 8, k < 128
+    if (i >= 8 * 128) return;
+    const int n = i >> 7, k = i & 127, kb = k >> 4, kk = k & 15;
+    const int lane = 4 * n + ((kk & 7) >> 1), w = 2 * kb + (kk >> 3);
+    const uint32_t off = (uint32_t)(w >> 2) * 512u + (uint32_t)lane * 16u + (uint32_t)(w & 3) * 4u + (uint32_t)(kk & 1) * 2u;
+    const float v = n < N ? W[(size_t)n * ld + k] : 0.f;
+    const __half h = __float2half_rn(v);
+    *reinterpret_cast<__half *>(hi + off) = h;
+    if (lo) *reinterpret_cast<__half *>(lo + off) = __float2half_rn(v - __half2float(h));
+}
+
+cudaError_t launch_pack_narrow_b(const float *W, int ld, int N, unsigned char *hi, unsigned char *lo, cudaStream_t st) {
+    if (N < 1 || N > 8) return cudaErrorInvalidValue;
+    k_pack_narrow_b<<<8 * 128 / 256, 256, 0, st>>>(W, ld, N, hi, lo);
+    return cudaGetLastError();
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Self-test: out[128][N] = A[128][K] * W[N][K]^T through exactly the tile layouts, descriptors, wgmma issue and accumulator
 // fragment layout the fused kernels use (warpgroup g computes rows 64g..64g+63).  K = 64*nt64 (+16 when k16_tail); the weight
