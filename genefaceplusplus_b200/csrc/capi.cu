@@ -212,7 +212,7 @@ PackedLayout packed_layout(uint32_t cascade = 8, uint32_t grid_size = 128, size_
 }
 
 struct WorkLayout {
-    size_t image, rays_t, wsum, depth, survivors, hits, zero_begin, hist, counters, B_total, valid, pcount, zero_end, bias_def,
+    size_t image, rays_t, wsum, depth, survivors, hits, hit_ts, zero_begin, hist, counters, B_total, valid, pcount, zero_end, bias_def,
         bias_can, bias_amb, total;
 };
 
@@ -226,6 +226,7 @@ WorkLayout work_layout(uint32_t F, uint32_t N, uint32_t max_steps) {
     W.depth = b.take(FN * 4);
     W.survivors = b.take(FN * 4);
     W.hits = b.take(FN * 64);   // HitRecord (head_common.cuh)
+    W.hit_ts = b.take(FN * HIT_TS * 4);   // pass-1 sample lists (k_march_list)
     W.zero_begin = b.end;
     W.hist = b.take((size_t)F * (max_steps + 2) * 4);
     W.counters = b.take(16 * 4);
@@ -280,6 +281,14 @@ HeadV2Args head_v2_args(const ModelHost &m, const char *cond_images, uint32_t n_
     v2.cond_hi = (const unsigned char *)cond_images;
     v2.cond_lo = v2.cond_hi + (size_t)n_frames * 128;
     return v2;
+}
+
+// pass 1 of gfpp_render_frames on k_head_v2 replays sample lists that k_march_list marches at full occupancy; GFPP_MARCH_LIST=0
+// keeps the march in the row owners (the launches of earlier versions) for A/B runs.  The render workspace always has room for
+// the lists; the frozen head's has none (its per-ray size is part of its ABI) and marches in the owners
+bool use_march_list(HeadKernel k) {
+    const char *e = getenv("GFPP_MARCH_LIST");
+    return k == HEAD_V2 && !(e && strcmp(e, "0") == 0);
 }
 
 // one head pass (a.pass) on the chosen kernel; train: pass 1 with composite_rays_train's termination (gfpp_frozen_head)
@@ -740,6 +749,10 @@ int gfpp_render_frames(const gfpp_model *model, const gfpp_frames *fr, const gfp
     CK(launch_ray_setup(a, st));
     HeadKernel hk;
     if (const int rc = choose_head_kernel("render_frames", m, hk); rc != GFPP_OK) return rc;
+    if (use_march_list(hk)) {
+        a.hit_ts = (float *)(ws + W.hit_ts);
+        CK(launch_march_list(a, st));
+    }
     const HeadV2Args v2 = head_v2_args(m, ws + W.bias_amb, fr->n_frames);
     if (hk == HEAD_V2) CK(launch_cond_images(fr->cond_feat, a.n_frames, ws + W.bias_amb, ws + W.bias_amb + (size_t)fr->n_frames * 128, st));
     if (g_profile) CKN(cudaEventRecord(g_ev[0], st));

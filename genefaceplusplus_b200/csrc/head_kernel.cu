@@ -579,6 +579,34 @@ __global__ void __launch_bounds__(256) k_ray_setup(const __grid_constant__ HeadA
     }
 }
 
+// Pass-1 sample lists (HeadArgs::hit_ts): one thread per hit record, at full occupancy for the same reason as k_ray_setup, marches
+// on from the first sample.  Every march step is a pure function of t, so k_head_v2's row owners rebuild each sample from its
+// pre-step t with sample_at, bit for bit, instead of marching on their own dependent bitfield reads at 12 warps per SM.
+__global__ void __launch_bounds__(256) k_march_list(const __grid_constant__ HeadArgs a) {
+    MarchConst mc = a.mc;
+    float occ_lo[3], occ_hi[3];
+    (void)setup_occupancy(a, mc, occ_lo, occ_hi);
+    mc.coarse = a.coarse_bits;
+    const int n = *a.n_hits, len = min(a.max_steps, HIT_TS) - 1;
+    for (int w = blockIdx.x * blockDim.x + threadIdx.x; w < n; w += gridDim.x * blockDim.x) {
+        HitRecord hr;
+        uint4 *q = reinterpret_cast<uint4 *>(&hr);
+        ldg256(a.hits + 4 * (size_t)w, q[0], q[1]);
+        ldg256(a.hits + 4 * (size_t)w + 2, q[2], q[3]);
+        RayGeom g;
+        ray_geom_init(g, hr.ox, hr.oy, hr.oz, hr.dx, hr.dy, hr.dz);
+        float *ts = a.hit_ts + (size_t)hr.gid * HIT_TS;
+        float t = hr.t;
+#pragma unroll 1
+        for (int k = 0; k < len; ++k) {
+            int budget = 1 << 30;
+            if (march_budget(mc, g, hr.far_m, t, budget) != 1) { ts[k] = HIT_TS_END; break; }
+            ts[k] = t;
+            t = __fadd_rn(t, step_len(mc, t));   // past the sample, as sample_at / march_next advance it
+        }
+    }
+}
+
 // Replays the reference's round schedule (renderer.py:354-384) on the death histogram of each frame:
 //   n_step_j = clamp(N // n_alive_j, 1, 8);  cum += n_step_j;  n_alive_{j+1} = #{D > cum};  until cum >= max_steps.
 __global__ void k_schedule(const int *__restrict__ hist, int n_frames, int n_rays, int max_steps, int *__restrict__ B_total) {
@@ -632,6 +660,13 @@ cudaError_t launch_head(const HeadArgs &a, int total_hint, cudaStream_t st, bool
 cudaError_t launch_ray_setup(const HeadArgs &a, cudaStream_t st) {
     const uint64_t total = (uint64_t)a.n_frames * a.n_rays;
     k_ray_setup<<<grid_for(total, 256), 256, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_march_list(const HeadArgs &a, cudaStream_t st) {
+    // the hit count is only known on the device: enough CTAs to fill every SM, grid-stride over the hits
+    const uint64_t total = (uint64_t)a.n_frames * a.n_rays, full = (uint64_t)sm_count() * 8 * 256;
+    k_march_list<<<grid_for(total < full ? total : full, 256), 256, 0, st>>>(a);
     return cudaGetLastError();
 }
 

@@ -52,7 +52,13 @@ struct HeadArgs {
     unsigned long long *phase_cycles;  // optional [32]: per-phase cycle totals of thread 0 of every CTA (diagnostics)
     // ---- appended last so the offsets above stay put ----
     const float *noises;            // [F,N] in [0,1): jittered ray starts (k_ray_setup), or nullptr = start at near
+    float *hit_ts;                  // [F*N][HIT_TS] pass-1 sample lists of the hit rays (k_march_list; read by k_head_v2), or nullptr
 };
+
+// k_march_list: per hit ray (indexed by ray id) the pre-step t of samples 2 .. HIT_TS (at most min(max_steps, HIT_TS) - 1 of them),
+// then HIT_TS_END if the march ran off the ray before the list was full.  64 bytes per ray; the last word is never written
+constexpr int HIT_TS = 16;
+#define HIT_TS_END (-INFINITY)
 
 // tensor-core variant: pre-swizzled 16-bit weight tiles (see pack_tc_weights in capi.cu)
 constexpr int HEAD_TC_NCHUNK = 12;
@@ -146,6 +152,7 @@ size_t head_smem_bytes();
 // train: pass 1 with composite_rays_train's termination (k_head<true>, k_head_tc<.., .., true>, k_head_v2_train; gfpp_frozen_head)
 cudaError_t launch_head(const HeadArgs &a, int total_hint, cudaStream_t st, bool train = false);
 cudaError_t launch_ray_setup(const HeadArgs &a, cudaStream_t st);
+cudaError_t launch_march_list(const HeadArgs &a, cudaStream_t st);
 cudaError_t launch_dump_rays(const HeadArgs &a, float *rays_o, float *rays_d, cudaStream_t st);
 cudaError_t launch_schedule(const int *hist, int n_frames, int n_rays, int max_steps, int *B_total, cudaStream_t st);
 

@@ -15,11 +15,11 @@ m.render_clip(poses, sc.intrinsics,512,512,**kw); torch.cuda.synchronize()
 _capi.lib().gfpp_profile_phases(None)
 v = buf.cpu().tolist(); nb = v[31]
 if not os.environ.get('GFPP_HEAD_V1') and prec in ('fp16', 'robust'):   # row-owner kernel: stamps of row 0 of slot 0 of every CTA
-    # PH(i) index -> phase of csrc/head_v2_kernel.cu (12 and 16-18 are not stamped; sigma L2's geo rows are folded into col L0).
+    # PH(i) index -> phase of csrc/head_v2_kernel.cu (16-18 are not stamped; sigma L2's geo rows are folded into col L0).
     # Ambient out and colour out run in the epilogues that feed them: 4 and 14 time their mma.sync and the owners' barrier; the
     # sigma row runs under colour L0's MMAs, inside 13. fp16 stamps 6 (its owners wait for the gather warp) and only the position
     # levels below GATHER_L0 as 8 / 10; robust stamps 8 and 10, not 6
-    names2 = {6: 'wait for staged position features', 0: 'operand rows (pos feats, cond, SH)', 1: 'fate + march + refill',
+    names2 = {6: 'wait for staged position features', 0: 'operand rows (pos feats, cond, SH)', 12: 'fate + march', 1: 'refill',
               2: 'MMA + epi amb L0', 3: 'MMA amb L1', 4: 'amb out (mma.sync) + hand-over', 5: 'tanh', 7: 'ambient gather',
               8: 'prefetch pos levels 0-7', 9: 'MMA + epi sig L0', 10: 'prefetch pos levels 8-15', 11: 'MMA + epi sig L1',
               13: 'MMA col L0 (+ sigma row under it)', 14: 'col out (mma.sync) + hand-over', 15: 'sigmoid',
